@@ -8,7 +8,7 @@
 Headline (configs[1]): one "step" = LoopClosure::icpAlignment (fast_lio_sam_qn/src/loop_closure.cpp:110-136: two index
 builds, two covariance passes, align, fitness) over 256 synthetic 100k x 100k pairs per rank, issued as 16 jobs of 16 pairs
 to the C ABI's batch driver (b200reg_batch_*, three engine contexts on C++ host threads).  The jobs rotate over 4 DISTINCT
-sub-batches (64 distinct pairs, 205 MB of raw points per rank -- more than the 126 MB L2), nothing is replaced or skipped.
+sub-batches (64 distinct pairs, 205 MB of raw points per rank -- more than the 50 MB L2), nothing is replaced or skipped.
 Prints ONE JSON line (rank 0):
 
   value    : pairs/s with the raw xyz already resident in HBM when the timed region starts
@@ -58,24 +58,23 @@ def parse():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--points", type=int, default=N_POINTS)
     ap.add_argument("--depth", type=int, default=int(os.environ.get("B200REG_PIPE_DEPTH", "3")),
-                    help="engine contexts of the batch driver.  Measured on this workload (value / e2e pairs/s, 20 steps): 2: 4420 / 3811; "
-                         "3: 4639 / 4145, 4641 / 4144, 4591 / 4107 (stable); 4: 3856 / 4290 (four contexts over four rotating sub-batches "
-                         "fall into lockstep); 5: 4653 / 4383, 4724 / 4372, but also 4066 / 4395 -- more contexts hide more of the uploads "
-                         "yet can phase-lock on the device-resident arm, so the default stays at the stable 3")
+                    help="engine contexts of the batch driver.  Measured on this workload on one H100 SXM at 700 W (value / e2e pairs/s, "
+                         "20 steps, one run each): 2: 2837 / 2543; 3: 2918 / 2653; 4: 2884 / 2729; 5: 2962 / 2797 -- beyond 3 the "
+                         "device-resident arm gains no more than the run-to-run spread")
     ap.add_argument("--depth-e2e", type=int, default=int(os.environ.get("B200REG_PIPE_DEPTH_E2E", "3")),
                     help="engine contexts of the batch driver of the from-host arm (default: the same driver as the device-resident arm). "
-                         "It has uploads to hide and rises steadily with the depth (3811 / 4145 / 4290 / 4383 pairs/s at 2 / 3 / 4 / 5; 4420-4434 "
-                         "measured at 5 over ~30 runs), but ONE of those runs ended in a CUDA 'illegal memory access' that could not be "
-                         "reproduced or explained (profiles/README.md), so the default stays with the configuration that has never failed")
+                         "It has uploads to hide and rises with the depth (see --depth)")
     ap.add_argument("--depth-lc", type=int, default=3,
                     help="engine contexts of the batch driver of the loop-closure secondaries (default: the headline's driver; the coarse "
-                         "stage has latency-bound kernels and gains from more contexts in flight -- 4613 / 4745 / 4810 / 4870 pairs/s on the "
-                         "voxelised workload at 3 / 5 / 6 / 8 -- but see --depth-e2e for why the defaults stay at 3)")
+                         "stage has latency-bound kernels and may gain from more contexts in flight)")
     ap.add_argument("--secondary", default="all", help="comma list of secondary workloads: voxel,raw,sequence,batch512 | all | none")
     ap.add_argument("--keyframes", type=int, default=2761, help="sequence workload: keyframes generated (KITTI 05: 2761)")
     ap.add_argument("--matching", default="optimized", choices=["optimized", "advanced"])
     ap.add_argument("--cpu-sample-pairs", type=int, default=6)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write the result records of the headline's last timed step (device-resident arm) "
+                         "as DIR/<field>.npy, one row per pair in submission order")
     return ap.parse_args()
 
 
@@ -103,7 +102,7 @@ def gen_pairs(seeds, n_points, mode="gicp", voxel=None, threads=None):
 def primary_seeds(rank=0):
     """SURVEY §8(d): config 2 uses seeds 1000...  Weak scaling fixes the per-GPU work, so EVERY rank registers the same pool
     of 64 pairs (each rank starts the rotation at its own sub-batch); synthetic pools differ in cost -- the pool 1064..1127
-    holds the 32-iteration seed 1104 and is 12 % heavier (profiles/r02/n2_diag.txt) -- and rank-distinct pools would measure
+    holds the 32-iteration seed 1104 and is heavier (profiles/n2_diag.py) -- and rank-distinct pools would measure
     that difference, not the system.  They are measured too: `secondary.rank_distinct_pools` (N>1)."""
     return [1000 + i for i in range(JOB_PAIRS * DISTINCT_JOBS)]
 
@@ -120,7 +119,7 @@ def primary_config(args):
             "points_per_cloud": args.points, "pairs_per_step_per_gpu": JOB_PAIRS * JOBS_PER_STEP,
             "distinct_pairs_per_gpu": JOB_PAIRS * DISTINCT_JOBS,
             "seeds": "1000 + i, i < 64, the same pool on every rank (no pair replaced or skipped); rank r starts its rotation at sub-batch r",
-            "l2": "the jobs of a step rotate over 4 distinct 16-pair sub-batches: %.0f MB of raw points per rank (> 126 MB L2); "
+            "l2": "the jobs of a step rotate over 4 distinct 16-pair sub-batches: %.0f MB of raw points per rank (> 50 MB L2); "
                   "every job rebuilds all derived data from the raw xyz" % (2 * JOB_PAIRS * DISTINCT_JOBS * args.points * 16 / 1e6)}
 
 
@@ -276,8 +275,8 @@ class ClockSampler:
 
 
 def ncu_traffic(kernel_family, workload):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed
-    `ncu --set full` capture (profiles/traffic.json, written by profiles/extract_traffic.py)."""
+    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from an
+    `ncu --set full` capture digested into profiles/traffic.json by profiles/extract_traffic.py, when one is present."""
     p = os.path.join(REPO, "profiles", "traffic.json")
     if not os.path.exists(p):
         return None
@@ -299,7 +298,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -471,6 +470,15 @@ def parity_vs_oracle(gpu_results, cpu_results, what, gpu_T=lambda r: np.array(r.
                 tolerance="%g rad / %g m" % (ROT_TOL, TRANS_TOL))
 
 
+def dump_outputs(directory, results):
+    """One .npy per field of the Result records (b200reg_result) a caller of the timed path receives: Tf in float32,
+    every other field (counters and flags included) in float64."""
+    os.makedirs(directory, exist_ok=True)
+    recs = [r.as_dict() for r in results]
+    for name in recs[0]:
+        np.save(os.path.join(directory, name + ".npy"), np.array([r[name] for r in recs], np.float32 if name == "Tf" else np.float64))
+
+
 def percentiles(x):
     x = np.asarray(x, np.float64)
     return dict(p50=float(np.percentile(x, 50)), p99=float(np.percentile(x, 99)), max=float(x.max()), n=int(len(x)))
@@ -570,6 +578,8 @@ def main():
     if batch_h is not batch:
         batch_h.close()
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0 and res_dev:
+        dump_outputs(args.dump_outputs, [r for job in res_dev[-JOBS_PER_STEP:] for r in job])
 
     # one result per distinct pair (jobs 0..3 of the device arm), bit-identical across repeats and arms
     first = {(j + rank) % DISTINCT_JOBS: j for j in reversed(range(DISTINCT_JOBS))}  # sub-batch -> first job that ran it

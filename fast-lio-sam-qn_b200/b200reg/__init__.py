@@ -1,4 +1,4 @@
-"""b200reg -- B200-native loop-closure registration engine (Nano-GICP + Quatro path of FAST-LIO-SAM-QN).
+"""b200reg -- H100-native loop-closure registration engine (Nano-GICP + Quatro path of FAST-LIO-SAM-QN).
 
 Python here is plumbing only (ctypes over the C ABI in include/b200reg.h, synthetic inputs,
 torch.distributed sharding); the product is csrc/*.cu.

@@ -1,4 +1,4 @@
-"""In-tree build of libb200reg.so (hand-written sm_100a CUDA behind the C ABI of include/b200reg.h)."""
+"""In-tree build of libb200reg.so (hand-written sm_90a CUDA behind the C ABI of include/b200reg.h)."""
 import os
 import subprocess
 from concurrent.futures import ThreadPoolExecutor
@@ -12,7 +12,7 @@ EXTRA = {"quatro.cu": ["-fmad=false"],    # fixed fp32 operation order for the F
 HEADERS = ["internal.cuh", "knn.cuh", "smallmath.cuh", "fpfh_basis.cuh", os.path.join(REPO, "include", "b200reg.h")]
 LIB = os.path.join(CSRC, "libb200reg.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-Xcompiler", "-fPIC",
+FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC",
          "-ccbin", "/usr/bin/g++"]
 
 
@@ -21,7 +21,7 @@ def _mtime(p):
 
 
 def build_native(force=False, verbose=False):
-    """Compile every .cu of the package for sm_100a and link libb200reg.so.  Returns the path."""
+    """Compile every .cu of the package for sm_90a and link libb200reg.so.  Returns the path."""
     deps = [os.path.join(CSRC, s) for s in SOURCES] + [h if os.path.isabs(h) else os.path.join(CSRC, h) for h in HEADERS]
     if not force and os.path.exists(LIB) and all(_mtime(d) <= _mtime(LIB) for d in deps):
         return LIB

@@ -1,6 +1,6 @@
 """ctypes binding of libb200reg.so -- the C ABI of include/b200reg.h.
 
-The product path: every call below lands in hand-written sm_100a kernels.  There is no CPU
+The product path: every call below lands in hand-written sm_90a kernels.  There is no CPU
 fallback; if the library or a GPU is missing these functions raise.
 """
 import ctypes as C

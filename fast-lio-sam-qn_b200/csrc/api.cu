@@ -68,7 +68,7 @@ struct b200reg_ctx {
   cudaStream_t copy_stream = nullptr;  // H2D uploads of later chunks overlap the compute of earlier ones
   cudaMemPool_t pool = nullptr;        // per-context pool: reuse never adds dependencies on another context's streams
   int pipeline_chunks = 4;
-  int sm_count = 148;
+  int sm_count = 132;
   // persistent arena of the batched LM solve: every kernel argument of the solve's CUDA graph points in here, so the graph is
   // instantiated once and re-launched by every b200reg_gicp_align call until a larger batch makes the arena grow
   struct LmArena {
@@ -236,7 +236,7 @@ static int lm_arena_ensure(b200reg_ctx* c, int count) {
   if (!a.graph.exec) {
     // persistent grids: as many blocks as can be resident (search: 16 per SM at 32 registers, accumulate: 8 per SM);
     // blocks beyond the current number of work items exit at once
-    const int bps = 32, bpa = 32;  // measured: 8 / 16 / 32 / 64 blocks per SM -> 1.83-1.92 ms per 16-pair solve, flat from 32 on
+    const int bps = 32, bpa = 32;  // 8 to 64 blocks per SM: the solve time is flat from 32 on
     const cudaError_t e = lm_graph_build(&a.graph, a.d_pairs, a.d_states, a.d_guess, a.d_call, a.d_sched, c->sm_count * bps, c->sm_count * bpa);
     if (e != cudaSuccess) return fail(B200REG_ECUDA, std::string("building the LM graph: ") + cudaGetErrorString(e));
   }
@@ -260,7 +260,7 @@ void b200reg_default_gicp_params(b200reg_gicp_params* p) {
 
 const char* b200reg_last_error(void) { return g_err.c_str(); }
 void b200reg_set_last_error(const char* message) { g_err = message ? message : ""; }
-const char* b200reg_version(void) { return "b200reg 0.2 (sm_100a)"; }
+const char* b200reg_version(void) { return "b200reg 0.2 (sm_90a)"; }
 size_t b200reg_struct_size(int which) {
   switch (which) {
     case 0: return sizeof(b200reg_gicp_params);
@@ -1517,7 +1517,7 @@ int b200reg_allgather_results(b200reg_ctx* c, const b200reg_result* local, int n
 // Keyframe clouds live in SLABS of their own (plain cudaMalloc, never the context's stream-ordered pool): a store only
 // grows, while every registration call takes and returns hundreds of MB of scratch from the pool; 480 KB keyframes carved
 // out of the pool's free scratch blocks between two calls fragmented it, and the pool then grew by a fresh block in almost
-// every call (tens of ms each: profiles/diag_sequence_e2e.py measured 5.4 -> 11 ... 37 ms per 16-attempt step).
+// every call (profiles/diag_sequence_e2e.py times the steps).
 struct KfSlab {
   float4* base = nullptr;
   size_t cap = 0, used = 0;  // points

@@ -3,7 +3,7 @@
 // over pairs (blockIdx.y = pair) and driven by a per-pair device-side state machine so that the
 // host never synchronises inside an LM iteration.
 //
-// Reference behaviour being replaced (paths relative to /root/reference):
+// Reference behaviour being replaced (paths relative to the reference tree's root):
 //   third_party/nano_gicp/include/nano_gicp/impl/nano_gicp_impl.hpp
 //       calculate_covariances :298-357, update_correspondences :173-211, linearize :213-270,
 //       compute_error :272-296
@@ -295,7 +295,7 @@ __global__ void __launch_bounds__(256) k_gicp_init(const PairDev* pairs, PairSta
 // K is the CAPACITY of the result set; k <= K neighbours enter the covariance (the k nearest of the K nearest are the
 // k nearest), so every k in 1..32 is served by the next instantiated capacity.
 // The result set is a max-heap in shared memory (KnnHeap, knn.cuh): the covariance needs the SET of neighbours, not their
-// order.  (Round 1 kept a sorted list in registers: 1.98 ms for 32 x 100k points against 1.58 ms, profiles/r02/README.md.)
+// order.  (A sorted list in registers, the earlier design, spent most of its instructions in the insertion chain.)
 template <int K>
 __global__ void __launch_bounds__(STEP_THREADS, (K <= 16 ? 10 : 4)) k_covariance(const CloudDev* clouds, int k, int method) {
   const CloudDev& c = clouds[blockIdx.y];

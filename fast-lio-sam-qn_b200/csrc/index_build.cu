@@ -2,7 +2,7 @@
 // third_party/nano_gicp/include/nano_gicp/impl/nanoflann_impl.hpp:1199-1211, 867-1012, which the
 // reference runs twice per pair plus PCL's hidden third FLANN build, SURVEY.md §3.4).
 //
-// B200-first design: instead of a serial top-down pointer tree, every cloud becomes a
+// GPU-first design: instead of a serial top-down pointer tree, every cloud becomes a
 // Morton-sorted point array with a linear BVH on top (Karras 2012 radix tree, built with one
 // thread per node, no recursion).  All clouds of a batch are built together: blockIdx.y is the
 // cloud.  Seven launches per batch (round 1 needed eighteen):

@@ -60,8 +60,8 @@ __device__ __forceinline__ int orig_index(const float4* __restrict__ pts, int po
 // Insert a candidate with cd <= worst.  Hot path: strict '<' chain of branch-free selects; the candidate lands
 // AFTER entries of equal distance.  Exact ties (measure ~0 on real data) are repaired by one unrolled upward bubble
 // pass in a cold branch -- written without taking the address of the arrays, so that the result set provably stays
-// in registers (an out-of-line repair taking pointers forced it into local memory: 22% of k_covariance's
-// instructions were LDL/STL).  A candidate that ties with the current worst replaces it only if its original
+// in registers (an out-of-line repair taking pointers forced it into local memory: LDL/STL
+// in the hot loop).  A candidate that ties with the current worst replaces it only if its original
 // index is lower (the (d2, index) rule of SURVEY.md App. A.3).
 template <int K>
 __device__ __forceinline__ void knn_insert(KnnSet<K>& s, float cd, int cp, const float4* __restrict__ pts) {
@@ -110,7 +110,7 @@ __device__ __forceinline__ void KnnSet<K>::offer(float cd, int cp, const float4*
 // occupies 2K registers.
 // The heap is ordered by DISTANCE ONLY: the hot sift-down is strict float compares and nothing else (the first version
 // carried the (d2, original index) rule through every compare and cost as much as the register insertion chain it
-// replaced: ncu, 43% of the kernel's warp instructions at 7-9 active lanes).  The tie rule matters in exactly one place --
+// replaced).  The tie rule matters in exactly one place --
 // a candidate at EXACTLY the current worst distance -- and is resolved there, cold: among the entries tied at that
 // distance the one with the highest original index is the true worst; the candidate overwrites it in place (same
 // distance: the heap stays a heap) iff its own index is lower.
@@ -408,7 +408,7 @@ __device__ __forceinline__ void radius_visit_warp(const CloudDev& c, bool active
 // The same warp-shared walk, with the hits of all 32 queries POOLED in one per-warp ring and processed 32 at a time by
 // whichever lane is free: f(owner_lane, position) runs for entry e on lane e.  For per-pair work whose result is
 // order-independent (integer histograms in shared memory) this keeps every lane busy -- with per-lane hit lists the
-// lockstep processing ran at 12.5 of 32 lanes (profiles/r02: the lanes of a warp fill at different rates).
+// lockstep processing leaves lanes idle (the lanes of a warp fill their lists at different rates).
 // on_hit(position) runs on the OWNER lane when the hit is found (cheap bookkeeping such as a neighbour count).
 // ring: RV_RING unsigned per warp.  Must be called by every thread of the warp; control flow is warp-uniform.
 constexpr int RV_RING = 64;

@@ -1,7 +1,7 @@
 // quatro.cu -- the Quatro half of the loop-closure path as batched GPU kernels (blockIdx.y = cloud / pair).
 // Compiled with -fmad=false: the fp32 feature arithmetic follows a fixed operation order (see the oracle).
 //
-// Reference behaviour being replaced (paths relative to /root/reference; PCL / FLANN / TEASER++ semantics per
+// Reference behaviour being replaced (paths relative to the reference tree's root; PCL / FLANN / TEASER++ semantics per
 // SURVEY.md App. B because those libraries are not vendored):
 //   Q1 k_normals        pcl::NormalEstimation, radius 0.9, viewpoint (0,0,0)       third_party/Quatro/src/fpfh.cc:27-32
 //   Q2 k_spfh           FPFHEstimationOMP::computePointSPFHSignature                fpfh.cc:35-39

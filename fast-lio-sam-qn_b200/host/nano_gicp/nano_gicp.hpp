@@ -3,7 +3,7 @@
 // Keeps the public surface of third_party/nano_gicp/include/nano_gicp/nano_gicp.hpp:58-137 and of the base classes
 // it exposes (LsqRegistration, lsq_registration.hpp:56-116; the pcl::Registration setters/getters used at
 // fast_lio_sam_qn/src/loop_closure.cpp:9-16,120-133), so LoopClosure links against this header unchanged.
-// Nothing is computed on the host: every call forwards to hand-written sm_100a kernels; without a GPU the process
+// Nothing is computed on the host: every call forwards to hand-written sm_90a kernels; without a GPU the process
 // aborts (b200reg_host::context()).
 //
 // Differences a maintainer should know (also in INTEGRATION.md):

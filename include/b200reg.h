@@ -1,4 +1,4 @@
-/* b200reg.h -- C ABI of the B200-native loop-closure registration engine.
+/* b200reg.h -- C ABI of the H100-native loop-closure registration engine.
  *
  * This is the drop-in boundary for the ONE hot path of engcang/FAST-LIO-SAM-QN that
  * this repository replaces: the registration that FastLioSamQn::loopTimerFunc
@@ -24,7 +24,7 @@
  *   - host buffers passed to a call (pinned or pageable) have been consumed when the call returns; device buffers passed
  *     with on_device != 0 must stay valid until the context's stream has been synchronised or the call has returned a result;
  *   - b200reg_ctx_set_stream may only be called while the context is idle (everything it owns is ordered on ONE stream);
- *   - there is NO CPU fallback: if no sm_100 device is present b200reg_ctx_create fails.
+ *   - there is NO CPU fallback: if no CUDA device is present b200reg_ctx_create fails.
  */
 #ifndef B200REG_H
 #define B200REG_H

@@ -2,7 +2,7 @@
 //
 // CPU restatement of the Nano-GICP half of the loop-closure hot path, written
 // from the reference's behaviour (NOT copied).  Every function cites the
-// reference lines it follows; paths are relative to /root/reference/.
+// reference lines it follows; paths are relative to the reference tree's root.
 //   NG  = third_party/nano_gicp/include/nano_gicp
 //   QN  = fast_lio_sam_qn
 //

@@ -6,7 +6,7 @@
 //   teaser::Matcher::normalizePoints      third_party/Quatro/src/matcher.cc:58-116
 //   teaser::Matcher::optimizedMatching    third_party/Quatro/src/matcher.cc:358-561
 //   teaser::RobustRegistrationSolver      TEASER++ (not vendored), QUATRO rotation + PMC_HEU clique
-// The PCL / FLANN / TEASER++ arithmetic is NOT under /root/reference; it is restated from their published
+// The PCL / FLANN / TEASER++ arithmetic is NOT in the reference tree; it is restated from their published
 // algorithms as summarised in SURVEY.md App. B.  "Parity unpinned": no reference output exists for any
 // of this (no tests, libraries not installable), and the reference stage is itself nondeterministic
 // (srand(time(NULL)) matcher.cc:465; unsynchronised TBB writes :424-431).  Deliberate, documented

@@ -1,7 +1,7 @@
 // oracle/ref_nanoflann_shim.cpp -- TEST INFRASTRUCTURE ONLY.
 //
 // Thin C wrapper that compiles the REFERENCE's own kd-tree
-//   /root/reference/third_party/nano_gicp/include/nano_gicp/impl/nanoflann_impl.hpp
+//   <reference>/third_party/nano_gicp/include/nano_gicp/impl/nanoflann_impl.hpp
 // (std-only header, nanoflann v1.3.2) from where it lies, configured exactly as
 // the reference configures it in nano_gicp/nanoflann.hpp:
 //   * metric SO3_Adaptor<float, Adaptor>, DIM 3, int index   (nanoflann.hpp:100-102)
@@ -9,7 +9,7 @@
 //   * KNNResultSet<float,int> + findNeighbors(SearchParams()) (nanoflann.hpp:148-150)
 // Output goes to oracle/_ref/libref_nanoflann.so (git-ignored, travels to the GPU
 // box).  No reference source is copied into this repository; only the include
-// path points at /root/reference.  Built by oracle/Makefile target `ref`.
+// path points at the reference tree (Makefile variable REF).  Built by oracle/Makefile target `ref`.
 #include <nano_gicp/impl/nanoflann_impl.hpp>
 
 #include <cstddef>

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Where the FPFH deviation between the CUDA path and the CPU oracle comes from (row a11; run on the GPU box):
-    python profiles/diag_fpfh.py > gpurun_out/diag_fpfh.txt
+    python profiles/diag_fpfh.py > out/diag_fpfh.txt
 Compares (1) normals, (2) FPFH of the complete pipelines, (3) FPFH with the GPU's own normals fed to the oracle
 (stage isolation: what remains is atan2f / summation order)."""
 import os

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Warp-instruction share per SOURCE line of a kernel in an .ncu-rep captured with --import-source on (-lineinfo build):
-    python profiles/ncu_hot_lines.py gpurun_out/r02_cov.ncu-rep k_covariance [top]"""
+    python profiles/ncu_hot_lines.py out/r02_cov.ncu-rep k_covariance [top]"""
 import csv
 import subprocess
 import sys

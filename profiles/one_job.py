@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """A few 16-pair icpAlignment jobs on ONE context (no pipelining): the unit the per-kernel profiles are taken on.
     python profiles/one_job.py [jobs] [pairs]          # prints the per-family CUDA-event times
-    ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv python profiles/one_job.py 3
+    ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file out/launches.csv python profiles/one_job.py 3
 """
 import os
 import sys

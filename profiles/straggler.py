@@ -2,7 +2,7 @@
 """Per-pair LM scheduling, measured: a 16-pair icpAlignment batch in which ONE pair runs all 32 outer iterations (synthetic
 seed 1104: GICP itself diverges on it, identically on the CPU oracle) against the same batch with a clean pair in its place.
 Round 1 kept launching the blocks of the 15 finished pairs until the last pair was done.
-    python profiles/straggler.py > gpurun_out/straggler.txt"""
+    python profiles/straggler.py > out/straggler.txt"""
 import os
 import sys
 import time

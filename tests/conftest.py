@@ -9,7 +9,7 @@ sys.path.insert(0, os.path.join(REPO, "fast-lio-sam-qn_b200"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")

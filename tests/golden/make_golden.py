@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Generates the committed golden fixtures.  Run in the BUILD container (needs /root/reference for
-oracle/_ref = the reference's own nanoflann kd-tree); the GPU box only reads the .npz files.
+"""Generates the committed golden fixtures.  Run where the reference source tree is available (needs
+oracle/_ref = the reference's own nanoflann kd-tree); the tests only read the .npz files.
 
   knn_ref_nanoflann.npz  exact k-NN answers of the REFERENCE kd-tree
                          (third_party/nano_gicp/include/nano_gicp/impl/nanoflann_impl.hpp, configured as in
@@ -10,9 +10,13 @@ oracle/_ref = the reference's own nanoflann kd-tree); the GPU box only reads the
   quatro_oracle_2k.npz   the CPU oracle's Quatro outputs on a 2000 x 2300 pair (normals / FPFH samples, both matchers'
                          correspondence lists, both solves) -- same purpose (`python make_golden.py quatro` writes
                          only this one)
+  ref_nanoflann_samples.npz  the REFERENCE kd-tree's k-NN answers on sampled rows of the query sets the oracle and the
+                         CUDA k-NN are checked against, and the oracle's align with that kd-tree behind it
+                         (`python make_golden.py ref` writes only this one)
 """
 import os
 import sys
+import zlib
 
 import numpy as np
 
@@ -41,10 +45,37 @@ def quatro_golden():
     print("quatro golden:", len(opt), "optimized /", len(adv), "advanced correspondences; cliques", len(so["clique"]), len(sa["clique"]))
 
 
+def ref_samples_golden():
+    """The reference kd-tree's answers on the query sets of tests/test_oracle.py and tests/test_gpu_gicp.py, on a fixed
+    seeded sample of rows; the CRC32 of each generated cloud pins the synthetic input."""
+    rng = np.random.default_rng(2024)
+    out = {}
+
+    def sets(tag, src, dst, specs):
+        out[tag + "_crc"] = np.array([zlib.crc32(src.tobytes()), zlib.crc32(dst.tobytes())], np.uint32)
+        ref = oracle.RefNanoflann(dst)
+        for name, (q, k) in specs.items():
+            rows = np.sort(rng.choice(len(q), min(len(q), 1024 if k == 1 else 128), replace=False)).astype(np.int32)
+            out["%s_rows_%s" % (tag, name)] = rows
+            out["%s_idx_%s" % (tag, name)], out["%s_d2_%s" % (tag, name)] = ref.knn(q[rows], k)
+
+    src, dst, _ = synth.make_pair(77, 6000, 7000)
+    sets("cpu", src, dst, {"a": (dst[:2000], 15), "b": (src, 1), "c": (src[:500] + np.float32(2.5), 15)})
+    assert oracle.use_ref_nanoflann(True) == 0
+    r = oracle.gicp_align(src, dst)
+    oracle.use_ref_nanoflann(False)
+    out["cpu_T_ref"], out["cpu_fitness_ref"] = r["T"], r["fitness"]
+    src, dst, _ = synth.make_pair(1000, 20000)
+    sets("gpu", src, dst, {"a": (src, 1), "b": (dst[:8000], 15), "c": (src + np.float32(3.0), 1), "d": (src[:4000], 20)})
+    np.savez_compressed(os.path.join(HERE, "ref_nanoflann_samples.npz"), **out)
+
+
 def main():
     if len(sys.argv) > 1 and sys.argv[1] == "quatro":
         return quatro_golden()
     assert os.path.exists(oracle.ref_so_path()), "build oracle/_ref first (make -C oracle ref)"
+    if len(sys.argv) > 1 and sys.argv[1] == "ref":
+        return ref_samples_golden()
     src, dst, Texp = synth.make_pair(4242, 3000, 3500)
     src3, dst3 = np.ascontiguousarray(src[:, :3]), np.ascontiguousarray(dst[:, :3])
     # ---- k-NN from the reference kd-tree
@@ -69,6 +100,7 @@ def main():
                         converged=res["converged"], iterations=res["iterations"], n_linearize=res["n_linearize"],
                         n_error=res["n_error"], trace=res["trace"])
     quatro_golden()
+    ref_samples_golden()
     print("wrote", os.listdir(HERE))
 
 

@@ -1,5 +1,5 @@
 """N>1 on real GPUs: the sharded batch (NCCL all-gather) returns the same bytes as a single rank (SURVEY.md §8e).
-Needs >= 2 visible GPUs (`gpurun --gpus 2`); skipped on a 1-GPU box, where tests/test_sharding.py (gloo) covers the logic."""
+Needs >= 2 visible GPUs; skipped on a 1-GPU box, where tests/test_sharding.py (gloo) covers the logic."""
 import os
 import socket
 import subprocess

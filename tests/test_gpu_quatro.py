@@ -31,7 +31,7 @@ def test_normals_and_fpfh_match_oracle(ctx, oracle, qpair):
     assert (dots > 0.999).mean() > 0.995
     # FPFH, stage-isolated (SURVEY §8(c)(iii): <= 1e-3 abs per bin): the GPU's OWN normals through the oracle's SPFH/FPFH.
     # What is left is the fp32 summation order (tree-walk order vs the oracle's sorted order): EVERY bin of EVERY point
-    # within 1e-3 (measured max 1.8e-4, profiles/r02/diag_fpfh.txt).
+    # within 1e-3 (profiles/diag_fpfh.py measures the deviation).
     _, of2 = oracle.fpfh_from_normals(dst, np.where(np.isnan(gn), np.nan, gn), 1.5)
     err2 = np.abs(gf - of2).max(1)
     assert err2.max() < 1e-3, np.quantile(err2, [0.5, 0.9, 0.99, 1.0])

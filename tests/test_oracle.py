@@ -1,10 +1,10 @@
 """CPU tests of the oracle (test infrastructure) -- run with -m "not gpu".
 
 The oracle is pinned three ways: (1) its k-NN against the REFERENCE's own kd-tree (golden answers
-generated from third_party/nano_gicp/.../nanoflann_impl.hpp and, when oracle/_ref is present, the live
-library); (2) closed-form known answers for the covariance / SE(3) pieces; (3) ground-truth recovery.
+generated from third_party/nano_gicp/.../nanoflann_impl.hpp); (2) closed-form known answers for the covariance / SE(3) pieces; (3) ground-truth recovery.
 """
 import os
+import zlib
 
 import numpy as np
 import pytest
@@ -28,22 +28,18 @@ def test_oracle_knn_equals_reference_nanoflann_golden(oracle):
         assert np.array_equal(idx, bi) and np.array_equal(d2, bd)
 
 
-def test_oracle_knn_equals_live_reference_nanoflann(oracle, synth):
-    if not os.path.exists(oracle.ref_so_path()):
-        pytest.skip("oracle/_ref not built (no /root/reference on this box)")
+def test_oracle_knn_equals_reference_nanoflann_samples(oracle, synth):
+    """The reference kd-tree's answers on sampled rows of these query sets (tests/golden/make_golden.py)."""
+    g = np.load(os.path.join(GOLD, "ref_nanoflann_samples.npz"))
     src, dst, _ = synth.make_pair(77, 6000, 7000)
-    ref = oracle.RefNanoflann(dst)
-    for q, k in ((dst[:2000], 15), (src, 1), (src[:500] + np.float32(2.5), 15)):
-        ri, rd = ref.knn(q, k)
-        oi, od = oracle.knn(dst, q, k)
-        _tie_ok(oi, od, ri, rd)
-    # the switchable backend gives the same registration (H/b sums follow the OpenMP guided schedule
-    # like the reference's, nano_gicp_impl.hpp:225,256-266, so only round-off may differ)
+    assert [zlib.crc32(src.tobytes()), zlib.crc32(dst.tobytes())] == list(g["cpu_crc"]), "synthetic input drifted"
+    for name, q, k in (("a", dst[:2000], 15), ("b", src, 1), ("c", src[:500] + np.float32(2.5), 15)):
+        oi, od = oracle.knn(dst, q[g["cpu_rows_" + name]], k)
+        _tie_ok(oi, od, g["cpu_idx_" + name], g["cpu_d2_" + name])
+    # the oracle's own kd-tree gives the registration the reference's kd-tree gave (H/b sums follow the OpenMP guided
+    # schedule like the reference's, nano_gicp_impl.hpp:225,256-266, so only round-off may differ)
     a = oracle.gicp_align(src, dst)
-    assert oracle.use_ref_nanoflann(True) == 0
-    b = oracle.gicp_align(src, dst)
-    oracle.use_ref_nanoflann(False)
-    assert np.abs(a["T"] - b["T"]).max() < 1e-9 and a["fitness"] == b["fitness"]
+    assert np.abs(a["T"] - g["cpu_T_ref"]).max() < 1e-9 and a["fitness"] == g["cpu_fitness_ref"]
 
 
 def test_covariance_of_a_plane_is_closed_form(oracle):
