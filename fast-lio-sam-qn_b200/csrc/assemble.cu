@@ -105,11 +105,13 @@ __global__ void __launch_bounds__(256) k_voxel_keys(const AssembleJob* jobs, flo
     J.sort.vals[0][i] = (uint32_t)i;
     return;
   }
+  // PCL keeps the index as unsigned int; div_b can exceed the guard's per-axis count by one, so the index can pass 2^31
+  // (and even 2^32).  Unsigned arithmetic keeps that defined: mod 2^32, the bits PCL's wrapping int arithmetic gives.
   const float4 p = J.merged[i];
-  const int i0 = (int)(floorf(p.x * inv_leaf) - (float)min_b[0]);
-  const int i1 = (int)(floorf(p.y * inv_leaf) - (float)min_b[1]);
-  const int i2 = (int)(floorf(p.z * inv_leaf) - (float)min_b[2]);
-  J.sort.keys[0][i] = (uint32_t)(i0 + i1 * div_b[0] + i2 * div_b[0] * div_b[1]);
+  const uint32_t i0 = (uint32_t)(int)(floorf(p.x * inv_leaf) - (float)min_b[0]);
+  const uint32_t i1 = (uint32_t)(int)(floorf(p.y * inv_leaf) - (float)min_b[1]);
+  const uint32_t i2 = (uint32_t)(int)(floorf(p.z * inv_leaf) - (float)min_b[2]);
+  J.sort.keys[0][i] = i0 + i1 * (uint32_t)div_b[0] + i2 * ((uint32_t)div_b[0] * (uint32_t)div_b[1]);
   J.sort.vals[0][i] = (uint32_t)i;
 }
 

@@ -712,6 +712,9 @@ void orc_transform_pcd(const float* in, int n, int stride, const double* T16, fl
 // voxelizePcd (utilities.hpp:38-63) = pcl::VoxelGrid, leaf L on all axes, downsample_all_data (SURVEY App. B.1):
 // fp32 min/max -> min_b = floor(min * (1/L)); ijk = floor(p * (1/L)) - float(min_b); idx = i + j*dx + k*dx*dy;
 // sort by idx; per occupied voxel the centroid of x, y, z, intensity (fp32 running sums) in idx order.
+// PCL stores idx as unsigned int (cloud_point_index_idx) and compares it unsigned: the guard below tests trunc(extent/L)+1
+// per axis while dx, dy, dz are floor(max/L) - floor(min/L) + 1, up to one larger, so an index can pass 2^31 and must
+// then sort after the smaller ones.  It is computed here modulo 2^32 (PCL's int arithmetic wraps to the same bits).
 // Within a voxel PCL's std::sort leaves the order unspecified; ascending point index is used here.
 // in/out records: (x, y, z, intensity).  Returns the number of voxels, or -1 when dx*dy*dz overflows int32
 // (PCL then warns and returns the input unchanged).
@@ -732,11 +735,11 @@ int orc_voxelize(const float* in, int n, float leaf, float* out /* up to n x 4 *
     div_b[d] = (int)std::floor(mx[d] * inv) - min_b[d] + 1;
   }
   if (dd[0] * dd[1] * dd[2] > (long long)std::numeric_limits<int>::max()) return -1;
-  std::vector<std::pair<int, int>> iv(n);
+  std::vector<std::pair<uint32_t, int>> iv(n);
   for (int i = 0; i < n; i++) {
-    int ijk[3];
-    for (int d = 0; d < 3; d++) ijk[d] = (int)(std::floor(in[4 * (size_t)i + d] * inv) - (float)min_b[d]);
-    iv[i] = {ijk[0] + ijk[1] * div_b[0] + ijk[2] * div_b[0] * div_b[1], i};
+    uint32_t ijk[3];
+    for (int d = 0; d < 3; d++) ijk[d] = (uint32_t)(int)(std::floor(in[4 * (size_t)i + d] * inv) - (float)min_b[d]);
+    iv[i] = {ijk[0] + ijk[1] * (uint32_t)div_b[0] + ijk[2] * ((uint32_t)div_b[0] * (uint32_t)div_b[1]), i};
   }
   std::sort(iv.begin(), iv.end());
   int nv = 0;

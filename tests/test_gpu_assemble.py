@@ -29,8 +29,8 @@ def test_fetch_closest_equals_oracle(store, oracle, seq):
     assert (want >= 0).sum() > 10 and (want < 0).sum() > 10
 
 
-def _sorted_rows(a):
-    return a[np.lexsort((a[:, 2], a[:, 1], a[:, 0]))]
+def _bits(a):
+    return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
 def test_assemble_quatro_and_submap_modes(ctx, store, oracle, seq):
@@ -48,8 +48,8 @@ def test_assemble_quatro_and_submap_modes(ctx, store, oracle, seq):
             for cloud, want in ((sc[k], os_), (dc[k], od_)):
                 got = ctx.cloud_points(cloud)
                 assert got.shape[0] == want.shape[0], "voxel count must match pcl::VoxelGrid's"
-                # same voxel order (linear voxel index); centroids agree to fp32 summation-order noise
-                assert np.abs(got - want[:, :3]).max() < 2e-4
+                # same voxel order (linear voxel index), same fp32 sums in the same order: bit-identical centroids
+                assert np.array_equal(_bits(got), _bits(want[:, :3]))
         for c in sc + dc:
             c.destroy()
 
@@ -67,7 +67,7 @@ def test_perform_loop_closure_matches_oracle(ctx, store, oracle, synth, seq):
         if qi[k]["valid"]:
             o = oracle.coarse_to_fine(src, dst, quatro_T=qi[k]["T"])
             rot, tr = synth.se3_error(res[k]["T"], o["T"])
-            assert rot < 3e-4 and tr < 3e-3, (k, rot, tr)  # inputs differ by the voxel-centroid fp32 noise (2e-4 m)
+            assert rot < 3e-4 and tr < 3e-3, (k, rot, tr)  # same clouds bit for bit; the registrations reduce in other orders
             # the loop closure undoes the accumulated odometry drift between the two keyframes
             drift = seq["true_poses"][c] @ np.linalg.inv(seq["poses"][c]) @ seq["poses"][q] @ np.linalg.inv(seq["true_poses"][q])
             # T maps src (map frame by odom) onto dst: T ~= D_c * inv(D_q) with D = odom * inv(true)
@@ -126,7 +126,7 @@ def test_batched_queries_see_their_own_keyframe_count(ctx, store, oracle, seq):
         for cloud, want in ((sc[k], os_), (dc[k], od_)):
             got = ctx.cloud_points(cloud)
             assert got.shape[0] == want.shape[0], (k, got.shape, want.shape)
-            assert np.abs(got - want[:, :3]).max() < 2e-4
+            assert np.array_equal(_bits(got), _bits(want[:, :3])), k
     # the batch-wide bound (the old behaviour: size = max(query) + 1) gives DIFFERENT clouds for the non-maximal queries
     sc2, dc2 = store.assemble(queries, closest, cfg, n_keyframes=int(queries.max()) + 1)
     assert sc2[0].n != sc[0].n and sc2[2].n == sc[2].n
@@ -182,3 +182,113 @@ def test_keyframe_store_slabs_and_reserve(ctx, synth):
         pts, pose, ts = kf.get(i)
         assert np.array_equal(pts, c[:, :4].astype(np.float32)) and np.array_equal(pose, T) and ts == t
     kf.destroy()
+
+
+# ---- k_assemble point for point --------------------------------------------------------------------------------
+SUBMAP_SIZES = (1, 255, 256, 257, 3001)  # segment boundaries inside and on the edges of 256-thread blocks
+
+
+@pytest.fixture(scope="module")
+def ragged_store(ctx, seq):
+    """40 keyframes with the sequence's (non-identity) poses and point counts cycling through SUBMAP_SIZES."""
+    kf = ctx.keyframes()
+    clouds = [seq["clouds"][k][:SUBMAP_SIZES[k % len(SUBMAP_SIZES)]] for k in range(40)]
+    for k, c in enumerate(clouds):
+        kf.add(c, seq["poses"][k], seq["stamps"][k])
+    yield kf, clouds, seq["poses"][:40]
+    kf.destroy()
+
+
+def test_assemble_point_for_point(ctx, oracle, ragged_store):
+    """At a 1 mm leaf every merged cloud (but a lone 1-point keyframe) trips VoxelGrid's int32 guard, so the call returns
+    k_assemble's merged cloud itself: it must be the concatenation of oracle.transform_pcd over the sub-map, bit for bit.
+    num_submap_keyframes = 15 merges up to 31 keyframes; centres at 0 and at n_keyframes - 1; n_keyframes per pair."""
+    import b200reg
+    kf, clouds, poses = ragged_store
+    leaf, rng = 1e-3, 15
+    src = np.array([0, 39, 20, 21], np.int32)
+    dst = np.array([39, 0, 22, 3], np.int32)
+    nks = np.array([40, 40, 40, 22], np.int32)
+    cfg = b200reg.default_loop_config()
+    cfg.num_submap_keyframes, cfg.voxel_res = rng, leaf
+    nseg = []
+    for quatro, submap in ((1, 1), (0, 0), (1, 0)):
+        cfg.enable_quatro, cfg.enable_submap_matching = quatro, submap
+        sc, dc = kf.assemble(src, dst, cfg, n_keyframes=nks)
+        for k in range(len(src)):
+            for centre, cloud, merged in ((src[k], sc[k], submap), (dst[k], dc[k], submap or not quatro)):
+                ids = [i for i in range(centre - rng, centre + rng + 1) if 0 <= i < nks[k] - 1] if merged else [centre]
+                nseg.append(len(ids))
+                want = np.concatenate([oracle.transform_pcd(clouds[i], poses[i]) for i in ids])
+                assert np.array_equal(_bits(oracle.voxelize(want, leaf)), _bits(want))  # the guard trips (or one point)
+                got = ctx.cloud_points(cloud)
+                assert np.array_equal(_bits(got), _bits(want[:, :3])), (quatro, submap, k, centre)
+        for c in sc + dc:
+            c.destroy()
+    assert max(nseg) == 2 * rng + 1 and min(nseg) == 1
+    cfg.num_submap_keyframes = 16  # 33 keyframes > MAXSEG
+    with pytest.raises(b200reg.B200RegError, match="error -1:"):
+        kf.assemble(src, dst, cfg, n_keyframes=nks)
+
+
+# ---- k_fetch_closest at its edges ------------------------------------------------------------------------------
+def _fetch(ctx, oracle, pos, stamps, queries, radius, tdiff):
+    """Single-point keyframes at `pos`; the device answer for `queries`, checked against the oracle."""
+    kf = ctx.keyframes()
+    for p, t in zip(pos, stamps):
+        T = np.eye(4)
+        T[:3, 3] = p
+        kf.add(np.ones((1, 4), np.float32), T, float(t))
+    got = kf.fetch_closest(np.asarray(queries, np.int32), radius, tdiff)
+    kf.destroy()
+    want = np.array([oracle.fetch_closest(pos, stamps, q, radius, tdiff) for q in queries])
+    assert np.array_equal(got, want), (got, want)
+    return got
+
+
+def test_fetch_closest_ties_go_to_the_lowest_index(ctx, oracle):
+    """Equidistant candidates in the same lane (idx mod 32) and in different lanes; four scenes 1 km apart, queried by
+    keyframes 96..99.  The distances are exact (integer offsets), so the ties are exact."""
+    n = 100
+    pos = np.zeros((n, 3))
+    pos[:, 1] = 5000.0 + 10.0 * np.arange(n)  # fillers: out of reach of every query
+    stamps = np.arange(n, dtype=np.float64)
+    scenes = [  # (candidate idx, offset); the answer
+        ([(5, (3, 4, 0)), (37, (0, 3, 4))], 5),                      # same lane 5
+        ([(33, (0, -5, 0)), (12, (5, 0, 0))], 12),                   # lane 12 holds the lower index than lane 1
+        ([(40, (4, 3, 0)), (8, (0, 0, -5)), (70, (-3, 0, 4))], 8),   # three lanes, two of them the same
+        ([(9, (3, 4, 0)), (41, (0, 4, 3)), (90, (4.999, 0, 0))], 90),  # strictly closer beats the lower index
+    ]
+    for a, (cands, _) in enumerate(scenes):
+        o = np.array([1000.0 * (a + 1), 0.0, 0.0])
+        pos[96 + a] = o
+        for idx, off in cands:
+            pos[idx] = o + np.array(off, np.float64)
+    got = _fetch(ctx, oracle, pos, stamps, [96, 97, 98, 99], 35.0, 0.5)
+    assert got.tolist() == [w for _, w in scenes]
+
+
+def test_fetch_closest_bounds_are_strict(ctx, oracle):
+    """radius > dist and tdiff < stamp gap: a candidate at exactly the radius and one exactly tdiff older are excluded."""
+    pos = np.array([[3.0, 4.0, 0.0], [1.0, 0.0, 0.0], [0.0, 0.0, 0.0]])  # keyframe 0 at distance 5, keyframe 1 at distance 1
+    stamps = np.array([0.0, 98.0, 100.0])                                # keyframe 1 exactly 2 s before the query
+    up, down = np.nextafter(5.0, np.inf), np.nextafter(2.0, -np.inf)
+    assert _fetch(ctx, oracle, pos, stamps, [2, 0], 5.0, 2.0).tolist() == [-1, -1]
+    assert _fetch(ctx, oracle, pos, stamps, [2], up, 2.0).tolist() == [0]
+    assert _fetch(ctx, oracle, pos, stamps, [2], 5.0, down).tolist() == [1]
+    assert _fetch(ctx, oracle, pos, stamps, [2], up, down).tolist() == [1]
+
+
+def test_fetch_closest_query_sizes(ctx, oracle):
+    """2001 keyframes on an integer lattice (ties and dist == radius everywhere), stamps 0.25 s apart so that the
+    candidate exactly tdiff = 2 s older is excluded: queries with fewer candidates than a warp's lanes, exactly 32,
+    just over, and 2000, in one batch; then every query."""
+    rng = np.random.default_rng(5)
+    pos = rng.integers(-8, 9, (2001, 3)).astype(np.float64)
+    stamps = 0.25 * np.arange(2001)
+    got = _fetch(ctx, oracle, pos, stamps, [0, 1, 31, 32, 33, 64, 2000], 5.0, 2.0)
+    assert got[0] == -1 and got[1] == -1 and (got[3:] >= 0).all()
+    every = _fetch(ctx, oracle, pos, stamps, np.arange(2001), 5.0, 2.0)
+    d = np.linalg.norm(pos[:1992] - pos[2000], axis=1)
+    assert (d == 5.0).any() and len(set(np.round(d, 9))) < 1992  # the boundary distance and ties occur
+    assert (every >= 0).mean() > 0.9

@@ -8,11 +8,14 @@ itertools) and compared with oracle/.  CPU only.
   6x6 solve                  numpy.linalg.solve                vs the step the LM trace implies
   33-D feature 1-NN + mutual sklearn brute force               vs oracle.match              (matcher.cc:378-455)
   max clique                 exhaustive search (<= 20 nodes)   vs the greedy k-core clique  (PMC_HEU substitute)
+  pcl::VoxelGrid             numpy fp32 restatement            vs orc_voxelize              (voxel_grid.hpp, SURVEY App. B.1)
 """
 import itertools
 
 import numpy as np
 import pytest
+
+import voxel_cases as vc
 
 
 @pytest.fixture(scope="module")
@@ -226,3 +229,60 @@ def test_greedy_clique_vs_exhaustive_max_clique(oracle):
             assert abs(est_yaw - yaw) < 0.05
     gaps = np.array(gaps)
     assert (gaps == 0).mean() >= 0.9 and gaps.max() <= 1, gaps  # measured: the greedy clique is maximum on these graphs
+
+
+def _np_voxel_grid(pts, leaf):
+    """pcl::VoxelGrid::applyFilter (PCL 1.10) in numpy, fp32 wherever PCL is: inverse leaf 1.0f / L; the int64 guard on
+    trunc((max - min) * inv) + 1 per axis; min_b = floor(min * inv), div_b = floor(max * inv) - min_b + 1; the index
+    ijk0 + ijk1 * div_b0 + ijk2 * div_b0 * div_b1 wrapped to unsigned int as PCL stores it; a stable sort by that
+    index alone (ascending point index inside a voxel); fp32 running sums added strictly in that order, divided once.
+    -> (points, dict(overflow, cells = guard product, max_key))."""
+    p = np.ascontiguousarray(pts, np.float32)
+    xyz = p[:, :3]
+    inv = np.float32(1) / np.float32(leaf)
+    mn, mx = xyz.min(0), xyz.max(0)
+    cells = int(np.prod(((mx - mn) * inv).astype(np.int64) + 1, dtype=object))
+    if cells > vc.INT32_MAX:
+        return p.copy(), dict(overflow=True, cells=cells, max_key=None)
+    min_b = np.floor(mn * inv).astype(np.int64)
+    div_b = np.floor(mx * inv).astype(np.int64) - min_b + 1
+    ijk = (np.floor(xyz * inv) - min_b.astype(np.float32)).astype(np.int64)
+    key = ((ijk[:, 0] + ijk[:, 1] * div_b[0] + ijk[:, 2] * (div_b[0] * div_b[1])) & 0xFFFFFFFF).astype(np.uint32)
+    order = np.argsort(key, kind="stable")
+    ks = key[order]
+    starts = np.flatnonzero(np.r_[True, ks[1:] != ks[:-1]])
+    counts = np.diff(np.r_[starts, len(ks)])
+    s = np.zeros((len(starts), 4), np.float32)
+    for k in range(int(counts.max())):  # k-th point of every voxel that has one: sequential per voxel (np.sum is pairwise)
+        live = counts > k
+        s[live] = s[live] + p[order[starts[live] + k]]
+    return s / counts[:, None].astype(np.float32), dict(overflow=False, cells=cells, max_key=int(ks[-1]))
+
+
+def _bits(a):
+    return np.ascontiguousarray(a, np.float32).view(np.uint32)
+
+
+def test_voxel_grid_vs_numpy_restatement(oracle, synth):
+    """orc_voxelize equals the numpy restatement bit for bit (count, order, centroids incl. intensity) on every crafted
+    cloud of voxel_cases and on keyframes of the test sequence at five leaf sizes; the cases reach what they are meant to."""
+    info = {}
+    for name, leaf, cloud in vc.crafted():
+        want, info[name] = _np_voxel_grid(cloud, leaf)
+        got = oracle.voxelize(cloud, leaf)
+        assert got.shape == want.shape and np.array_equal(_bits(got), _bits(want)), name
+    seq = vc.sweep_sequence(synth)
+    for k in vc.SWEEP_KEYFRAMES:
+        for leaf in vc.SWEEP_LEAVES:
+            want, info[(k, leaf)] = _np_voxel_grid(seq["clouds"][k], leaf)
+            got = oracle.voxelize(seq["clouds"][k], leaf)
+            assert got.shape == want.shape and np.array_equal(_bits(got), _bits(want)), (k, leaf)
+    assert info["guard_below"]["cells"] == vc.INT32_MAX - 1 and not info["guard_below"]["overflow"]
+    assert info["guard_above"]["cells"] == 2 ** 31 and info["guard_above"]["overflow"]
+    assert not info["index_wrap"]["overflow"] and info["index_wrap"]["max_key"] > vc.INT32_MAX
+    # the third 11-bit pass of the device sort sees real digits: keys above 2^28
+    big = sorted(str(c) for c, i in info.items() if not i["overflow"] and i["max_key"] >= 2 ** 28)
+    assert big == sorted(map(str, ["guard_below", "index_wrap", (0, 0.05), (70, 0.05)])), big
+    assert [c for c, i in info.items() if i["overflow"]] == ["guard_above"]
+    assert len(oracle.voxelize(vc.one_voxel(13), 0.3)) == 1
+    assert len(oracle.voxelize(vc.own_voxels(14), 1.0)) == 3000
