@@ -6,10 +6,10 @@ from concurrent.futures import ThreadPoolExecutor
 PKG = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(PKG, "csrc")
 REPO = os.path.dirname(PKG)
-SOURCES = ["api.cu", "index_build.cu", "gicp.cu", "quatro.cu", "assemble.cu", "batch.cu"]
+SOURCES = ["api.cu", "api_gicp.cu", "api_quatro.cu", "api_keyframes.cu", "index_build.cu", "gicp.cu", "quatro.cu", "assemble.cu", "batch.cu"]
 EXTRA = {"quatro.cu": ["-fmad=false"],    # fixed fp32 operation order for the FPFH / matcher arithmetic
          "assemble.cu": ["-fmad=false"]}  # transformPcd / VoxelGrid / candidate distances as the (FMA-free) reference computes them
-HEADERS = ["internal.cuh", "knn.cuh", "smallmath.cuh", "fpfh_basis.cuh", os.path.join(REPO, "include", "b200reg.h")]
+HEADERS = ["api.cuh", "launchers.cuh", "internal.cuh", "knn.cuh", "smallmath.cuh", "fpfh_basis.cuh", os.path.join(REPO, "include", "b200reg.h")]
 LIB = os.path.join(CSRC, "libb200reg.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC",

@@ -1,0 +1,169 @@
+// api.cuh -- what the host files of the C ABI share (api.cu, api_gicp.cu, api_quatro.cu, api_keyframes.cu): the context and
+// cloud objects, error reporting, profiling scopes, stream-ordered scratch memory and the helpers more than one area uses.
+// Host orchestration only; every arithmetic step of the path runs in the kernels of index_build.cu / gicp.cu / quatro.cu /
+// assemble.cu.  There is no CPU fallback anywhere in this library.
+#pragma once
+#include <cuda_runtime.h>
+#include <nccl.h>  // types only: the library is dlopen()ed in b200reg_comm_*
+
+#include <cstddef>
+#include <cstdint>
+#include <string>
+#include <vector>
+
+#include "../../include/b200reg.h"
+#include "internal.cuh"
+#include "launchers.cuh"
+
+using namespace b200;
+
+namespace b200 {
+int fail(int code, const std::string& msg);  // sets b200reg_last_error() and returns code
+}  // namespace b200
+#define CU(call)                                                                                              \
+  do {                                                                                                        \
+    cudaError_t _e = (call);                                                                                  \
+    if (_e != cudaSuccess)                                                                                    \
+      return fail(B200REG_ECUDA, std::string(#call) + ": " + cudaGetErrorString(_e) + " @" + __FILE__ + ":" + \
+                                     std::to_string(__LINE__));                                               \
+  } while (0)
+
+enum { CLS_BUILD = 0, CLS_COV = 1, CLS_STEP = 2, CLS_MISC = 3, CLS_FPFH = 4, CLS_MATCH = 5, CLS_SEARCH = 6, CLS_ACCUM = 7, CLS_CTRL = 8, NCLS = 9 };
+
+struct b200reg_ctx {
+  int device = 0;
+  cudaStream_t own_stream = nullptr;
+  cudaStream_t stream = nullptr;
+  cudaStream_t copy_stream = nullptr;  // H2D uploads of later chunks overlap the compute of earlier ones
+  cudaMemPool_t pool = nullptr;        // per-context pool: reuse never adds dependencies on another context's streams
+  int pipeline_chunks = 4;
+  int sm_count = 132;
+  // persistent arena of the batched LM solve: every kernel argument of the solve's CUDA graph points in here, so the graph is
+  // instantiated once and re-launched by every b200reg_gicp_align call until a larger batch makes the arena grow
+  struct LmArena {
+    int cap = 0;
+    PairDev* d_pairs = nullptr;
+    PairState* d_states = nullptr;
+    LmSched* d_sched = nullptr;  // header + slots[cap]
+    double* d_guess = nullptr;   // [16 * cap]
+    LmCall* d_call = nullptr;
+    LmCall* h_call = nullptr;    // pinned staging
+    PairState* h_states = nullptr;  // pinned read-back
+    LmGraph graph;
+  } lm;
+  // the path's one collective (b200reg_comm_*): NCCL communicator of this rank
+  ncclComm_t comm = nullptr;
+  int rank = -1, world = 1;
+  int64_t launches = 0;
+  // optional per-kernel-family timing with CUDA events on the launching stream
+  bool profiling = false;
+  struct Span { int cls; cudaEvent_t a, b; };
+  std::vector<Span> pending;
+  std::vector<cudaEvent_t> free_events;
+  double prof_ms[NCLS] = {0};
+  double prof_bytes[NCLS] = {0};
+  int64_t prof_launches[NCLS] = {0};
+};
+
+struct b200reg_cloud {
+  CloudDev dev;            // device pointers + sizes
+  void* slab = nullptr;    // persistent allocation (pts, tnodes, cov, rank)
+  void* fslab = nullptr;   // Quatro features (nrm, spfh, fpfh), allocated on demand
+  bool has_cov = false;
+  bool cov_user = false;   // set by b200reg_set_covariances: never recomputed on demand (nano_gicp_impl.hpp:162-167)
+  int cov_k = 0;
+  int cov_method = 3;
+  bool has_fpfh = false;
+  double normal_r = 0, fpfh_r = 0;
+};
+
+namespace b200 {
+
+cudaEvent_t prof_event(b200reg_ctx* c);
+struct ProfScope {  // brackets the kernels launched while it is alive
+  b200reg_ctx* c;
+  int cls;
+  cudaEvent_t a = nullptr;
+  int64_t l0;
+  ProfScope(b200reg_ctx* c_, int cls_) : c(c_), cls(cls_), l0(c_->launches) {
+    if (c->profiling) {
+      a = prof_event(c);
+      cudaEventRecord(a, c->stream);
+    }
+  }
+  ~ProfScope() {
+    if (c->profiling) {
+      cudaEvent_t b = prof_event(c);
+      cudaEventRecord(b, c->stream);
+      c->pending.push_back({cls, a, b});
+      c->prof_launches[cls] += c->launches - l0;
+    }
+  }
+};
+
+// Stream-ordered scratch memory with scope lifetime: everything allocated through it is returned to the context's
+// pool when the scope ends -- on every path, including the early error returns of the CU() macro.
+struct Scratch {
+  b200reg_ctx* c;
+  std::vector<void*> ptrs;
+  explicit Scratch(b200reg_ctx* c_) : c(c_) {}
+  Scratch(const Scratch&) = delete;
+  Scratch& operator=(const Scratch&) = delete;
+  cudaError_t alloc(void** p, size_t bytes) {
+    cudaError_t e = cudaMallocFromPoolAsync(p, bytes ? bytes : 16, c->pool, c->stream);
+    if (e == cudaSuccess) ptrs.push_back(*p);
+    return e;
+  }
+  // a device copy of `bytes` of host memory, queued on the context's stream
+  template <class T>
+  cudaError_t upload(T** p, const void* host, size_t bytes) {
+    const cudaError_t e = alloc((void**)p, bytes);
+    return e == cudaSuccess ? cudaMemcpyAsync(*p, host, bytes, cudaMemcpyHostToDevice, c->stream) : e;
+  }
+  ~Scratch() {
+    for (void* p : ptrs) cudaFreeAsync(p, c->stream);
+  }
+};
+
+// scope guard: cloud handles created inside a call are released on EVERY exit path (the CU() macro returns early)
+struct CloudBag {
+  b200reg_ctx* c;
+  std::vector<b200reg_cloud*> cl;
+  explicit CloudBag(b200reg_ctx* c_) : c(c_) {}
+  ~CloudBag() {
+    for (b200reg_cloud* p : cl) b200reg_cloud_destroy(c, p);
+  }
+};
+
+// Sub-buffers carved out of one allocation, each starting at a 256-byte boundary: take() returns the offset of the next
+// one, size is what the whole allocation needs.
+struct Layout {
+  size_t size = 0;
+  size_t take(size_t bytes) {
+    const size_t o = size;
+    size = (size + bytes + 255) / 256 * 256;
+    return o;
+  }
+};
+
+// RegistrationOutput's defaults (loop_closure.h:64-70): identity transforms, score_ = DBL_MAX, not valid
+b200reg_result default_result();
+
+// The clouds of `count` pairs, built in one batch: the source clouds come first, then the targets.  They go to src_out /
+// tgt_out and are owned by `bag`.
+int create_pair_clouds(b200reg_ctx* c, int count, const float* const* src_xyz, const size_t* src_n, const float* const* tgt_xyz,
+                       const size_t* tgt_n, size_t stride_bytes, int on_device, CloudBag& bag, b200reg_cloud** src_out,
+                       b200reg_cloud** tgt_out);
+
+// orig[p] = the original index of the point at sorted position p (the int bits of pts[p].w).  Synchronises the stream, so
+// the downloads the caller queued before have landed too.  pts_out, if given, receives the sorted points.
+int sorted_to_original(b200reg_ctx* c, const CloudDev& d, std::vector<int>& orig, std::vector<float4>* pts_out = nullptr);
+
+void lm_arena_free(b200reg_ctx* c);  // api_gicp.cu
+
+// LoopClosure::coarseToFineAlignment on cloud handles (api_quatro.cu)
+int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst,
+                             const b200reg_quatro_params* qp, const b200reg_gicp_params* gp, b200reg_result* out,
+                             b200reg_quatro_info* quatro_out);
+
+}  // namespace b200

@@ -5,11 +5,9 @@
 // Keyframe clouds stay on the device from the moment they are added, so a loop-closure attempt moves no point data
 // over PCIe: candidate search, cloud assembly, voxel grid, index build and registration all start from HBM.
 #include "internal.cuh"
+#include "launchers.cuh"
 
 namespace b200 {
-
-int launch_radix_sort(const CloudDev* d_clouds, int count, int max_n, int key_bits, cudaStream_t s);
-int radix_sort_result_buf(int key_bits);
 
 // one warp per query keyframe q (treated as the LATEST keyframe: candidates are idx < q)
 __global__ void __launch_bounds__(256) k_fetch_closest(const double* pos, const double* stamp, const int* queries, int count, double radius,

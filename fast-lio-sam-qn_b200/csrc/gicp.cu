@@ -13,6 +13,7 @@
 //   pcl::Registration::getFitnessScore (call site fast_lio_sam_qn/src/loop_closure.cpp:127)
 #include "internal.cuh"
 #include "knn.cuh"
+#include "launchers.cuh"
 #include "smallmath.cuh"
 
 namespace b200 {
@@ -782,7 +783,7 @@ void launch_gicp_init(const PairDev* pairs, PairState* states, const double* d_g
 }
 
 // One LM step over every still-active pair = search + accumulate + controller.  blocks_*: persistent grid sizes (work
-// items are strided over them); the kernels are correct for any value >= 1.  Returns the launches issued.
+// items are strided over them); the kernels are correct for any value >= 1.
 constexpr int CTRL_BLOCKS = 64;
 void launch_gicp_search(const PairDev* pairs, const PairState* states, int blocks, const LmCall* call, const LmSched* sched, cudaStream_t s) {
   k_gicp_search<<<blocks, STEP_THREADS, 0, s>>>(pairs, states, call, sched);
@@ -792,13 +793,6 @@ void launch_gicp_accum(const PairDev* pairs, const PairState* states, int blocks
 }
 void launch_gicp_control(const PairDev* pairs, PairState* states, LmCall* call, LmSched* sched, cudaStream_t s) {
   k_gicp_control<<<CTRL_BLOCKS, CTRL_THREADS, 0, s>>>(pairs, states, call, sched);
-}
-int launch_gicp_step(const PairDev* pairs, PairState* states, int blocks_search, int blocks_accum, LmCall* call, LmSched* sched,
-                     cudaStream_t s) {
-  launch_gicp_search(pairs, states, blocks_search, call, sched, s);
-  launch_gicp_accum(pairs, states, blocks_accum, sched, s);
-  launch_gicp_control(pairs, states, call, sched, s);
-  return 3;
 }
 
 // The whole solve as ONE CUDA graph: init kernel, then a WHILE node whose body is the three step kernels; the controller's

@@ -20,6 +20,7 @@
 // straddle octant boundaries give huge overlapping boxes (195 node + 71 leaf visits per 15-NN
 // query vs 29 + 7 with prefix splits on the 100k KITTI-shaped scan).
 #include "internal.cuh"
+#include "launchers.cuh"
 
 namespace b200 {
 

@@ -1,0 +1,43 @@
+// launchers.cuh -- host entry points of the kernel files.  Both the file that defines a launcher and every file that calls
+// it include this header, so a signature that drifts fails the build instead of the load.
+#pragma once
+#include <cstddef>
+
+#include "internal.cuh"
+
+namespace b200 {
+
+// index_build.cu
+size_t radix_sort_ws_bytes(int n, int key_bits);
+int radix_sort_result_buf(int key_bits);
+int launch_radix_sort(const CloudDev* d_clouds, int count, int max_n, int key_bits, cudaStream_t s);
+int launch_index_build(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s);
+
+// gicp.cu
+int launch_covariances(const CloudDev* d_clouds, int count, int max_n, int k, int method, cudaStream_t s);
+void launch_gicp_init(const PairDev* pairs, PairState* states, const double* d_guess, LmCall* call, LmSched* sched, cudaStream_t s);
+void launch_gicp_search(const PairDev* pairs, const PairState* states, int blocks, const LmCall* call, const LmSched* sched, cudaStream_t s);
+void launch_gicp_accum(const PairDev* pairs, const PairState* states, int blocks, const LmSched* sched, cudaStream_t s);
+void launch_gicp_control(const PairDev* pairs, PairState* states, LmCall* call, LmSched* sched, cudaStream_t s);
+cudaError_t lm_graph_build(LmGraph* g, const PairDev* pairs, PairState* states, const double* guess, LmCall* call, LmSched* sched,
+                           int blocks_search, int blocks_accum);
+void lm_graph_destroy(LmGraph* g);
+int launch_knn_queries(const CloudDev& c, const float* d_q, int nq, int qstride, int k, int* idx, float* d2, cudaStream_t s, int brute);
+void launch_set_covariances(const CloudDev& c, const double* d_cov9, cudaStream_t s);
+void launch_transform_out(const CloudDev& c, const float* d_Tf, float* d_out3, cudaStream_t s);
+
+// quatro.cu
+cudaError_t quatro_init_device();
+int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2, float fpfh_r2, cudaStream_t s);
+int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, int max_nj, const QuatroParamsDev& prm, cudaStream_t s);
+void launch_transform_raw(const CloudDev* d_clouds, const double* d_T16s, int count, int max_n, float4* const* d_outs, cudaStream_t s);
+
+// assemble.cu
+void launch_pack_xyzi(const float* d_raw, int stride, int n, float4* d_out, cudaStream_t s);
+void launch_ingest_world(const float* d_raw, int stride, int n, const double* d_Tinv, float4* d_out, cudaStream_t s);
+int launch_fetch_closest(const double* d_pos, const double* d_stamp, const int* d_queries, int count, double radius, double tdiff,
+                         int* d_out, cudaStream_t s);
+int launch_assemble_voxelize(const AssembleJob* d_jobs, const CloudDev* d_sort, int count, int max_total, const KeyframeDev* d_kfs,
+                             const double* d_poses, float inv_leaf, cudaStream_t s);
+
+}  // namespace b200

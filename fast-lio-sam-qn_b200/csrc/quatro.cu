@@ -18,6 +18,7 @@
 #include "internal.cuh"
 #include "fpfh_basis.cuh"
 #include "knn.cuh"
+#include "launchers.cuh"
 #include "smallmath.cuh"
 
 namespace b200 {
@@ -1734,8 +1735,6 @@ __global__ void __launch_bounds__(256) k_transform_raw(const CloudDev* clouds, c
 // ------------------------------------------------------------------------------------------------
 // host launchers
 // ------------------------------------------------------------------------------------------------
-int launch_radix_sort(const CloudDev* d_clouds, int count, int max_n, int key_bits, cudaStream_t s);  // index_build.cu
-
 int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2, float fpfh_r2, cudaStream_t s) {
   dim3 grid((max_n + STEP_THREADS - 1) / STEP_THREADS, count);
   k_normals<<<grid, STEP_THREADS, 0, s>>>(d_clouds, normal_r2);
