@@ -81,8 +81,9 @@ EXPORTS = [
     "b200reg_batch_create", "b200reg_batch_destroy", "b200reg_batch_submit_icp", "b200reg_batch_submit_loop_closure",
     "b200reg_batch_wait", "b200reg_batch_wait_all", "b200reg_batch_launch_count", "b200reg_batch_depth",
     "b200reg_comm_unique_id", "b200reg_comm_init", "b200reg_comm_destroy", "b200reg_comm_rank", "b200reg_comm_world",
-    "b200reg_allgather_results",
+    "b200reg_allgather_results", "b200reg_radius_search",
 ]
+ESTATE = -4  # B200REG_ESTATE
 
 
 def _point_at_bundled_nccl():
@@ -384,6 +385,27 @@ class Context:
                                  C.c_size_t(q.shape[1] * 4), int(k), idx.ctypes.data_as(C.c_void_p),
                                  d2.ctypes.data_as(C.c_void_p)))
         return idx, d2
+
+    def radius_search(self, cloud, queries, sq_radius, sorted=True):
+        """KdTreeFLANN::radiusSearch for every row of `queries` -> (offsets (nq+1,) int64, idx int32, d2 float32), CSR:
+        the neighbours of query i are idx[offsets[i]:offsets[i+1]] (ORIGINAL point indices).  sq_radius is SQUARED, as the
+        reference takes it (points with d2 < float32(sq_radius)); sorted: ascending (d2, index), else ascending index."""
+        q = _pts(queries)
+        nq = len(q)
+        offsets = np.empty(nq + 1, np.int64)
+        cap = nq * min(cloud.n, 64)  # a first guess; on ESTATE the offsets hold the exact total
+        for _ in range(2):
+            idx = np.empty(max(cap, 1), np.int32)
+            d2 = np.empty(max(cap, 1), np.float32)
+            rc = lib().b200reg_radius_search(self.h, cloud.h, q.ctypes.data_as(C.c_void_p), C.c_size_t(nq), C.c_size_t(q.shape[1] * 4),
+                                             C.c_double(sq_radius), int(bool(sorted)), offsets.ctypes.data_as(C.c_void_p),
+                                             C.c_size_t(cap), idx.ctypes.data_as(C.c_void_p), d2.ctypes.data_as(C.c_void_p))
+            if rc != ESTATE:
+                break
+            cap = int(offsets[-1])
+        _check(rc)
+        total = int(offsets[-1])
+        return offsets, idx[:total], d2[:total]
 
     def get_covariances(self, cloud):
         out = np.empty((cloud.n, 3, 3), np.float64)

@@ -426,6 +426,131 @@ static int knn_impl(b200reg_ctx* c, const b200reg_cloud* cl, const float* querie
   return B200REG_OK;
 }
 
+// Fixed-radius search (radius.cu).  The neighbours of the queries are produced chunk by chunk: a chunk is a run of
+// consecutive caller queries with at most kRadiusChunk neighbours (or one query with more), so device memory stays bounded
+// by max(kRadiusChunk, cloud size) entries, 28 bytes each, whatever the total, and each chunk's block of the output is
+// contiguous on the host.
+static constexpr int64_t kRadiusChunk = int64_t(1) << 23;
+
+int b200reg_radius_search(b200reg_ctx* c, const b200reg_cloud* cl, const float* queries, size_t nq, size_t qstride_bytes,
+                          double sq_radius, int sorted, int64_t* offsets_out, size_t capacity, int32_t* idx_out, float* d2_out) {
+  if (!c || !cl || !queries || !offsets_out || nq == 0 || nq >= ((size_t)1 << 30) || qstride_bytes < 12 || qstride_bytes % 4)
+    return fail(B200REG_EINVAL, "bad argument (nq must be 1..2^30-1, qstride_bytes a multiple of 4, >= 12)");
+  if ((idx_out == nullptr) != (d2_out == nullptr)) return fail(B200REG_EINVAL, "idx_out and d2_out: both or neither (count only)");
+  const float r2 = (float)sq_radius;  // RadiusResultSet<float, int>(radius): converted to float, NOT squared
+  const int n = (int)nq, qs = (int)(qstride_bytes / 4);
+  CU(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  Scratch scratch(c);
+  ProfScope ps(c, CLS_MISC);
+  float* d_q = nullptr;
+  uint32_t *qk[2], *qv[2];
+  int* d_cnt = nullptr;
+  int64_t* d_off = nullptr;
+  char* d_ws = nullptr;  // zeroed sort work memory: query order, then (several chunks) chunk grouping
+  void* d_scan = nullptr;
+  const size_t sort_ws = radix_sort_ws_bytes(n, 30);
+  CU(scratch.upload(&d_q, queries, nq * qstride_bytes));
+  for (int b = 0; b < 2; b++) {
+    CU(scratch.alloc((void**)&qk[b], nq * 4));
+    CU(scratch.alloc((void**)&qv[b], nq * 4));
+  }
+  CU(scratch.alloc((void**)&d_cnt, nq * 4));
+  CU(scratch.alloc((void**)&d_off, (nq + 1) * 8));
+  CU(scratch.alloc((void**)&d_scan, radius_scan_ws_bytes(n)));
+  CU(scratch.alloc((void**)&d_ws, 2 * sort_ws));
+  CU(cudaMemsetAsync(d_ws, 0, 2 * sort_ws, s));
+  // Stable sort of (k0, v0) with k1 / v1 as the ping-pong halves; *out = whichever value buffer holds the result.  The radix
+  // sort reads its arrays through a device-side descriptor (only n / keys / vals / hist are used).
+  auto sort = [&](int m, uint32_t* k0, uint32_t* k1, uint32_t* v0, uint32_t* v1, void* hist, int key_bits, uint32_t** out) -> int {
+    CloudDev d = {};
+    d.n = m;
+    d.keys[0] = k0; d.keys[1] = k1;
+    d.vals[0] = v0; d.vals[1] = v1;
+    d.hist = (uint32_t*)hist;
+    CloudDev* dd = nullptr;
+    CU(scratch.upload(&dd, &d, sizeof(d)));
+    c->launches += launch_radix_sort(dd, 1, m, key_bits, s);
+    *out = radix_sort_result_buf(key_bits) ? v1 : v0;
+    return B200REG_OK;
+  };
+  // 1. queries in the cloud's Morton order, 2. counts, 3. offsets
+  c->launches += launch_radius_query_keys(cl->dev, d_q, n, qs, qk[0], qv[0], s);
+  uint32_t* order = nullptr;
+  if (const int rc = sort(n, qk[0], qk[1], qv[0], qv[1], d_ws, 30, &order)) return rc;
+  c->launches += launch_radius_count(cl->dev, d_q, qs, order, n, r2, d_cnt, s);
+  c->launches += launch_radius_scan(d_cnt, n, d_off, d_scan, s);
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(offsets_out, d_off, (nq + 1) * 8, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  const int64_t total = offsets_out[n];
+  if (!idx_out || total == 0) return B200REG_OK;
+  if ((uint64_t)total > (uint64_t)capacity)
+    return fail(B200REG_ESTATE, "radius search found " + std::to_string(total) + " neighbours, capacity is " + std::to_string(capacity));
+  // 4. chunks of consecutive caller queries
+  std::vector<int> starts{0};
+  int64_t max_entries = 0;
+  for (int i = 0, a = 0; i <= n; i++) {
+    if (i == n || (offsets_out[i + 1] - offsets_out[a] > kRadiusChunk && i > a)) {
+      max_entries = std::max(max_entries, offsets_out[i] - offsets_out[a]);
+      if (i == n) break;
+      starts.push_back(i);
+      a = i;
+    }
+  }
+  const int nchunks = (int)starts.size();
+  starts.push_back(n);
+  if (max_entries >= (int64_t)INT32_MAX) return fail(B200REG_EINVAL, "one query has 2^31 or more neighbours");
+  if (nchunks > 1) {  // group the Morton-ordered queries by chunk (stable: Morton order inside each chunk)
+    int* d_starts = nullptr;
+    CU(scratch.upload(&d_starts, starts.data(), starts.size() * 4));
+    uint32_t* other = order == qv[0] ? qv[1] : qv[0];
+    c->launches += launch_radius_chunk_keys(order, n, d_starts, nchunks, qk[0], other, s);
+    if (const int rc = sort(n, qk[0], qk[1], other, order, d_ws + sort_ws, 30, &order)) return rc;
+  }
+  // per chunk: entries, three sort passes' key / value ping-pong, three zeroed sort work areas
+  const size_t m = (size_t)max_entries;
+  int* e_idx = nullptr;
+  float* e_d2 = nullptr;
+  uint32_t *e_seg = nullptr, *K[2], *V[2];
+  char* ews = nullptr;
+  const size_t ews1 = radix_sort_ws_bytes((int)m, 32);
+  CU(scratch.alloc((void**)&e_idx, m * 4));
+  CU(scratch.alloc((void**)&e_d2, m * 4));
+  CU(scratch.alloc((void**)&e_seg, m * 4));
+  for (int b = 0; b < 2; b++) {
+    CU(scratch.alloc((void**)&K[b], m * 4));
+    CU(scratch.alloc((void**)&V[b], m * 4));
+  }
+  CU(scratch.alloc((void**)&ews, 3 * ews1));
+  for (int ci = 0; ci < nchunks; ci++) {
+    RadiusChunk ch;
+    ch.q0 = ch.r0 = starts[ci];
+    ch.nr = starts[ci + 1] - starts[ci];
+    ch.base = offsets_out[ch.q0];
+    const int me = (int)(offsets_out[starts[ci + 1]] - ch.base);
+    if (me == 0) continue;
+    ch.e_idx = e_idx; ch.e_d2 = e_d2; ch.e_seg = e_seg; ch.keys = K[0]; ch.vals = V[0];
+    CU(cudaMemsetAsync(ews, 0, 3 * ews1, s));
+    c->launches += launch_radius_fill(cl->dev, d_q, qs, order, r2, d_off, ch, s);
+    // stable LSD passes: original index, (sorted) d2, query -> per query ascending index or ascending (d2, index)
+    uint32_t* cur = nullptr;
+    if (const int rc = sort(me, K[0], K[1], V[0], V[1], ews, 30, &cur)) return rc;
+    if (sorted) {  // d2 >= 0 and never NaN here: its bit pattern orders like the value
+      c->launches += launch_radius_rekey(cur, me, (const uint32_t*)e_d2, K[0], s);
+      if (const int rc = sort(me, K[0], K[1], cur, cur == V[0] ? V[1] : V[0], ews + ews1, 32, &cur)) return rc;
+    }
+    c->launches += launch_radius_rekey(cur, me, e_seg, K[0], s);
+    if (const int rc = sort(me, K[0], K[1], cur, cur == V[0] ? V[1] : V[0], ews + 2 * ews1, 30, &cur)) return rc;
+    c->launches += launch_radius_gather(cur, me, e_idx, e_d2, (int*)K[0], (float*)K[1], s);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(idx_out + ch.base, K[0], (size_t)me * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(d2_out + ch.base, K[1], (size_t)me * 4, cudaMemcpyDeviceToHost, s));
+  }
+  CU(cudaStreamSynchronize(s));
+  return B200REG_OK;
+}
+
 int b200reg_get_covariances(b200reg_ctx* c, const b200reg_cloud* cl, double* cov9_out) {
   if (!c || !cl || !cov9_out) return fail(B200REG_EINVAL, "bad argument");
   if (!cl->has_cov) return fail(B200REG_ESTATE, "covariances not computed");

@@ -62,15 +62,6 @@ __global__ void __launch_bounds__(256) k_bbox(const CloudDev* clouds) {
   }
 }
 
-__device__ __forceinline__ uint32_t expand10(uint32_t v) {
-  v &= 0x3FFu;
-  v = (v | (v << 16)) & 0x030000FFu;
-  v = (v | (v << 8)) & 0x0300F00Fu;
-  v = (v | (v << 4)) & 0x030C30C3u;
-  v = (v | (v << 2)) & 0x09249249u;
-  return v;
-}
-
 // ------------------------------------------------------------------------------------
 // stable LSD radix sort with one kernel per pass
 // ------------------------------------------------------------------------------------

@@ -228,4 +228,14 @@ __device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i
 
 __host__ __device__ __forceinline__ int leaf_ref(int start, int count) { return -1 - ((start << 4) | count); }
 
+// 10 bits -> every third bit of 30 (one axis of a 30-bit Morton key: the index build's cells, radius.cu's query order)
+__device__ __forceinline__ uint32_t expand10(uint32_t v) {
+  v &= 0x3FFu;
+  v = (v | (v << 16)) & 0x030000FFu;
+  v = (v | (v << 8)) & 0x0300F00Fu;
+  v = (v | (v << 4)) & 0x030C30C3u;
+  v = (v | (v << 2)) & 0x09249249u;
+  return v;
+}
+
 }  // namespace b200

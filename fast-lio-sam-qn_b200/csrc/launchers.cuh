@@ -32,6 +32,28 @@ int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2,
 int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, int max_nj, const QuatroParamsDev& prm, cudaStream_t s);
 void launch_transform_raw(const CloudDev* d_clouds, const double* d_T16s, int count, int max_n, float4* const* d_outs, cudaStream_t s);
 
+// radius.cu: the stages of b200reg_radius_search (order, count, scan, fill, segmented sort); each returns its launches
+int launch_radius_query_keys(const CloudDev& c, const float* d_q, int nq, int qstride, uint32_t* keys, uint32_t* vals, cudaStream_t s);
+int launch_radius_count(const CloudDev& c, const float* d_q, int qstride, const uint32_t* order, int nq, float r2, int* counts,
+                        cudaStream_t s);
+size_t radius_scan_ws_bytes(int nq);
+int launch_radius_scan(const int* counts, int nq, int64_t* offsets, void* ws, cudaStream_t s);
+int launch_radius_chunk_keys(const uint32_t* order, int nq, const int* starts, int nchunks, uint32_t* keys, uint32_t* vals,
+                             cudaStream_t s);
+struct RadiusChunk {  // one chunk of queries: sorted rows [r0, r0 + nr) of `order`, caller indices [q0, q0 + nr)
+  int r0, nr, q0;
+  int64_t base;     // offsets[q0]: entry e of the chunk is neighbour (base + e) of the whole call
+  int* e_idx;       // [entries] original point index
+  float* e_d2;      // [entries]
+  uint32_t* e_seg;  // [entries] caller index - q0
+  uint32_t* keys;   // [entries] sort input: the original index ...
+  uint32_t* vals;   // [entries] ... and the entry itself
+};
+int launch_radius_fill(const CloudDev& c, const float* d_q, int qstride, const uint32_t* order, float r2, const int64_t* offsets,
+                       const RadiusChunk& ch, cudaStream_t s);
+int launch_radius_rekey(const uint32_t* perm, int m, const uint32_t* src, uint32_t* keys, cudaStream_t s);
+int launch_radius_gather(const uint32_t* perm, int m, const int* e_idx, const float* e_d2, int* idx_out, float* d2_out, cudaStream_t s);
+
 // assemble.cu
 void launch_pack_xyzi(const float* d_raw, int stride, int n, float4* d_out, cudaStream_t s);
 void launch_ingest_world(const float* d_raw, int stride, int n, const double* d_Tinv, float4* d_out, cudaStream_t s);

@@ -11,9 +11,11 @@
 //   * setNumThreads is accepted and ignored; RANSAC* / EuclideanFitnessEpsilon setters are stored and never read,
 //     exactly like the reference's LSQ path (SURVEY.md §8b);
 //   * all five RegularizationMethods are built (PLANE is the default, nano_gicp_impl.hpp:61); k may be 1..32;
-//   * source_kdtree_/target_kdtree_ do not exist (the index is a device-side LBVH); covariances live on the device and are
-//     materialised on the host lazily by getSource/TargetCovariances() as Eigen::Matrix4d (4th row/column zero, like the
-//     reference's, nano_gicp_impl.hpp:354); setSource/TargetCovariances upload the caller's.
+//   * source_kdtree_/target_kdtree_ are nanoflann::KdTreeFLANN facades (nanoflann.hpp in this directory) over the SAME device
+//     cloud and index the class builds for registration: no second upload, no second build;
+//   * covariances live on the device and are materialised on the host lazily by getSource/TargetCovariances() as
+//     Eigen::Matrix4d (4th row/column zero, like the reference's, nano_gicp_impl.hpp:354); setSource/TargetCovariances
+//     upload the caller's.
 #pragma once
 #include <array>
 #include <cmath>
@@ -23,6 +25,7 @@
 #include <vector>
 
 #include "../b200reg_compat.hpp"
+#include "nanoflann.hpp"
 
 namespace nano_gicp {
 
@@ -45,6 +48,8 @@ class NanoGICP {
   using Matrix6d = Eigen::Matrix<double, 6, 6>;
 
   NanoGICP() {
+    source_kdtree_.reset(new nanoflann::KdTreeFLANN<PointSource>);  // nano_gicp_impl.hpp:62-63
+    target_kdtree_.reset(new nanoflann::KdTreeFLANN<PointTarget>);
     b200reg_default_gicp_params(&prm_);
     prm_.k_correspondences = 20;                                 // nano_gicp_impl.hpp:57
     prm_.max_iterations = 64;                                    // lsq_registration_impl.hpp:51
@@ -92,12 +97,14 @@ class NanoGICP {
     if (input_ == cloud) return;
     input_ = cloud;
     upload(cloud, &src_);
+    source_kdtree_->shareDeviceCloud(cloud, src_);
     src_cov_ok_ = false;
   }
   void setInputTarget(const PointCloudTargetConstPtr& cloud) {
     if (target_ == cloud) return;
     target_ = cloud;
     upload(cloud, &tgt_);
+    target_kdtree_->shareDeviceCloud(cloud, tgt_);
     tgt_cov_ok_ = false;
   }
   void registerInputSource(const PointCloudSourceConstPtr& cloud) { setInputSource(cloud); }
@@ -115,14 +122,15 @@ class NanoGICP {
     std::swap(input_, target_);
     std::swap(src_, tgt_);
     std::swap(src_cov_ok_, tgt_cov_ok_);
+    source_kdtree_.swap(target_kdtree_);
   }
-  bool calculateSourceCovariances() { return covariances(src_, &src_cov_ok_); }
-  bool calculateTargetCovariances() { return covariances(tgt_, &tgt_cov_ok_); }
-  CovVector getSourceCovariances() { return fetch_covs(src_, &src_cov_ok_); }
-  CovVector getTargetCovariances() { return fetch_covs(tgt_, &tgt_cov_ok_); }
+  bool calculateSourceCovariances() { return covariances(src_.get(), &src_cov_ok_); }
+  bool calculateTargetCovariances() { return covariances(tgt_.get(), &tgt_cov_ok_); }
+  CovVector getSourceCovariances() { return fetch_covs(src_.get(), &src_cov_ok_); }
+  CovVector getTargetCovariances() { return fetch_covs(tgt_.get(), &tgt_cov_ok_); }
   // nano_gicp.hpp:91-93, nano_gicp_impl.hpp:142-150: the caller's covariances replace the computed ones
-  void setSourceCovariances(const CovVector& covs) { push_covs(src_, covs, &src_cov_ok_); }
-  void setTargetCovariances(const CovVector& covs) { push_covs(tgt_, covs, &tgt_cov_ok_); }
+  void setSourceCovariances(const CovVector& covs) { push_covs(src_.get(), covs, &src_cov_ok_); }
+  void setTargetCovariances(const CovVector& covs) { push_covs(tgt_.get(), covs, &tgt_cov_ok_); }
   // lsq_registration.hpp:88: H of the last linearize (Identity before the first align)
   const Matrix6d& getFinalHessian() const { return final_hessian_; }
 
@@ -136,8 +144,8 @@ class NanoGICP {
     }
     double g[16];
     b200reg_host::to_rowmajor(guess, g);
-    b200reg_cloud* s[1] = {src_};
-    b200reg_cloud* t[1] = {tgt_};
+    b200reg_cloud* s[1] = {src_.get()};
+    b200reg_cloud* t[1] = {tgt_.get()};
     const int rc = b200reg_gicp_align(b200reg_host::context(), 1, s, t, g, &prm_, &res_);
     if (rc != 0) {
       std::fprintf(stderr, "b200reg: gicp_align failed (%d): %s\n", rc, b200reg_last_error());
@@ -151,7 +159,7 @@ class NanoGICP {
       for (int c = 0; c < 6; c++) final_hessian_(r, c) = res_.final_hessian[6 * r + c];
     // output = transformPointCloud(*input_, final_transformation_) (lsq_registration_impl.hpp:114): all fields kept
     std::vector<float> xyz(3 * input_->size());
-    b200reg_transform_cloud(b200reg_host::context(), src_, res_.Tf, xyz.data());
+    b200reg_transform_cloud(b200reg_host::context(), src_.get(), res_.Tf, xyz.data());
     output = *input_;
     for (size_t i = 0; i < output.size(); i++) {
       output.points[i].x = xyz[3 * i];
@@ -171,10 +179,10 @@ class NanoGICP {
   double getFitnessScore(double max_range = std::numeric_limits<double>::max()) {
     if (max_range == std::numeric_limits<double>::max()) return res_.fitness;
     std::vector<float> xyz(3 * input_->size());
-    b200reg_transform_cloud(b200reg_host::context(), src_, res_.Tf, xyz.data());
+    b200reg_transform_cloud(b200reg_host::context(), src_.get(), res_.Tf, xyz.data());
     std::vector<int32_t> idx(input_->size());
     std::vector<float> d2(input_->size());
-    b200reg_knn(b200reg_host::context(), tgt_, xyz.data(), input_->size(), 12, 1, idx.data(), d2.data());
+    b200reg_knn(b200reg_host::context(), tgt_.get(), xyz.data(), input_->size(), 12, 1, idx.data(), d2.data());
     double s = 0;
     size_t nr = 0;
     for (float v : d2)
@@ -187,22 +195,19 @@ class NanoGICP {
   int nr_iterations() const { return res_.iterations; }
   const b200reg_result& lastResult() const { return res_; }
 
+  // nano_gicp.hpp:121-122: search the clouds set by setInputSource / setInputTarget (radiusSearch takes a SQUARED radius)
+  std::shared_ptr<nanoflann::KdTreeFLANN<PointSource>> source_kdtree_;
+  std::shared_ptr<nanoflann::KdTreeFLANN<PointTarget>> target_kdtree_;
+
  private:
   template <typename CloudPtr>
-  void upload(const CloudPtr& cloud, b200reg_cloud** slot) {
+  void upload(const CloudPtr& cloud, b200reg_host::DeviceCloud* slot) {
     destroy(slot);
     if (!cloud || cloud->size() == 0) return;
     using P = typename std::remove_reference<decltype(cloud->points[0])>::type;
-    const float* xyz = reinterpret_cast<const float*>(cloud->points.data());
-    const float* ptrs[1] = {xyz};
-    const size_t ns[1] = {cloud->size()};
-    const int rc = b200reg_clouds_create(b200reg_host::context(), 1, ptrs, ns, sizeof(P), 0, slot);
-    if (rc != 0) std::fprintf(stderr, "b200reg: clouds_create failed (%d): %s\n", rc, b200reg_last_error());
+    *slot = b200reg_host::make_device_cloud(reinterpret_cast<const float*>(cloud->points.data()), cloud->size(), sizeof(P));
   }
-  void destroy(b200reg_cloud** slot) {
-    if (*slot) b200reg_cloud_destroy(b200reg_host::context(), *slot);
-    *slot = nullptr;
-  }
+  void destroy(b200reg_host::DeviceCloud* slot) { slot->reset(); }  // the device cloud goes when its last user (a tree) does
   void release() {
     destroy(&src_);
     destroy(&tgt_);
@@ -250,8 +255,7 @@ class NanoGICP {
   b200reg_result res_{};
   PointCloudSourceConstPtr input_;
   PointCloudTargetConstPtr target_;
-  b200reg_cloud* src_ = nullptr;
-  b200reg_cloud* tgt_ = nullptr;
+  b200reg_host::DeviceCloud src_, tgt_;
   bool src_cov_ok_ = false, tgt_cov_ok_ = false, converged_ = false;
   std::array<float, 16> final_;
   Matrix6d final_hessian_;

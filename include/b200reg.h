@@ -337,6 +337,22 @@ int b200reg_knn(b200reg_ctx* ctx, const b200reg_cloud* cloud, const float* queri
  * anchor the tree traversal is verified against at full size (100k x 100k).                               */
 int b200reg_knn_bruteforce(b200reg_ctx* ctx, const b200reg_cloud* cloud, const float* queries, size_t nq,
                            size_t qstride_bytes, int k, int32_t* idx_out, float* d2_out);
+/* Fixed-radius search: KdTreeFLANN::radiusSearch (nanoflann.hpp:154-175) for nq host queries at once, CSR output.
+ * !! sq_radius is a SQUARED radius, exactly as the reference takes it: radiusSearch hands its `radius` argument unchanged
+ * to RadiusResultSet<float, int> (nanoflann.hpp:162), which compares it with squared distances.  Passing 1.5 finds every
+ * point with d2 < 1.5f (strict; the double is converted to float first); a PCL user expecting r -> r*r gets a ball of
+ * radius sqrt(1.5).  d2 is the same fp32 expression as b200reg_knn's (((dx*dx) + dy*dy) + dz*dz, no FMA).
+ * Queries are (x, y, z [, ...]) records qstride_bytes apart (a multiple of 4, >= 12), 1 <= nq < 2^30.
+ * Results: the neighbours of query i are idx_out / d2_out [offsets_out[i], offsets_out[i+1]), offsets_out has nq + 1
+ * entries; indices refer to the cloud's ORIGINAL order.  sorted != 0: ascending (d2, index) (the reference sorts by d2 with
+ * ties unspecified); sorted == 0: ascending index (the reference returns its kd-tree's visit order, which no other index
+ * reproduces).  The result is deterministic: repeated calls return identical bytes.
+ * idx_out == d2_out == NULL: count only (offsets_out is filled).  If the total exceeds `capacity` (entries of each output)
+ * the call fills offsets_out, leaves idx_out / d2_out untouched and returns B200REG_ESTATE, the total in the message.
+ * Device memory is bounded: the queries are processed in chunks of ~8M neighbours (or one query, if it has more).   */
+int b200reg_radius_search(b200reg_ctx* ctx, const b200reg_cloud* cloud, const float* queries, size_t nq,
+                          size_t qstride_bytes, double sq_radius, int sorted, int64_t* offsets_out, size_t capacity,
+                          int32_t* idx_out, float* d2_out);
 /* normals (n x 3, NaN where fewer than 3 neighbours) and FPFH (n x 33), original point order.            */
 int b200reg_get_fpfh(b200reg_ctx* ctx, const b200reg_cloud* cloud, float* normals_out, float* fpfh_out);
 /* n x 9 doubles (row-major 3x3 block of the reference's Matrix4d), original point order.          */
