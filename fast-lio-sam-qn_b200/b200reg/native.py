@@ -377,6 +377,9 @@ class Context:
 
     # -- debug taps ----------------------------------------------------------------------
     def knn(self, cloud, queries, k, brute=False):
+        """KdTreeFLANN::nearestKSearch for every row of `queries` -> (idx (nq, k) int32, d2 (nq, k) float32), each row
+        ascending by (d2, original index); any k >= 1 (brute: 1..32).  Slots past the last neighbour hold -1 / FLT_MAX
+        (k > n, and every slot of a query with a NaN coordinate)."""
         q = _pts(queries)
         idx = np.empty((len(q), k), np.int32)
         d2 = np.empty((len(q), k), np.float32)

@@ -3,6 +3,7 @@
 #include <dlfcn.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
@@ -403,10 +404,15 @@ int b200reg_knn_bruteforce(b200reg_ctx* c, const b200reg_cloud* cl, const float*
   return knn_impl(c, cl, queries, nq, qstride_bytes, k, idx_out, d2_out, 1);
 }
 
+static int knn_large(b200reg_ctx* c, const b200reg_cloud* cl, const float* queries, size_t nq, size_t qstride_bytes, int k,
+                     int32_t* idx_out, float* d2_out);
+
 static int knn_impl(b200reg_ctx* c, const b200reg_cloud* cl, const float* queries, size_t nq, size_t qstride_bytes, int k,
                     int32_t* idx_out, float* d2_out, int brute) {
-  if (!c || !cl || !queries || nq == 0 || k <= 0 || k > 32 || !idx_out || !d2_out || qstride_bytes < 12 || qstride_bytes % 4)
-    return fail(B200REG_EINVAL, "bad argument (k must be 1..32)");
+  if (!c || !cl || !queries || nq == 0 || k <= 0 || !idx_out || !d2_out || qstride_bytes < 12 || qstride_bytes % 4)
+    return fail(B200REG_EINVAL, "bad argument (k must be >= 1, qstride_bytes a multiple of 4, >= 12)");
+  if (brute && k > 32) return fail(B200REG_EINVAL, "bad argument (the brute-force k-NN takes k in 1..32)");
+  if (k > 32) return knn_large(c, cl, queries, nq, qstride_bytes, k, idx_out, d2_out);
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Scratch scratch(c);
@@ -422,6 +428,57 @@ static int knn_impl(b200reg_ctx* c, const b200reg_cloud* cl, const float* querie
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(idx_out, d_idx, nq * k * 4, cudaMemcpyDeviceToHost, s));
   CU(cudaMemcpyAsync(d2_out, d_d2, nq * k * 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  return B200REG_OK;
+}
+
+// k > 32 (knn_large.cu).  The queries run in chunks of consecutive rows holding at most max(kKnnChunk, cloud size) result
+// entries (or one row, if k is larger), so the device copy of the output -- and, for lists longer than KL_SMEM_K, the
+// per-query slab -- stays bounded whatever nq * k is; each chunk's rows are copied to the caller's buffers.
+// k >= n: every point is a neighbour, and the sorted radius search with r2 = +inf lists exactly the points the kernel would
+// (d2 < +inf, ascending (d2, index)); its compact rows are spread to stride k and padded with (-1, FLT_MAX) here.
+static constexpr int64_t kKnnChunk = int64_t(1) << 23;
+
+static int knn_large(b200reg_ctx* c, const b200reg_cloud* cl, const float* queries, size_t nq, size_t qstride_bytes, int k,
+                     int32_t* idx_out, float* d2_out) {
+  const int n = cl->dev.n;
+  if (k >= n) {
+    std::vector<int64_t> off(nq + 1);
+    if (const int rc = b200reg_radius_search(c, cl, queries, nq, qstride_bytes, HUGE_VAL, 1, off.data(), nq * (size_t)k, idx_out,
+                                             d2_out))
+      return rc;
+    for (size_t i = nq; i-- > 0;) {  // last row first: row i's source [off[i], off[i+1]) lies at or below its target i * k
+      const size_t cnt = (size_t)(off[i + 1] - off[i]);
+      std::memmove(idx_out + i * k, idx_out + off[i], cnt * 4);
+      std::memmove(d2_out + i * k, d2_out + off[i], cnt * 4);
+      std::fill(idx_out + i * k + cnt, idx_out + (i + 1) * k, -1);
+      std::fill(d2_out + i * k + cnt, d2_out + (i + 1) * k, 3.402823466e+38f);
+    }
+    return B200REG_OK;
+  }
+  const int qs = (int)(qstride_bytes / 4);
+  const size_t rows = (size_t)std::max<int64_t>(1, std::max<int64_t>(kKnnChunk, n) / k);
+  CU(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  Scratch scratch(c);
+  ProfScope ps(c, CLS_MISC);
+  float* d_q = nullptr;
+  int* d_idx = nullptr;
+  float* d_d2 = nullptr;
+  unsigned long long* d_slab = nullptr;
+  const size_t cap = std::min(rows, nq) * (size_t)k;
+  CU(scratch.upload(&d_q, queries, nq * qstride_bytes));
+  CU(scratch.alloc((void**)&d_idx, cap * 4));
+  CU(scratch.alloc((void**)&d_d2, cap * 4));
+  if (k > KL_SMEM_K) CU(scratch.alloc((void**)&d_slab, cap * 8));
+  for (size_t r0 = 0; r0 < nq; r0 += rows) {
+    const size_t nr = std::min(rows, nq - r0);
+    c->launches += launch_knn_large(cl->dev, d_q + r0 * qs, (int)nr, qs, k, d_slab, d_idx, d_d2, s);
+    CU(cudaGetLastError());
+    c->prof_bytes[CLS_MISC] += 16.0 * nr + 8.0 * nr * k;
+    CU(cudaMemcpyAsync(idx_out + r0 * k, d_idx, nr * k * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(d2_out + r0 * k, d_d2, nr * k * 4, cudaMemcpyDeviceToHost, s));
+  }
   CU(cudaStreamSynchronize(s));
   return B200REG_OK;
 }

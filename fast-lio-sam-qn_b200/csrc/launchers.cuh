@@ -54,6 +54,12 @@ int launch_radius_fill(const CloudDev& c, const float* d_q, int qstride, const u
 int launch_radius_rekey(const uint32_t* perm, int m, const uint32_t* src, uint32_t* keys, cudaStream_t s);
 int launch_radius_gather(const uint32_t* perm, int m, const int* e_idx, const float* e_d2, int* idx_out, float* d2_out, cudaStream_t s);
 
+// knn_large.cu: exact k-NN for k > 32, one warp per query.  Lists of up to KL_SMEM_K entries live in shared memory; longer
+// ones need slab = nq * k keys of device scratch (unused otherwise)
+constexpr int KL_SMEM_K = 256;
+int launch_knn_large(const CloudDev& c, const float* d_q, int nq, int qstride, int k, unsigned long long* slab, int* idx, float* d2,
+                     cudaStream_t s);
+
 // assemble.cu
 void launch_pack_xyzi(const float* d_raw, int stride, int n, float4* d_out, cudaStream_t s);
 void launch_ingest_world(const float* d_raw, int stride, int n, const double* d_Tinv, float4* d_out, cudaStream_t s);

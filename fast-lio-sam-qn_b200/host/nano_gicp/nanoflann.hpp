@@ -14,8 +14,8 @@
 //     visit order, and sorts by d2 alone with ties in unspecified order;
 //   * setEpsilon is stored and not used: the reference prunes approximately with eps > 0 (nanoflann_impl.hpp:1408), the
 //     engine always returns the exact set, a superset of the reference's;
-//   * nearestKSearch takes k in 1..32 (larger fails loudly); k > n pads with index -1 and d2 FLT_MAX and returns n;
-//     equal distances resolve to the lower index;
+//   * nearestKSearch takes any k >= 1 and returns min(k, n); k > n pads with index -1 and d2 FLT_MAX; equal distances
+//     resolve to the lower index; a query with a NaN coordinate gets a row of padding;
 //   * Ptr / ConstPtr / IndicesPtr are std::shared_ptr (the reference uses boost::shared_ptr); the copy constructor (declared
 //     but not defined by the reference) shares the device index;
 //   * the calls are thread-safe (the reference's radiusSearch keeps its results in a function-local static vector).

@@ -329,12 +329,19 @@ int b200reg_allgather_results(b200reg_ctx* ctx, const b200reg_result* local, int
 int b200reg_transform_cloud(b200reg_ctx* ctx, const b200reg_cloud* cloud, const float* Tf16, float* out_xyz);
 
 /* ---- debug taps used by the parity tests ------------------------------------------- */
-/* exact k-NN of host queries in a cloud: KdTreeFLANN::nearestKSearch (nanoflann.hpp:140-152).
- * idx_out/d2_out: nq x k, ascending; indices refer to the ORIGINAL point order; -1 pads k > n.   */
+/* Exact k-NN of host queries in a cloud: KdTreeFLANN::nearestKSearch (nanoflann.hpp:140-152), any k >= 1.
+ * Queries are (x, y, z [, ...]) records qstride_bytes apart (a multiple of 4, >= 12), nq >= 1 (nq < 2^30 when k >= the
+ * cloud size).  idx_out / d2_out: nq x k, each row ascending by (d2, original index) -- equal distances resolve to the lower
+ * index; indices refer to the ORIGINAL point order; d2 is ((dx*dx) + dy*dy) + dz*dz in fp32 without FMA.  Slots past the
+ * last neighbour hold index -1 and d2 FLT_MAX: k > n, points whose d2 overflows to +inf (never neighbours), and every slot
+ * of a query with a NaN coordinate.  A row depends only on its query and the cloud: repeated calls, other batch sizes and
+ * other query orders return identical bytes.  k <= 32 runs one thread per query, k > 32 one warp per query with the
+ * queries in chunks, so device memory stays bounded (about 16 bytes per result entry of one chunk of max(2^23, cloud size)
+ * entries) whatever nq * k is.  k <= 0, NULL pointers and bad strides: B200REG_EINVAL.                                */
 int b200reg_knn(b200reg_ctx* ctx, const b200reg_cloud* cloud, const float* queries, size_t nq,
                 size_t qstride_bytes, int k, int32_t* idx_out, float* d2_out);
 /* Same answer by brute force (every point tested, tiles staged into shared memory by TMA bulk copies): the on-GPU
- * anchor the tree traversal is verified against at full size (100k x 100k).                               */
+ * anchor the tree traversal is verified against at full size (100k x 100k).  k in 1..32.                   */
 int b200reg_knn_bruteforce(b200reg_ctx* ctx, const b200reg_cloud* cloud, const float* queries, size_t nq,
                            size_t qstride_bytes, int k, int32_t* idx_out, float* d2_out);
 /* Fixed-radius search: KdTreeFLANN::radiusSearch (nanoflann.hpp:154-175) for nq host queries at once, CSR output.
