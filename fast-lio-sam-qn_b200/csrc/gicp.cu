@@ -474,7 +474,7 @@ __global__ void __launch_bounds__(STEP_THREADS, 16) k_gicp_search(const PairDev*
         res.p[0] = pp;
       }
     }
-    knn_search<1>(P.tgt, qx, qy, qz, res);
+    knn_walk(P.tgt, qx, qy, qz, res);
     P.sqd[i] = res.d[0];
     if (phase == PH_LINEARIZE) P.corr[i] = ((double)res.d[0] < max_corr_dist2) ? res.p[0] : -1;
   }
@@ -671,7 +671,7 @@ __global__ void __launch_bounds__(STEP_THREADS) k_knn_queries(CloudDev c, const 
   const float* qq = q + (size_t)i * qstride;
   KnnSet<K> res;
   res.init();
-  knn_search<K>(c, qq[0], qq[1], qq[2], res);
+  knn_walk(c, qq[0], qq[1], qq[2], res);
 #pragma unroll
   for (int j = 0; j < K; j++) {
     if (j < kout) {
@@ -729,7 +729,7 @@ __global__ void __launch_bounds__(STEP_THREADS) k_knn_brute(CloudDev c, const fl
       for (int j = 0; j < cnt; j++) {
         const float4 p = tile[t & 1][j];
         const float d2 = dist2_rn(qx, qy, qz, p.x, p.y, p.z);
-        if (!(d2 > res.worst())) knn_insert<K>(res, d2, t * BF_TILE + j, c.pts);
+        if (!(d2 > res.worst())) res.offer(d2, t * BF_TILE + j, c.pts);
       }
     }
     __syncthreads();

@@ -29,6 +29,26 @@ constexpr int FDIM = 33;           // FPFHSignature33
 constexpr int FPAD = 36;           // descriptor record padded to 144 B (9 x float4, TMA-bulk friendly)
 constexpr int MAX_STACK = 64;      // >= LBVH depth: 30 key bits + index tie-break bits
 
+// The tnodes record format above, in one place: leaf_ref encodes a leaf, leaf_span decodes it, load_node reads a record.
+__host__ __device__ __forceinline__ int leaf_ref(int start, int count) { return -1 - ((start << 4) | count); }
+
+struct LeafSpan {
+  int base, count;  // points [base, base + count) of the sorted cloud
+};
+__host__ __device__ __forceinline__ LeafSpan leaf_span(int ref) {
+  const int code = -1 - ref;
+  return {code >> 4, code & 15};
+}
+
+struct NodeRec {  // one 64-B record: the boxes and refs of both children of an internal node
+  float4 lo0, hi0, lo1, hi1;
+  __device__ __forceinline__ int ref0() const { return __float_as_int(lo0.w); }
+  __device__ __forceinline__ int ref1() const { return __float_as_int(lo1.w); }
+};
+__device__ __forceinline__ NodeRec load_node(const float4* __restrict__ tnodes, int ref) {
+  return {__ldg(&tnodes[4 * ref]), __ldg(&tnodes[4 * ref + 1]), __ldg(&tnodes[4 * ref + 2]), __ldg(&tnodes[4 * ref + 3])};
+}
+
 struct CloudDev {
   const float* raw;    // device copy of the caller's records (xyz at stride)
   int raw_stride;      // in floats
@@ -225,8 +245,6 @@ __device__ __forceinline__ int f2ord(float f) {
   return i >= 0 ? i : i ^ 0x7FFFFFFF;
 }
 __device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7FFFFFFF); }
-
-__host__ __device__ __forceinline__ int leaf_ref(int start, int count) { return -1 - ((start << 4) | count); }
 
 // 10 bits -> every third bit of 30 (one axis of a 30-bit Morton key: the index build's cells, radius.cu's query order)
 __device__ __forceinline__ uint32_t expand10(uint32_t v) {

@@ -30,6 +30,10 @@ __device__ __forceinline__ float box_dist2_rn(float qx, float qy, float qz, floa
   return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
 }
 
+__device__ __forceinline__ int orig_index(const float4* __restrict__ pts, int pos) {
+  return pos < 0 ? 0x7FFFFFFF : __float_as_int(__ldg(&pts[pos].w));
+}
+
 // Result set of K entries kept ascending in registers (fully unrolled; no dynamic indexing).
 template <int K>
 struct KnnSet {
@@ -43,7 +47,46 @@ struct KnnSet {
     }
   }
   __device__ __forceinline__ float worst() const { return d[K - 1]; }
-  __device__ __forceinline__ void offer(float cd, int cp, const float4* __restrict__ pts);  // candidate with cd <= worst()
+  // Insert a candidate with cd <= worst().  Hot path: strict '<' chain of branch-free selects; the candidate lands
+  // AFTER entries of equal distance.  Exact ties (measure ~0 on real data) are repaired by one unrolled upward bubble
+  // pass in a cold branch -- written without taking the address of the arrays, so that the result set provably stays
+  // in registers (an out-of-line repair taking pointers forced it into local memory: LDL/STL
+  // in the hot loop).  A candidate that ties with the current worst replaces it only if its original
+  // index is lower (the (d2, index) rule of SURVEY.md App. A.3).
+  __device__ __forceinline__ void offer(float cd, int cp, const float4* __restrict__ pts) {
+    bool tie = false;
+    if (cd == d[K - 1]) {  // ties with the worst entry: decide by original index
+      if (!(orig_index(pts, cp) < orig_index(pts, p[K - 1]))) return;
+      d[K - 1] = cd;
+      p[K - 1] = cp;
+      tie = true;
+    } else {
+      bool placed = false;  // once the candidate is in, everything below simply shifts down by one (a carried entry must
+                            // never leapfrog its equal-distance peers: it is the lowest index of its run)
+#pragma unroll
+      for (int j = 0; j < K; j++) {
+        const bool lt = placed || cd < d[j];
+        tie |= (!placed && cd == d[j]);
+        placed = lt;
+        const float td = d[j];
+        const int tp = p[j];
+        d[j] = lt ? cd : td;
+        p[j] = lt ? cp : tp;
+        cd = lt ? td : cd;
+        cp = lt ? tp : cp;
+      }
+    }
+    if (tie) {  // cold: the new entry sits below its equal-distance peers; bubble it up by original index
+#pragma unroll
+      for (int j = K - 1; j > 0; j--) {
+        if (d[j] == d[j - 1] && p[j] >= 0 && orig_index(pts, p[j]) < orig_index(pts, p[j - 1])) {
+          const int t = p[j];
+          p[j] = p[j - 1];
+          p[j - 1] = t;
+        }
+      }
+    }
+  }
   // distance of leaf slot j out of the register-resident dl[]: a select chain (no dynamic register indexing)
   __device__ __forceinline__ float leaf_distance(const float (&dl)[LEAF], int j, const float4* __restrict__, int, float, float, float) const {
     float dj = dl[0];
@@ -52,57 +95,6 @@ struct KnnSet {
     return dj;
   }
 };
-
-__device__ __forceinline__ int orig_index(const float4* __restrict__ pts, int pos) {
-  return pos < 0 ? 0x7FFFFFFF : __float_as_int(__ldg(&pts[pos].w));
-}
-
-// Insert a candidate with cd <= worst.  Hot path: strict '<' chain of branch-free selects; the candidate lands
-// AFTER entries of equal distance.  Exact ties (measure ~0 on real data) are repaired by one unrolled upward bubble
-// pass in a cold branch -- written without taking the address of the arrays, so that the result set provably stays
-// in registers (an out-of-line repair taking pointers forced it into local memory: LDL/STL
-// in the hot loop).  A candidate that ties with the current worst replaces it only if its original
-// index is lower (the (d2, index) rule of SURVEY.md App. A.3).
-template <int K>
-__device__ __forceinline__ void knn_insert(KnnSet<K>& s, float cd, int cp, const float4* __restrict__ pts) {
-  bool tie = false;
-  if (cd == s.d[K - 1]) {  // ties with the worst entry: decide by original index
-    if (!(orig_index(pts, cp) < orig_index(pts, s.p[K - 1]))) return;
-    s.d[K - 1] = cd;
-    s.p[K - 1] = cp;
-    tie = true;
-  } else {
-    bool placed = false;  // once the candidate is in, everything below simply shifts down by one (a carried entry must
-                          // never leapfrog its equal-distance peers: it is the lowest index of its run)
-#pragma unroll
-    for (int j = 0; j < K; j++) {
-      const bool lt = placed || cd < s.d[j];
-      tie |= (!placed && cd == s.d[j]);
-      placed = lt;
-      const float td = s.d[j];
-      const int tp = s.p[j];
-      s.d[j] = lt ? cd : td;
-      s.p[j] = lt ? cp : tp;
-      cd = lt ? td : cd;
-      cp = lt ? tp : cp;
-    }
-  }
-  if (tie) {  // cold: the new entry sits below its equal-distance peers; bubble it up by original index
-#pragma unroll
-    for (int j = K - 1; j > 0; j--) {
-      if (s.d[j] == s.d[j - 1] && s.p[j] >= 0 && orig_index(pts, s.p[j]) < orig_index(pts, s.p[j - 1])) {
-        const int t = s.p[j];
-        s.p[j] = s.p[j - 1];
-        s.p[j - 1] = t;
-      }
-    }
-  }
-}
-
-template <int K>
-__device__ __forceinline__ void KnnSet<K>::offer(float cd, int cp, const float4* __restrict__ pts) {
-  knn_insert<K>(*this, cd, cp, pts);
-}
 
 // The K best candidates as a binary MAX-heap in shared memory, one column per thread ([slot][thread]: the bank is the
 // thread, so the divergent, dynamically indexed accesses of a sift-down are conflict free).  For consumers that need the
@@ -219,12 +211,31 @@ struct KnnHeap {
   }
 };
 
+// One descent step of the best-first k-NN walks (knn_walk here, kl_walk in knn_large.cu): order record n's two children
+// by their box bound (child 1 first only if strictly nearer), hand the far child to push(ref, bound) unless its bound is
+// strictly greater than the current worst distance w, and move to the near child.  Returns false when the near child is
+// pruned as well.
+template <typename Push>
+__device__ __forceinline__ bool near_far_step(const NodeRec& n, float qx, float qy, float qz, float w, int& ref, float& dnode, Push&& push) {
+  const float d0 = box_dist2_rn(qx, qy, qz, n.lo0, n.hi0);
+  const float d1 = box_dist2_rn(qx, qy, qz, n.lo1, n.hi1);
+  int nref = n.ref0(), fref = n.ref1();
+  float nd = d0, fd = d1;
+  if (d1 < d0) {
+    nref = n.ref1(); fref = n.ref0(); nd = d1; fd = d0;
+  }
+  if (!(fd > w)) push(fref, fd);
+  ref = nref;
+  dnode = nd;
+  return !(nd > w);
+}
+
 // Exact K-NN of (qx,qy,qz) in cloud c.  One thread per query; Morton-sorted queries keep
 // neighbouring lanes on neighbouring paths (coherent loads, low divergence).
 template <typename Res>
 __device__ __forceinline__ void knn_walk(const CloudDev& c, float qx, float qy, float qz, Res& res, int skip_lo = 1, int skip_hi = 0) {
   const float4* __restrict__ pts = c.pts;
-  const float4* __restrict__ tn = c.tnodes;
+  const float4* __restrict__ tn = c.tnodes;  // read once: c may be a reference into global memory (clouds[blockIdx.y])
   int stack_ref[MAX_STACK];
   float stack_d[MAX_STACK];
   int sp = 0;
@@ -232,29 +243,15 @@ __device__ __forceinline__ void knn_walk(const CloudDev& c, float qx, float qy, 
   float dnode = 0.f;
   for (;;) {
     bool alive = !(dnode > res.worst());
-    while (alive && ref >= 0) {  // internal node: both children's boxes live in one 64-B record
-      const float4 a0 = __ldg(&tn[4 * ref]), a1 = __ldg(&tn[4 * ref + 1]);
-      const float4 b0 = __ldg(&tn[4 * ref + 2]), b1 = __ldg(&tn[4 * ref + 3]);
-      const float d0 = box_dist2_rn(qx, qy, qz, a0, a1);
-      const float d1 = box_dist2_rn(qx, qy, qz, b0, b1);
-      int nref = __float_as_int(a0.w), fref = __float_as_int(b0.w);
-      float nd = d0, fd = d1;
-      if (d1 < d0) {
-        nref = __float_as_int(b0.w); fref = __float_as_int(a0.w); nd = d1; fd = d0;
-      }
-      const float w = res.worst();
-      if (!(fd > w)) {
-        stack_ref[sp] = fref;
-        stack_d[sp] = fd;
+    while (alive && ref >= 0)  // internal node: both children's boxes live in one 64-B record
+      alive = near_far_step(load_node(tn, ref), qx, qy, qz, res.worst(), ref, dnode, [&](int r, float d) {
+        stack_ref[sp] = r;
+        stack_d[sp] = d;
         sp++;
-      }
-      ref = nref;
-      dnode = nd;
-      alive = !(nd > w);
-    }
+      });
     if (alive) {  // leaf: up to LEAF consecutive points
-      const int code = -1 - ref;
-      const int base = code >> 4, cnt = code & 15;
+      const LeafSpan leaf = leaf_span(ref);
+      const int base = leaf.base, cnt = leaf.count;
       float dl[LEAF];
       unsigned mask = 0;
       const float w0 = res.worst();
@@ -286,76 +283,65 @@ __device__ __forceinline__ void knn_walk(const CloudDev& c, float qx, float qy, 
   }
 }
 
-template <int K>
-__device__ __forceinline__ void knn_search(const CloudDev& c, float qx, float qy, float qz, KnnSet<K>& res, int skip_lo = 1,
-                                           int skip_hi = 0) {
-  knn_walk<KnnSet<K>>(c, qx, qy, qz, res, skip_lo, skip_hi);
-}
-
-// Fixed-radius traversal: calls f(position, d2) for every point with fp32 d2 < r2 (strict, like FLANN's
-// RadiusResultSet).  A subtree is skipped when its box bound >= r2: every point inside is then >= r2 too.
-template <typename F>
-__device__ __forceinline__ void radius_visit(const CloudDev& c, float qx, float qy, float qz, float r2, F&& f) {
-  const float4* __restrict__ pts = c.pts;
-  const float4* __restrict__ tn = c.tnodes;
-  int stack_ref[MAX_STACK];
+// Fixed-radius search with a WARP-SHARED traversal and deferred, lockstep processing of the hits.
+// Why per warp (profiles/README.md): with the callback inside a per-thread traversal the SPFH kernel ran with 4.75 of 32
+// lanes active; collecting hits per thread and processing them warp-convergently brought that to 12.7, but the SASS
+// profile still had half of all instructions in the private traversals at 4-7 active lanes (lanes fill their buffers at
+// different rates and wait; a bigger buffer cost more occupancy than it won).  The 32 queries of a warp are
+// Morton-neighbours, so their balls overlap almost completely; the warp therefore walks the tree once.
+//
+// radius_descend_warp is that one walk: a node is entered if ANY active lane's own exact box test passes (box bound
+// < r2; a subtree whose bound is >= r2 holds no point with d2 < r2, so no lane misses anything), the stack is
+// warp-uniform, and leaf(base, count) runs warp-uniformly for every leaf reached.  Control flow is warp-uniform
+// throughout; the order of the leaves is deterministic for a given cloud.
+// Must be called by every thread of the warp.  wstack: MAX_STACK ints private to the warp.
+template <typename L>
+__device__ __forceinline__ void radius_descend_warp(const CloudDev& c, bool active, float qx, float qy, float qz, float r2, int* wstack,
+                                                    L&& leaf) {
+  const float4* __restrict__ tn = c.tnodes;  // read once, as in knn_walk
+  constexpr unsigned FULL = 0xffffffffu;
   int sp = 0;
   int ref = c.root_ref;
   for (;;) {
     while (ref >= 0) {
-      const float4 a0 = __ldg(&tn[4 * ref]), a1 = __ldg(&tn[4 * ref + 1]);
-      const float4 b0 = __ldg(&tn[4 * ref + 2]), b1 = __ldg(&tn[4 * ref + 3]);
-      const bool in0 = box_dist2_rn(qx, qy, qz, a0, a1) < r2;
-      const bool in1 = box_dist2_rn(qx, qy, qz, b0, b1) < r2;
-      const int r0 = __float_as_int(a0.w), r1 = __float_as_int(b0.w);
+      const NodeRec n = load_node(tn, ref);
+      const bool in0 = __any_sync(FULL, active && box_dist2_rn(qx, qy, qz, n.lo0, n.hi0) < r2);
+      const bool in1 = __any_sync(FULL, active && box_dist2_rn(qx, qy, qz, n.lo1, n.hi1) < r2);
       if (in0 && in1) {
-        stack_ref[sp++] = r1;
-        ref = r0;
+        wstack[sp++] = n.ref1();  // every lane writes the same value
+        ref = n.ref0();
       } else if (in0) {
-        ref = r0;
+        ref = n.ref0();
       } else if (in1) {
-        ref = r1;
+        ref = n.ref1();
       } else {
         ref = 0x7FFFFFFF;  // dead end
         break;
       }
     }
     if (ref < 0) {
-      const int code = -1 - ref;
-      const int base = code >> 4, cnt = code & 15;
-      for (int j = 0; j < cnt; j++) {
-        const float4 p = __ldg(&pts[base + j]);
-        const float d2 = dist2_rn(qx, qy, qz, p.x, p.y, p.z);
-        if (d2 < r2) f(base + j, d2, p);
-      }
+      const LeafSpan s = leaf_span(ref);
+      leaf(s.base, s.count);
     }
     if (sp == 0) break;
-    ref = stack_ref[--sp];
+    __syncwarp();  // the pushes of this round are visible to every lane ...
+    ref = wstack[--sp];
+    __syncwarp();  // ... and every lane has popped before the slot can be pushed again
   }
 }
 
-// Fixed-radius search with a WARP-SHARED traversal and deferred, lockstep processing of the hits.
-// History (profiles/README.md): with the callback inside a per-thread traversal (radius_visit) the SPFH kernel ran with
-// 4.75 of 32 lanes active; collecting hits per thread and processing them warp-convergently brought that to 12.7, but
-// the SASS profile still had half of all instructions in the private traversals at 4-7 active lanes (lanes fill their
-// buffers at different rates and wait; a bigger buffer cost more occupancy than it won).  The 32 queries of a warp
-// are Morton-neighbours, so their balls overlap almost completely; the warp therefore walks the tree once: a node is entered if
-// ANY lane's own exact box test passes (the same per-lane criterion as radius_visit, so nothing is missed), the
-// stack is warp-uniform, every lane tests every point of a visited leaf against its own query and collects its own
-// hits, and whenever some lane's buffer could overflow the whole warp processes what it has collected, in lockstep.
-// Control flow is warp-uniform throughout.  Each lane still receives exactly its own neighbour set; the ORDER is that
-// of the warp's walk (deterministic for a given cloud).
+// The shared walk with PER-LANE hit lists: every lane tests every point of a visited leaf against its own query and
+// collects its own hits, and whenever some lane's buffer could overflow the whole warp processes what it has collected,
+// in lockstep: f(position, d2) on the owner lane, in the order of the warp's walk.  Each lane receives exactly its own
+// neighbour set in a fixed order (k_fpfh's fp32 sums depend on it).
 // Must be called by every thread of the warp.  spos (and sd2 unless nullptr): [BUF][blockDim.x]; wstack: MAX_STACK
 // ints private to the warp.
 template <int BUF, typename F>
 __device__ __forceinline__ void radius_visit_warp(const CloudDev& c, bool active, float qx, float qy, float qz, float r2, int* spos,
                                                   float* sd2, int* wstack, F&& f) {
   const float4* __restrict__ pts = c.pts;
-  const float4* __restrict__ tn = c.tnodes;
   const int tid = threadIdx.x, stride = blockDim.x;
   constexpr unsigned FULL = 0xffffffffu;
-  int sp = 0;
-  int ref = c.root_ref;
   int cnt = 0;
   auto flush = [&]() {
     const int most = __reduce_max_sync(FULL, cnt);
@@ -364,48 +350,22 @@ __device__ __forceinline__ void radius_visit_warp(const CloudDev& c, bool active
     cnt = 0;
   };
   if (!__any_sync(FULL, active)) return;
-  for (;;) {
-    while (ref >= 0) {
-      const float4 a0 = __ldg(&tn[4 * ref]), a1 = __ldg(&tn[4 * ref + 1]);
-      const float4 b0 = __ldg(&tn[4 * ref + 2]), b1 = __ldg(&tn[4 * ref + 3]);
-      const bool in0 = __any_sync(FULL, active && box_dist2_rn(qx, qy, qz, a0, a1) < r2);
-      const bool in1 = __any_sync(FULL, active && box_dist2_rn(qx, qy, qz, b0, b1) < r2);
-      const int r0 = __float_as_int(a0.w), r1 = __float_as_int(b0.w);
-      if (in0 && in1) {
-        wstack[sp++] = r1;  // every lane writes the same value
-        ref = r0;
-      } else if (in0) {
-        ref = r0;
-      } else if (in1) {
-        ref = r1;
-      } else {
-        ref = 0x7FFFFFFF;  // dead end
-        break;
+  radius_descend_warp(c, active, qx, qy, qz, r2, wstack, [&](int base, int n) {
+    for (int j = 0; j < n; j++) {
+      const float4 p = __ldg(&pts[base + j]);
+      const float d2 = dist2_rn(qx, qy, qz, p.x, p.y, p.z);
+      if (active && d2 < r2) {
+        spos[cnt * stride + tid] = base + j;
+        if (sd2) sd2[cnt * stride + tid] = d2;
+        cnt++;
       }
     }
-    if (ref < 0) {
-      const int code = -1 - ref;
-      const int base = code >> 4, n = code & 15;
-      for (int j = 0; j < n; j++) {
-        const float4 p = __ldg(&pts[base + j]);
-        const float d2 = dist2_rn(qx, qy, qz, p.x, p.y, p.z);
-        if (active && d2 < r2) {
-          spos[cnt * stride + tid] = base + j;
-          if (sd2) sd2[cnt * stride + tid] = d2;
-          cnt++;
-        }
-      }
-      if (__any_sync(FULL, cnt > BUF - LEAF)) flush();
-    }
-    if (sp == 0) break;
-    __syncwarp();  // the pushes of this round are visible to every lane ...
-    ref = wstack[--sp];
-    __syncwarp();  // ... and every lane has popped before the slot can be pushed again
-  }
+    if (__any_sync(FULL, cnt > BUF - LEAF)) flush();
+  });
   flush();
 }
 
-// The same warp-shared walk, with the hits of all 32 queries POOLED in one per-warp ring and processed 32 at a time by
+// The shared walk with the hits of all 32 queries POOLED in one per-warp ring and processed 32 at a time by
 // whichever lane is free: f(owner_lane, position) runs for entry e on lane e.  For per-pair work whose result is
 // order-independent (integer histograms in shared memory) this keeps every lane busy -- with per-lane hit lists the
 // lockstep processing leaves lanes idle (the lanes of a warp fill their lists at different rates).
@@ -416,12 +376,9 @@ template <typename H, typename F>
 __device__ __forceinline__ void radius_visit_warp_pooled(const CloudDev& c, bool active, float qx, float qy, float qz, float r2,
                                                          unsigned* ring, int* wstack, H&& on_hit, F&& f) {
   const float4* __restrict__ pts = c.pts;
-  const float4* __restrict__ tn = c.tnodes;
   constexpr unsigned FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const unsigned lt = (1u << lane) - 1u;
-  int sp = 0;
-  int ref = c.root_ref;
   int head = 0, tail = 0;  // warp-uniform: entries [head, tail) of the ring are pending
   auto process = [&](int take) {
     if (lane < take) {
@@ -432,48 +389,22 @@ __device__ __forceinline__ void radius_visit_warp_pooled(const CloudDev& c, bool
     __syncwarp();
   };
   if (!__any_sync(FULL, active)) return;
-  for (;;) {
-    while (ref >= 0) {
-      const float4 a0 = __ldg(&tn[4 * ref]), a1 = __ldg(&tn[4 * ref + 1]);
-      const float4 b0 = __ldg(&tn[4 * ref + 2]), b1 = __ldg(&tn[4 * ref + 3]);
-      const bool in0 = __any_sync(FULL, active && box_dist2_rn(qx, qy, qz, a0, a1) < r2);
-      const bool in1 = __any_sync(FULL, active && box_dist2_rn(qx, qy, qz, b0, b1) < r2);
-      const int r0 = __float_as_int(a0.w), r1 = __float_as_int(b0.w);
-      if (in0 && in1) {
-        wstack[sp++] = r1;  // every lane writes the same value
-        ref = r0;
-      } else if (in0) {
-        ref = r0;
-      } else if (in1) {
-        ref = r1;
-      } else {
-        ref = 0x7FFFFFFF;  // dead end
-        break;
+  radius_descend_warp(c, active, qx, qy, qz, r2, wstack, [&](int base, int n) {
+    for (int j = 0; j < n; j++) {
+      const float4 p = __ldg(&pts[base + j]);
+      const bool hit = active && dist2_rn(qx, qy, qz, p.x, p.y, p.z) < r2;
+      const unsigned m = __ballot_sync(FULL, hit);
+      if (hit) {
+        ring[(tail + __popc(m & lt)) & (RV_RING - 1)] = ((unsigned)(base + j) << 5) | (unsigned)lane;
+        on_hit(base + j);
+      }
+      tail += __popc(m);
+      if (tail - head >= 32) {  // at most 31 + 32 pending: the ring never overflows
+        __syncwarp();
+        process(32);
       }
     }
-    if (ref < 0) {
-      const int code = -1 - ref;
-      const int base = code >> 4, n = code & 15;
-      for (int j = 0; j < n; j++) {
-        const float4 p = __ldg(&pts[base + j]);
-        const bool hit = active && dist2_rn(qx, qy, qz, p.x, p.y, p.z) < r2;
-        const unsigned m = __ballot_sync(FULL, hit);
-        if (hit) {
-          ring[(tail + __popc(m & lt)) & (RV_RING - 1)] = ((unsigned)(base + j) << 5) | (unsigned)lane;
-          on_hit(base + j);
-        }
-        tail += __popc(m);
-        if (tail - head >= 32) {  // at most 31 + 32 pending: the ring never overflows
-          __syncwarp();
-          process(32);
-        }
-      }
-    }
-    if (sp == 0) break;
-    __syncwarp();  // the pushes of this round are visible to every lane ...
-    ref = wstack[--sp];
-    __syncwarp();  // ... and every lane has popped before the slot can be pushed again
-  }
+  });
   __syncwarp();
   if (tail > head) process(tail - head);
 }

@@ -117,21 +117,7 @@ __device__ __forceinline__ void kl_walk(const CloudDev& c, float qx, float qy, f
   float dnode = 0.f;
   for (;;) {
     bool alive = !(dnode > wd);
-    while (alive && ref >= 0) {  // internal record: both children's boxes
-      const float4 a0 = __ldg(&tn[4 * ref]), a1 = __ldg(&tn[4 * ref + 1]);
-      const float4 b0 = __ldg(&tn[4 * ref + 2]), b1 = __ldg(&tn[4 * ref + 3]);
-      const float d0 = box_dist2_rn(qx, qy, qz, a0, a1);
-      const float d1 = box_dist2_rn(qx, qy, qz, b0, b1);
-      int nref = __float_as_int(a0.w), fref = __float_as_int(b0.w);
-      float nd = d0, fd = d1;
-      if (d1 < d0) {
-        nref = __float_as_int(b0.w); fref = __float_as_int(a0.w); nd = d1; fd = d0;
-      }
-      if (!(fd > wd)) push(fref, fd);
-      ref = nref;
-      dnode = nd;
-      alive = !(nd > wd);
-    }
+    while (alive && ref >= 0) alive = near_far_step(load_node(tn, ref), qx, qy, qz, wd, ref, dnode, push);
     if (alive) {  // leaf step: this leaf and up to three more from the top of the stack
       int l1 = 0, l2 = 0, l3 = 0, nl = 1;
       while (nl < 4 && sp > 0) {
@@ -149,8 +135,8 @@ __device__ __forceinline__ void kl_walk(const CloudDev& c, float qx, float qy, f
         nl++;
       }
       const int t = lane >> 3, j = lane & 7;
-      const int code = -1 - (t == 0 ? ref : t == 1 ? l1 : t == 2 ? l2 : l3);
-      const int base = code >> 4, cnt = code & 15;
+      const LeafSpan leaf = leaf_span(t == 0 ? ref : t == 1 ? l1 : t == 2 ? l2 : l3);
+      const int base = leaf.base, cnt = leaf.count;
       unsigned long long key = 0;
       bool take = false;
       if (t < nl && j < cnt) {

@@ -26,7 +26,7 @@ namespace b200 {
 // ------------------------------------------------------------------------------------------------
 // Q1 normals
 // ------------------------------------------------------------------------------------------------
-constexpr int RV_BUF = 16;     // deferred-neighbour buffer per thread (radius_visit_batched), positions only
+constexpr int RV_BUF = 16;     // per-lane hit buffer of the warp-shared walk (radius_visit_warp), positions only
 constexpr int RV_BUF_D2 = 16;  // ... when the distance travels with the position (k_fpfh)
 
 __global__ void __launch_bounds__(STEP_THREADS) k_normals(const CloudDev* clouds, float r2) {

@@ -28,9 +28,9 @@ __global__ void __launch_bounds__(256) k_rs_query_keys(CloudDev c, const float* 
   if (i >= nq) return;
   uint32_t key = 0;
   if (c.n > LEAF) {  // the root record holds both children's boxes: their union is the cloud's bounding box
-    const float4 a0 = __ldg(&c.tnodes[0]), a1 = __ldg(&c.tnodes[1]), b0 = __ldg(&c.tnodes[2]), b1 = __ldg(&c.tnodes[3]);
-    const float lo0 = fminf(a0.x, b0.x), lo1 = fminf(a0.y, b0.y), lo2 = fminf(a0.z, b0.z);
-    const float ext = fmaxf(fmaxf(fmaxf(a1.x, b1.x) - lo0, fmaxf(a1.y, b1.y) - lo1), fmaxf(a1.z, b1.z) - lo2);
+    const NodeRec root = load_node(c.tnodes, 0);
+    const float lo0 = fminf(root.lo0.x, root.lo1.x), lo1 = fminf(root.lo0.y, root.lo1.y), lo2 = fminf(root.lo0.z, root.lo1.z);
+    const float ext = fmaxf(fmaxf(fmaxf(root.hi0.x, root.hi1.x) - lo0, fmaxf(root.hi0.y, root.hi1.y) - lo1), fmaxf(root.hi0.z, root.hi1.z) - lo2);
     const float scale = ext > 0.f ? 1023.0f / ext : 0.f;  // cubic cells, as k_morton_ghist quantises the cloud itself
     const float* p = q + (size_t)i * qstride;
     const uint32_t q0 = (uint32_t)min(max((int)((p[0] - lo0) * scale), 0), 1023);
