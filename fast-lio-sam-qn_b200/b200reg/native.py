@@ -81,7 +81,7 @@ EXPORTS = [
     "b200reg_batch_create", "b200reg_batch_destroy", "b200reg_batch_submit_icp", "b200reg_batch_submit_loop_closure",
     "b200reg_batch_wait", "b200reg_batch_wait_all", "b200reg_batch_launch_count", "b200reg_batch_depth",
     "b200reg_comm_unique_id", "b200reg_comm_init", "b200reg_comm_destroy", "b200reg_comm_rank", "b200reg_comm_world",
-    "b200reg_allgather_results", "b200reg_radius_search",
+    "b200reg_allgather_results", "b200reg_radius_search", "b200reg_quatro_align_ex", "b200reg_quatro_solve_tap",
 ]
 ESTATE = -4  # B200REG_ESTATE
 
@@ -328,19 +328,25 @@ class Context:
         return nrm, f
 
     def quatro_align(self, srcs, dsts, params=None, want_corr=False):
-        """quatro<T>::align for a batch of cloud handles."""
+        """quatro<T>::align for a batch of cloud handles.  want_corr: each info also holds "corr", the (n_corr, 2) final
+        (src, dst) correspondences (any number: advancedMatching sets beyond ADV_MAXC included)."""
         cnt = len(srcs)
         prm = params or default_quatro_params()
         sa = (C.c_void_p * cnt)(*[c.h for c in srcs])
         da = (C.c_void_p * cnt)(*[c.h for c in dsts])
         info = (QuatroInfo * cnt)()
-        corr = np.zeros((cnt, MAXC if prm.use_optimized_matching else ADV_MAXC, 2), np.int32) if want_corr else None
-        _check(lib().b200reg_quatro_align(self.h, cnt, sa, da, C.byref(prm), info,
-                                          None if corr is None else corr.ctypes.data_as(C.c_void_p)))
+        if not want_corr:
+            _check(lib().b200reg_quatro_align(self.h, cnt, sa, da, C.byref(prm), info, None))
+            return [i.as_dict() for i in info]
+        # enough for any answer: optimizedMatching keeps at most MAXC pairs, advancedMatching's pairs are one-to-one
+        cap = sum(MAXC if prm.use_optimized_matching else min(s.n, d.n) for s, d in zip(srcs, dsts))
+        offsets = np.empty(cnt + 1, np.int64)
+        corr = np.empty((max(cap, 1), 2), np.int32)
+        _check(lib().b200reg_quatro_align_ex(self.h, cnt, sa, da, C.byref(prm), info, offsets.ctypes.data_as(C.c_void_p),
+                                             C.c_size_t(cap), corr.ctypes.data_as(C.c_void_p)))
         out = [i.as_dict() for i in info]
-        if want_corr:
-            for o, cc in zip(out, corr):
-                o["corr"] = cc[:o["n_corr"]].copy()
+        for k, o in enumerate(out):
+            o["corr"] = corr[offsets[k]:offsets[k + 1]].copy()
         return out
 
     def loop_closure(self, src_arrays, tgt_arrays, qparams=None, gparams=None):
@@ -409,6 +415,21 @@ class Context:
         _check(rc)
         total = int(offsets[-1])
         return offsets, idx[:total], d2[:total]
+
+    def quatro_solve_tap(self, src_xyz, dst_xyz, params=None, wide=False):
+        """The TEASER++ solve of the advancedMatching path on given correspondences (row i of src_xyz joined to row i of
+        dst_xyz) -> info dict with "clique" (ascending correspondence indices).  wide: the path of sets beyond ADV_MAXC."""
+        S = np.ascontiguousarray(np.asarray(src_xyz)[:, :3], np.float32)
+        D = np.ascontiguousarray(np.asarray(dst_xyz)[:, :3], np.float32)
+        assert S.shape == D.shape
+        prm = params or default_quatro_params()
+        info = QuatroInfo()
+        clique = np.empty(len(S), np.int32)
+        _check(lib().b200reg_quatro_solve_tap(self.h, len(S), S.ctypes.data_as(C.c_void_p), D.ctypes.data_as(C.c_void_p),
+                                              int(bool(wide)), C.byref(prm), C.byref(info), clique.ctypes.data_as(C.c_void_p)))
+        out = info.as_dict()
+        out["clique"] = clique[:out["clique_size"]].copy()
+        return out
 
     def get_covariances(self, cloud):
         out = np.empty((cloud.n, 3, 3), np.float64)

@@ -211,18 +211,21 @@ struct MatchDev {
 };
 
 // Global-memory workspace of the multi-kernel TEASER++ solve used when the correspondence set is not capped at MAXC
-// (Matcher::advancedMatching, matcher.cc:118-356).  cap is a multiple of 1024, words = cap / 32.
+// (Matcher::advancedMatching, matcher.cc:118-356).  cap is a multiple of 1024, words = cap / 32, p2 = the power of two
+// >= cap (the bitonic sorts' length).  big_ws_layout (api_quatro.cu) is the one place that sizes it.
 struct BigSolveWs {
-  int cap, words;
+  int cap, words, p2;
   double* S;                 // [cap * 3] source points of the correspondences
   double* D;                 // [cap * 3]
   unsigned* adj;             // [cap * words] TIM consistency graph, bit j of row i
   unsigned* radj;            // [cap * words] same graph with vertices renamed by their rank in the clique order
   int *deg, *pdeg, *core, *alive, *rank, *order, *csize, *clique, *list;  // [cap] each
-  unsigned long long* skey;  // [cap]
+  unsigned long long* skey;  // [p2]
   double *w, *res;           // [cap]
-  double* hval;              // [2 * cap]
-  int* hidx;                 // [2 * cap]
+  double* hval;              // [2 * p2]
+  int* hidx;                 // [2 * p2]
+  unsigned long long* best;  // [1] best (clique size, rank) key found so far by k_big_greedy_wide
+  int* slot;                 // [source cloud size] k_adv_select_wide's scatter (sets beyond BIGC only, else nullptr)
 };
 
 struct QuatroParamsDev {
@@ -237,7 +240,9 @@ struct QuatroParamsDev {
 };
 
 constexpr int MAXC = 512;  // capacity of the final correspondence set (max_corres + 3 <= MAXC)
-constexpr int BIGC = 8192; // capacity of the advancedMatching correspondence set (B200REG_ADV_CORR_CAPACITY)
+constexpr int BIGC = 8192; // largest advancedMatching set solved per pair in one batched pass (B200REG_ADV_CORR_CAPACITY);
+                           // larger sets are solved one pair at a time in a workspace sized for them
+constexpr int BIG_NMAX = 1 << 20;  // sets must stay below this: k_big_core packs vertex indices into 20 bits
 
 // ---- ordered-int encoding of floats for atomicMin/atomicMax ------------------------
 __device__ __forceinline__ int f2ord(float f) {

@@ -30,6 +30,8 @@ void launch_transform_out(const CloudDev& c, const float* d_Tf, float* d_out3, c
 cudaError_t quatro_init_device();
 int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2, float fpfh_r2, cudaStream_t s);
 int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, int max_nj, const QuatroParamsDev& prm, cudaStream_t s);
+int launch_adv_wide(const MatchDev* d_pair, int n, const QuatroParamsDev& prm, cudaStream_t s);
+int launch_big_graph_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, int n_wide, cudaStream_t s);
 void launch_transform_raw(const CloudDev* d_clouds, const double* d_T16s, int count, int max_n, float4* const* d_outs, cudaStream_t s);
 
 // radius.cu: the stages of b200reg_radius_search (order, count, scan, fill, segmented sort); each returns its launches

@@ -1292,6 +1292,73 @@ __global__ void __launch_bounds__(1024) k_adv_select(const MatchDev* pairs, Quat
   if (threadIdx.x == 0) P.counters[2] = total;
 }
 
+// ordered compaction by one block of 1024 threads: emit(pos, v) for every v < n with keep(v), pos ascending with v.
+// Returns the number kept (to every thread).
+template <class Keep, class Emit>
+__device__ int block_compact(int n, Keep keep, Emit emit) {
+  __shared__ int wsum[32];
+  __shared__ int carry;
+  const int tid = threadIdx.x;
+  if (tid == 0) carry = 0;
+  __syncthreads();
+  for (int base = 0; base < n; base += 1024) {
+    const int v = base + tid;
+    const int k = (v < n && keep(v)) ? 1 : 0;
+    int incl = k;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, incl, o);
+      if ((tid & 31) >= o) incl += t;
+    }
+    if ((tid & 31) == 31) wsum[tid >> 5] = incl;
+    __syncthreads();
+    if (tid < 32) {
+      const int w = wsum[tid];
+      int wi = w;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, wi, o);
+        if (tid >= o) wi += t;
+      }
+      wsum[tid] = wi - w;
+    }
+    __syncthreads();
+    const int pos = carry + wsum[tid >> 5] + incl - k;
+    if (k) emit(pos, v);
+    __syncthreads();
+    if (tid == 1023) carry = pos + k;
+    __syncthreads();
+  }
+  return carry;
+}
+
+// k_adv_select for a set larger than BIGC (one pair, one block; W.slot holds a source cloud's worth of ints).  The
+// cross-checked pairs are one-to-one: (i, j) is kept only if j = rnn[i], so no fi point appears twice, and no fj point
+// either (k_mutual lists each j once).  Hence the (src, dst) order is the order of src alone: scatter dst by src and
+// compact in source-index order.  Same list as k_adv_select's sort, for any size.
+__global__ void __launch_bounds__(1024) k_adv_select_wide(const MatchDev* pairs, QuatroParamsDev prm) {
+  const MatchDev& P = pairs[blockIdx.x];
+  const BigSolveWs& W = *P.big;
+  const int ncorr = P.counters[1];
+  const int nsrc = P.swapped ? P.fj.n : P.fi.n;
+  const bool keepall = prm.tuple_scale == 0.f;
+  for (int v = threadIdx.x; v < nsrc; v += 1024) W.slot[v] = -1;
+  __syncthreads();
+  for (int r = threadIdx.x; r < ncorr; r += 1024) {
+    if (!keepall && P.tkey[r] == 0xFFFFFFFFu) continue;
+    const int i = P.corres[2 * r], j = P.corres[2 * r + 1];
+    W.slot[P.swapped ? j : i] = P.swapped ? i : j;
+  }
+  __syncthreads();
+  const int total = block_compact(
+      nsrc, [&](int v) { return W.slot[v] >= 0; },
+      [&](int pos, int v) {
+        P.out_corr[2 * pos] = v;
+        P.out_corr[2 * pos + 1] = W.slot[v];
+      });
+  if (threadIdx.x == 0) P.counters[2] = total;
+}
+
 __global__ void __launch_bounds__(256) k_big_gather(const MatchDev* pairs) {
   const MatchDev& P = pairs[blockIdx.y];
   const BigSolveWs& W = *P.big;
@@ -1387,8 +1454,8 @@ __global__ void __launch_bounds__(1024) k_big_core(const MatchDev* pairs) {
       }
     __syncthreads();
     const int f = nf;
-    for (int idx = tid; idx < f * wn; idx += 1024) {
-      const int fv = W.list[idx / wn], w = idx % wn;
+    for (long long idx = tid; idx < (long long)f * wn; idx += 1024) {
+      const int fv = W.list[idx / wn], w = (int)(idx % wn);
       unsigned bits = W.adj[(size_t)fv * W.words + w];
       while (bits) {
         const int u = w * 32 + __ffs(bits) - 1;
@@ -1399,11 +1466,13 @@ __global__ void __launch_bounds__(1024) k_big_core(const MatchDev* pairs) {
     __syncthreads();
     remaining -= f;
   }
+  // core and degree are at most n - 1 and i < n < 2^20 (BIG_NMAX), so each field fits its bits
   int n2 = 2;
   while (n2 < n) n2 <<= 1;
   for (int i = tid; i < n2; i += 1024)
-    W.skey[i] = i < n ? (((unsigned long long)(BIGC - W.core[i]) << 40) | ((unsigned long long)(BIGC - W.deg[i]) << 20) | (unsigned)i)
+    W.skey[i] = i < n ? (((unsigned long long)(n - W.core[i]) << 40) | ((unsigned long long)(n - W.deg[i]) << 20) | (unsigned)i)
                       : 0xFFFFFFFFFFFFFFFFull;
+  if (tid == 0) *W.best = 0;
   __syncthreads();
   for (int kk = 2; kk <= n2; kk <<= 1)
     for (int j = kk >> 1; j > 0; j >>= 1) {
@@ -1446,6 +1515,11 @@ __global__ void __launch_bounds__(256) k_big_radj(const MatchDev* pairs) {
 }
 
 constexpr int BIG_WPL = BIGC / 32 / 32;  // candidate-set words per lane
+
+// the order in which greedy cliques compete: larger clique first, then lower start rank
+__device__ __forceinline__ unsigned long long clique_key(int size, int r) {
+  return ((unsigned long long)size << 32) | (unsigned)(0xFFFFFFFFu - (unsigned)r);
+}
 
 // the greedy clique grown from start vertex `r` by one warp: the candidate set lives in registers, word w in lane
 // w % 32; "first candidate in the global order" is a warp-wide minimum over bit positions.  mark != nullptr lists
@@ -1490,6 +1564,60 @@ __global__ void __launch_bounds__(256) k_big_greedy(const MatchDev* pairs) {
   }
 }
 
+// warp_greedy_clique for any n: the candidate set lives in Pm[wn] (shared or global memory), word w always handled by
+// lane w % 32, so no lane reads a word another lane wrote.  The chosen vertex is the lowest candidate and its own row has
+// no bit at itself, so after each step every candidate lies above it: the pass starts at its 32-word block.
+__device__ __forceinline__ int warp_greedy_clique_buf(const BigSolveWs& W, int wn, int r, unsigned* Pm, int* mark) {
+  const int lane = threadIdx.x & 31;
+  const unsigned* row = W.radj + (size_t)r * W.words;
+  unsigned pos = 0xFFFFFFFFu;
+  for (int w = lane; w < wn; w += 32) {
+    const unsigned b = row[w];
+    Pm[w] = b;
+    if (pos == 0xFFFFFFFFu && b) pos = (unsigned)(w * 32 + __ffs(b) - 1);
+  }
+  pos = __reduce_min_sync(0xffffffffu, pos);
+  if (mark && lane == 0) mark[W.order[r]] = 1;
+  int size = 1;
+  while (pos != 0xFFFFFFFFu) {
+    size++;
+    if (mark && lane == 0) mark[W.order[pos]] = 1;
+    const unsigned* urow = W.radj + (size_t)pos * W.words;
+    unsigned next = 0xFFFFFFFFu;
+    for (int w = (int)((pos >> 5) & ~31u) + lane; w < wn; w += 32) {
+      const unsigned b = Pm[w] & urow[w];
+      Pm[w] = b;
+      if (next == 0xFFFFFFFFu && b) next = (unsigned)(w * 32 + __ffs(b) - 1);
+    }
+    pos = __reduce_min_sync(0xffffffffu, next);
+  }
+  return size;
+}
+
+// The greedy cliques of a set of any size (one pair): one warp per start rank, its candidate set in shared memory.
+// Pruning keeps the winner.  The winner is the start with the largest clique_key(size, r) (largest clique, lowest rank on
+// ties).  A clique grown from r lies in r's neighbourhood and every member has at least size - 1 neighbours inside it,
+// so size <= core(r) + 1 and clique_key(core(r) + 1, r) bounds r's key.  W.best only ever holds keys that some start
+// reached, so it never exceeds the winner's key: a start whose bound is below W.best cannot be the winner and is skipped
+// (csize 0), and the winner is never skipped.  Ranks are ordered by core number descending and blocks start roughly in
+// rank order, so the large cores run first and set W.best early.
+__global__ void __launch_bounds__(256) k_big_greedy_wide(const MatchDev* pairs) {
+  extern __shared__ unsigned cand[];  // [warps per block][wn]
+  const MatchDev& P = pairs[blockIdx.y];
+  const BigSolveWs& W = *P.big;
+  const int n = P.counters[2];
+  const int wn = (n + 31) >> 5;
+  const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (r >= n) return;
+  const unsigned long long seen = *(volatile unsigned long long*)W.best;
+  int size = 0;
+  if (clique_key(W.core[W.order[r]] + 1, r) >= seen) size = warp_greedy_clique_buf(W, wn, r, cand + (threadIdx.x >> 5) * wn, nullptr);
+  if ((threadIdx.x & 31) == 0) {
+    W.csize[r] = size;
+    if (size) atomicMax(W.best, clique_key(size, r));
+  }
+}
+
 __device__ __forceinline__ double block_sum_d(double v, double* red) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   __syncthreads();
@@ -1510,7 +1638,7 @@ __device__ __forceinline__ double block_max_d(double v, double* red) {
 }
 
 // pick the largest clique (lowest rank on ties), list it, GNC-TLS yaw rotation, TLS translation.  One block per pair.
-__global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, QuatroParamsDev prm) {
+__global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, QuatroParamsDev prm, int wide) {
   const MatchDev& P = pairs[blockIdx.x];
   const BigSolveWs& W = *P.big;
   const int n = P.counters[2];
@@ -1519,15 +1647,14 @@ __global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, Quat
   const int tid = threadIdx.x;
   __shared__ double red[32];
   __shared__ unsigned long long kred[32];
-  __shared__ int wsum[32];
-  __shared__ int carry, stop;
+  __shared__ int stop;
   __shared__ double s_mu, s_prev, s_R2[4], s_t[3];
   constexpr int SWEEP = 2048;
   __shared__ double cX[SWEEP];
   __shared__ int cE[SWEEP];
   {
     unsigned long long key = 0;
-    for (int r = tid; r < n; r += 1024) key = max(key, ((unsigned long long)W.csize[r] << 32) | (unsigned)(0xFFFFFFFFu - (unsigned)r));
+    for (int r = tid; r < n; r += 1024) key = max(key, clique_key(W.csize[r], r));
     for (int o = 16; o > 0; o >>= 1) key = max(key, __shfl_xor_sync(0xffffffffu, key, o));
     if ((tid & 31) == 0) kred[tid >> 5] = key;
     __syncthreads();
@@ -1536,40 +1663,15 @@ __global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, Quat
     const int br = (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull));
     for (int v = tid; v < n; v += 1024) W.alive[v] = 0;  // member flags
     __syncthreads();
-    if (tid < 32) warp_greedy_clique(W, wn, br, W.alive);
-    if (tid == 0) carry = 0;
-    __syncthreads();
-  }
-  // members in ascending ORIGINAL correspondence index: ordered block compaction
-  for (int base = 0; base < n; base += 1024) {
-    const int v = base + tid;
-    const int keep = (v < n && W.alive[v]) ? 1 : 0;
-    int incl = keep;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, incl, o);
-      if ((tid & 31) >= o) incl += t;
-    }
-    if ((tid & 31) == 31) wsum[tid >> 5] = incl;
-    __syncthreads();
     if (tid < 32) {
-      const int w = wsum[tid];
-      int wi = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, wi, o);
-        if (tid >= o) wi += t;
-      }
-      wsum[tid] = wi - w;
+      if (wide) warp_greedy_clique_buf(W, wn, br, (unsigned*)W.list, W.alive);  // list is free once k_big_core is done
+      else warp_greedy_clique(W, wn, br, W.alive);
     }
     __syncthreads();
-    const int pos = carry + wsum[tid >> 5] + incl - keep;
-    if (keep) W.clique[pos] = v;
-    __syncthreads();
-    if (tid == 1023) carry = pos + keep;
-    __syncthreads();
   }
-  const int m = carry;
+  // members in ascending ORIGINAL correspondence index
+  const int m = block_compact(
+      n, [&](int v) { return W.alive[v] != 0; }, [&](int pos, int v) { W.clique[pos] = v; });
   if (tid == 0) P.counters[4] = m;
   if (m <= 1) return;  // solution_.valid stays false
   const int nt = m - 1;
@@ -1748,12 +1850,15 @@ int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2,
 }
 
 size_t solve_smem_bytes() { return sizeof(SolveSmem); }
-int launch_big_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, cudaStream_t s);
+
+constexpr int WIDE_SMEM = 227 * 1024;  // opt-in shared memory per block on sm_90
 
 // Opt-in shared-memory sizes are a PER-DEVICE function attribute: b200reg_ctx_create calls this after cudaSetDevice, so
 // every context (one per GPU in a multi-GPU process) gets them on its own device.
 cudaError_t quatro_init_device() {
   cudaError_t e = cudaFuncSetAttribute(k_teaser_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SolveSmem));
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(k_big_greedy_wide, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM);
   if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(k_adv_select, cudaFuncAttributeMaxDynamicSharedMemorySize, BIGC * 8);
 }
@@ -1774,19 +1879,35 @@ int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, in
     return l;
   }
   k_adv_select<<<count, 1024, BIGC * 8, s>>>(d_pairs, prm); l++;
-  return l + launch_big_solve(d_pairs, count, prm, s);
+  k_big_gather<<<dim3(BIGC / 256, count), 256, 0, s>>>(d_pairs); l++;
+  return l + launch_big_graph_solve(d_pairs, count, prm, 0, s);
 }
 
-// TEASER++ solve over the global-memory workspace (correspondences already in out_corr / counters[2])
-int launch_big_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, cudaStream_t s) {
+// one pair whose advancedMatching set outgrew k_adv_select (n > BIGC correspondences, counters[6] = n): select into the
+// pair's own workspace, gather, solve
+int launch_adv_wide(const MatchDev* d_pair, int n, const QuatroParamsDev& prm, cudaStream_t s) {
+  k_adv_select_wide<<<1, 1024, 0, s>>>(d_pair, prm);
+  k_big_gather<<<(n + 255) / 256, 256, 0, s>>>(d_pair);
+  return 2 + launch_big_graph_solve(d_pair, 1, prm, n, s);
+}
+
+// TEASER++ solve over the global-memory workspace (S / D gathered, counters[2] set): TIM graph, core order, greedy
+// cliques, GNC-TLS.  n_wide == 0: sets of at most BIGC, candidate sets in registers, any batch; n_wide > 0: one pair of
+// n_wide correspondences, candidate sets in shared memory and pruned starts (k_big_greedy_wide).
+int launch_big_graph_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, int n_wide, cudaStream_t s) {
   int l = 0;
   const int wide = 592 / count > 0 ? 592 / count : 1;  // ~4 CTAs per SM over the batch
-  k_big_gather<<<dim3(BIGC / 256, count), 256, 0, s>>>(d_pairs); l++;
   k_big_tim<<<dim3(wide, count), 256, 0, s>>>(d_pairs, prm); l++;
   k_big_core<<<count, 1024, 0, s>>>(d_pairs); l++;
   k_big_radj<<<dim3(wide, count), 256, 0, s>>>(d_pairs); l++;
-  k_big_greedy<<<dim3(wide, count), 256, 0, s>>>(d_pairs); l++;
-  k_big_finish<<<count, 1024, 0, s>>>(d_pairs, prm); l++;
+  if (n_wide > 0) {
+    const int wn = (n_wide + 31) / 32;
+    const int wpb = std::min(8, WIDE_SMEM / (wn * 4));  // >= 1: n < 2^20 needs 128 KB per warp at most
+    k_big_greedy_wide<<<dim3((n_wide + wpb - 1) / wpb, count), 32 * wpb, (size_t)wpb * wn * 4, s>>>(d_pairs); l++;
+  } else {
+    k_big_greedy<<<dim3(wide, count), 256, 0, s>>>(d_pairs); l++;
+  }
+  k_big_finish<<<count, 1024, 0, s>>>(d_pairs, prm, n_wide > 0); l++;
   return l;
 }
 

@@ -182,12 +182,24 @@ int b200reg_clouds_fpfh(b200reg_ctx* ctx, int count, b200reg_cloud* const* cloud
  * optimizedMatching (matcher.cc:358-561) or, with use_optimized_matching = 0, advancedMatching (matcher.cc:118-356:
  * ungated forward / reverse 1-NN, cross check, three-edge tuple test, sort + unique), then the TEASER++ QUATRO solve.
  * corr_out (optional): count x 2*CAP ints, the (src, dst) ORIGINAL indices of the final correspondences of each
- * pair, CAP = B200REG_CORR_CAPACITY (optimized) or B200REG_ADV_CORR_CAPACITY (advanced).  An advancedMatching set
- * larger than B200REG_ADV_CORR_CAPACITY fails the call with B200REG_ESTATE (nothing is truncated silently).     */
+ * pair, CAP = B200REG_CORR_CAPACITY (optimized) or B200REG_ADV_CORR_CAPACITY (advanced).  advancedMatching sets of any
+ * size (below 2^20) are solved; a set larger than B200REG_ADV_CORR_CAPACITY does not fit corr_out, so with a non-NULL
+ * corr_out such a set fails the call with B200REG_ESTATE (nothing is truncated silently), and with corr_out NULL the
+ * call solves it.  b200reg_quatro_align_ex returns the correspondences of any size.
+ * Pairs with at most B200REG_ADV_CORR_CAPACITY correspondences are solved together; larger sets are solved one pair at
+ * a time in one device workspace sized for the largest (about n^2 / 4 bytes for n correspondences: 1 GB at n = 65536).
+ * If that workspace cannot be allocated the call returns B200REG_ECUDA with the bytes needed in the message.     */
 #define B200REG_CORR_CAPACITY 512
 #define B200REG_ADV_CORR_CAPACITY 8192
 int b200reg_quatro_align(b200reg_ctx* ctx, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst,
                          const b200reg_quatro_params* params, b200reg_quatro_info* out, int32_t* corr_out);
+/* Same solve; the final correspondences come back as CSR, as b200reg_radius_search returns neighbours: those of pair i
+ * are the (src, dst) pairs corr_out[2 * offsets_out[i] ..  2 * offsets_out[i + 1]), offsets_out has count + 1 entries
+ * and must not be NULL.  If the total exceeds `capacity` (in pairs) the call fills offsets_out, writes nothing else and
+ * returns B200REG_ESTATE.  corr_out == NULL: offsets and `out` only.                                              */
+int b200reg_quatro_align_ex(b200reg_ctx* ctx, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst,
+                            const b200reg_quatro_params* params, b200reg_quatro_info* out, int64_t* offsets_out,
+                            size_t capacity, int32_t* corr_out);
 /* LoopClosure::coarseToFineAlignment (fast_lio_sam_qn/src/loop_closure.cpp:138-159) for `count` pairs from raw
  * buffers: Quatro -> transformPcd(src, T_quatro) -> icpAlignment -> T = T_gicp * T_quatro.
  * out[i].T is the composed transform; quatro_out (optional) receives the coarse stage.                   */
@@ -360,6 +372,14 @@ int b200reg_knn_bruteforce(b200reg_ctx* ctx, const b200reg_cloud* cloud, const f
 int b200reg_radius_search(b200reg_ctx* ctx, const b200reg_cloud* cloud, const float* queries, size_t nq,
                           size_t qstride_bytes, double sq_radius, int sorted, int64_t* offsets_out, size_t capacity,
                           int32_t* idx_out, float* d2_out);
+/* The TEASER++ QUATRO solve that follows advancedMatching, on n given correspondences: correspondence i joins
+ * src_xyz[3i..3i+2] to dst_xyz[3i..3i+2] (host floats).  TIM graph, core-number order, greedy clique, GNC-TLS yaw and
+ * TLS translation, exactly as b200reg_quatro_align runs them.  wide == 0 takes the path of sets up to
+ * B200REG_ADV_CORR_CAPACITY (n must not exceed it); wide != 0 the path of larger sets, for any 1 <= n < 2^20.  Both
+ * give the same answer.  info: T, valid, clique_size, gnc_iterations (n_mutual = n_corr = n).  clique_out (optional,
+ * n ints): the clique's correspondence indices, ascending.                                                      */
+int b200reg_quatro_solve_tap(b200reg_ctx* ctx, int n, const float* src_xyz, const float* dst_xyz, int wide,
+                             const b200reg_quatro_params* params, b200reg_quatro_info* info, int32_t* clique_out);
 /* normals (n x 3, NaN where fewer than 3 neighbours) and FPFH (n x 33), original point order.            */
 int b200reg_get_fpfh(b200reg_ctx* ctx, const b200reg_cloud* cloud, float* normals_out, float* fpfh_out);
 /* n x 9 doubles (row-major 3x3 block of the reference's Matrix4d), original point order.          */
