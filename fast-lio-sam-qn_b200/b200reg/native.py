@@ -34,6 +34,20 @@ class Result(C.Structure):
                     lm_failed=bool(self.lm_failed), status=self.status)
 
 
+class LmTrial(C.Structure):
+    """b200reg_lm_trial: one LM trial of the device solve (decision 1 accepted, 0 rejected, 2 rejected but converged,
+    3 rejected on the last allowed trial)."""
+    _fields_ = [("outer", C.c_int32), ("trial", C.c_int32), ("decision", C.c_int32), ("reserved", C.c_int32),
+                ("y0", C.c_double), ("yi", C.c_double), ("rho", C.c_double), ("lambda", C.c_double), ("nu", C.c_double),
+                ("d", C.c_double * 6), ("T", C.c_double * 12)]
+
+
+# the same record as a numpy structured dtype (Context.lm_trace); T is x0 after the decision, row-major 3 x 4
+LM_TRIAL_DTYPE = np.dtype([("outer", "<i4"), ("trial", "<i4"), ("decision", "<i4"), ("reserved", "<i4"), ("y0", "<f8"),
+                           ("yi", "<f8"), ("rho", "<f8"), ("lambda", "<f8"), ("nu", "<f8"), ("d", "<f8", (6,)),
+                           ("T", "<f8", (3, 4))])
+
+
 class QuatroParams(C.Structure):
     _fields_ = [("fpfh_normal_radius", C.c_double), ("fpfh_radius", C.c_double), ("noise_bound", C.c_double),
                 ("rot_gnc_factor", C.c_double), ("rot_cost_thr", C.c_double), ("rot_max_iter", C.c_int32),
@@ -82,6 +96,7 @@ EXPORTS = [
     "b200reg_batch_wait", "b200reg_batch_wait_all", "b200reg_batch_launch_count", "b200reg_batch_depth",
     "b200reg_comm_unique_id", "b200reg_comm_init", "b200reg_comm_destroy", "b200reg_comm_rank", "b200reg_comm_world",
     "b200reg_allgather_results", "b200reg_radius_search", "b200reg_quatro_align_ex", "b200reg_quatro_solve_tap",
+    "b200reg_ctx_set_lm_trace", "b200reg_lm_trace",
 ]
 ESTATE = -4  # B200REG_ESTATE
 
@@ -217,6 +232,24 @@ class Context:
             _check(lib().b200reg_ctx_get_profile(self.h, f, C.byref(name), C.byref(ms), C.byref(by), C.byref(ln)))
             out[name.value.decode()] = dict(ms=ms.value, algo_bytes=by.value, launches=ln.value)
         return out
+
+    def set_lm_trace(self, enable):
+        """Record every LM trial of the following solves (LsqRegistration::setDebugPrint); results do not change."""
+        _check(lib().b200reg_ctx_set_lm_trace(self.h, int(bool(enable))))
+
+    def lm_trace(self):
+        """The trials of the last call that ran the LM solve: one LM_TRIAL_DTYPE array per pair of that call (the caller's
+        pair order; empty for a pair whose fine stage did not run), each in execution order."""
+        n = lib().b200reg_lm_trace(self.h, None, C.c_size_t(0), None)
+        _check(min(n, 0))
+        offsets = np.empty(n + 1, np.int64)
+        rc = lib().b200reg_lm_trace(self.h, offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None)  # offsets only
+        if rc != ESTATE:
+            _check(rc)
+        trials = np.empty(int(offsets[-1]), LM_TRIAL_DTYPE)
+        _check(lib().b200reg_lm_trace(self.h, offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(trials)),
+                                      trials.ctypes.data_as(C.c_void_p)))
+        return [trials[offsets[i]:offsets[i + 1]] for i in range(n)]
 
     # -- the path's one collective: all-gather of the result records over NCCL (SURVEY §8e) --------
     def comm_init(self, unique_id, rank, world):

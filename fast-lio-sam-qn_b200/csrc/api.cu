@@ -108,6 +108,7 @@ size_t b200reg_struct_size(int which) {
     case 3: return sizeof(b200reg_quatro_info);
     case 4: return sizeof(b200reg_loop_config);
     case 5: return sizeof(b200reg_loop_factor);
+    case 6: return sizeof(b200reg_lm_trial);
     default: return 0;
   }
 }

@@ -51,6 +51,14 @@ struct b200reg_ctx {
     PairState* h_states = nullptr;  // pinned read-back
     LmGraph graph;
   } lm;
+  // LM trace of the most recent call that ran the LM solve (b200reg_ctx_set_lm_trace / b200reg_lm_trace), CSR over the pairs
+  // of that call, on the host
+  struct LmTrace {
+    bool enabled = false;
+    bool valid = false;  // false before a traced solve and after an untraced one
+    std::vector<int64_t> offsets;  // pairs + 1
+    std::vector<b200reg_lm_trial> trials;
+  } lm_trace;
   // the path's one collective (b200reg_comm_*): NCCL communicator of this rank
   ncclComm_t comm = nullptr;
   int rank = -1, world = 1;
@@ -160,6 +168,11 @@ int create_pair_clouds(b200reg_ctx* c, int count, const float* const* src_xyz, c
 int sorted_to_original(b200reg_ctx* c, const CloudDev& d, std::vector<int>& orig, std::vector<float4>* pts_out = nullptr);
 
 void lm_arena_free(b200reg_ctx* c);  // api_gicp.cu
+
+// The stored LM trace belongs to the pairs of the last b200reg_gicp_align.  A caller that ran that solve on a subset of its
+// `count` pairs (solve pair k = its pair where[k]; `where` empty when no solve ran) renumbers it to its own pairs; the
+// others get no records.  Does nothing but keep the trace invalid when tracing is off.  (api_gicp.cu)
+void lm_trace_remap(b200reg_ctx* c, int count, const std::vector<int>& where);
 
 // LoopClosure::coarseToFineAlignment on cloud handles (api_quatro.cu)
 int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst,

@@ -74,6 +74,26 @@ void lm_arena_free(b200reg_ctx* c) {
   if (a.h_states) cudaFreeHost(a.h_states);
   a = b200reg_ctx::LmArena();
 }
+
+void lm_trace_remap(b200reg_ctx* c, int count, const std::vector<int>& where) {
+  auto& tr = c->lm_trace;
+  if (!tr.enabled) {
+    tr.valid = false;
+    return;
+  }
+  std::vector<int> solved(count, -1);  // caller pair -> solve pair
+  for (size_t k = 0; k < where.size(); k++) solved[where[k]] = (int)k;
+  std::vector<int64_t> offsets(count + 1, 0);
+  std::vector<b200reg_lm_trial> trials;
+  for (int i = 0; i < count; i++) {
+    const int k = solved[i];
+    if (k >= 0) trials.insert(trials.end(), tr.trials.begin() + tr.offsets[k], tr.trials.begin() + tr.offsets[k + 1]);
+    offsets[i + 1] = (int64_t)trials.size();
+  }
+  tr.offsets.swap(offsets);
+  tr.trials.swap(trials);
+  tr.valid = true;
+}
 }  // namespace b200
 
 // make the arena hold `count` pairs and make sure its graph exists
@@ -155,6 +175,25 @@ static int tap_begin(b200reg_ctx* c, const b200reg_cloud* src, const b200reg_clo
 
 extern "C" {
 
+int b200reg_ctx_set_lm_trace(b200reg_ctx* c, int enable) {
+  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
+  c->lm_trace.enabled = enable != 0;
+  return B200REG_OK;
+}
+
+int b200reg_lm_trace(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out) {
+  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
+  const auto& tr = c->lm_trace;
+  if (!tr.valid) return fail(B200REG_ESTATE, "no LM trace: the context's last LM solve was not traced (b200reg_ctx_set_lm_trace)");
+  const int pairs = (int)tr.offsets.size() - 1;
+  if (!offsets_out) return pairs;
+  memcpy(offsets_out, tr.offsets.data(), sizeof(int64_t) * tr.offsets.size());
+  if (tr.trials.size() > capacity)
+    return fail(B200REG_ESTATE, "LM trace holds " + std::to_string(tr.trials.size()) + " records, capacity " + std::to_string(capacity));
+  if (trials_out && !tr.trials.empty()) memcpy(trials_out, tr.trials.data(), sizeof(b200reg_lm_trial) * tr.trials.size());
+  return B200REG_OK;
+}
+
 int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* tgt,
                        const double* guess16, const b200reg_gicp_params* params, b200reg_result* out) {
   if (!c || count <= 0 || !src || !tgt || !params || !out) return fail(B200REG_EINVAL, "bad argument");
@@ -194,6 +233,18 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
   hc.max_steps = std::max(params->max_iterations, 0) * (1 + std::max(params->lm_max_iterations, 1)) + 2;
   hc.cond_handle = A.graph.cond_handle;
   hc.prm = prm;
+  auto& tr = c->lm_trace;
+  tr.valid = false;
+  if (tr.enabled) {
+    // every outer iteration makes at most max(lm_max_iterations, 1) trials: the buffer holds any solve's records
+    hc.trace_stride = (long long)std::max(params->max_iterations, 0) * std::max(params->lm_max_iterations, 1);
+    const size_t bytes = sizeof(b200reg_lm_trial) * (size_t)hc.trace_stride * count;
+    if (bytes) {
+      const cudaError_t e = scratch.alloc((void**)&hc.trace, bytes);
+      if (e != cudaSuccess)
+        return fail(B200REG_ECUDA, "LM trace: cannot allocate " + std::to_string(bytes) + " bytes: " + cudaGetErrorString(e));
+    }
+  }
   CU(cudaMemcpyAsync(A.d_call, A.h_call, sizeof(LmCall), cudaMemcpyHostToDevice, s));
   static const bool env_no_graph = getenv("B200REG_LM_NO_GRAPH") != nullptr;  // Nsight Compute does not list kernels that run
   const bool no_graph = env_no_graph || c->profiling;                          // inside a conditional graph node
@@ -224,6 +275,24 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
   CU(cudaStreamSynchronize(s));
   if (!no_graph) c->launches += 1 + 3 * (int64_t)hsched.steps;  // init + (search, accumulate, control) per executed step, counted by the device
   if (A.h_call->overrun) return fail(B200REG_ESTATE, "LM state machine did not terminate");
+  if (tr.enabled) {  // pair i's records are the first n_err of its region: one strided copy of the longest, then compacted
+    int widest = 0;
+    tr.offsets.assign(count + 1, 0);
+    for (int i = 0; i < count; i++) {
+      tr.offsets[i + 1] = tr.offsets[i] + states[i].n_err;
+      widest = std::max(widest, states[i].n_err);
+    }
+    std::vector<b200reg_lm_trial> rows((size_t)count * widest);
+    const size_t rec = sizeof(b200reg_lm_trial);
+    if (widest > 0) {
+      CU(cudaMemcpy2DAsync(rows.data(), rec * widest, hc.trace, rec * hc.trace_stride, rec * widest, count, cudaMemcpyDeviceToHost, s));
+      CU(cudaStreamSynchronize(s));
+    }
+    tr.trials.resize(tr.offsets[count]);
+    for (int i = 0; i < count; i++)
+      std::copy(rows.begin() + (size_t)i * widest, rows.begin() + (size_t)i * widest + states[i].n_err, tr.trials.begin() + tr.offsets[i]);
+    tr.valid = true;
+  }
   for (int i = 0; i < count; i++) {
     const PairState& st = states[i];
     b200reg_result& r = out[i];

@@ -426,7 +426,10 @@ int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int coun
       where.push_back(i);
     }
   }
-  if (qs.empty()) return B200REG_OK;
+  if (qs.empty()) {
+    lm_trace_remap(c, count, where);
+    return B200REG_OK;
+  }
   const int m = (int)qs.size();
   // at the time query q was the latest keyframe the vector held q + 1 keyframes (fast_lio_sam_qn.cpp:205-219); a batch
   // replays several ticks, so every pair carries the size its own tick saw (the sub-map bounds of loop_closure.cpp:72,79,100)
@@ -446,6 +449,7 @@ int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int coun
     out[where[k]] = res[k];
     if (quatro_out && cfg->enable_quatro) quatro_out[where[k]] = qi[k];
   }
+  if (!rc) lm_trace_remap(c, count, where);
   return rc;
 }
 

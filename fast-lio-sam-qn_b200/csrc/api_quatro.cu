@@ -86,6 +86,7 @@ int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* sr
       out[i] = r;
     }
   }
+  lm_trace_remap(c, count, vidx);
   return B200REG_OK;
 }
 

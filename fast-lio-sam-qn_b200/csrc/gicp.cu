@@ -132,8 +132,28 @@ __device__ void lm_finish(PairState* st, int converged) {
   st->phase = PH_FITNESS;
 }
 
+// One trace record (b200reg_lm_trial): the trial's inputs and outcome, and x0 after the decision.
+__device__ void lm_record(b200reg_lm_trial* r, const PairState* st, int trial, int decision, double yi, double rho, double lambda,
+                          double nu, const double d[6]) {
+  r->outer = st->nr_iterations;
+  r->trial = trial;
+  r->decision = decision;
+  r->reserved = 0;
+  r->y0 = st->y0;
+  r->yi = yi;
+  r->rho = rho;
+  r->lambda = lambda;
+  r->nu = nu;
+  for (int i = 0; i < 6; i++) r->d[i] = d[i];
+  for (int i = 0; i < 3; i++) {
+    for (int j = 0; j < 3; j++) r->T[4 * i + j] = st->R[3 * i + j];
+    r->T[4 * i + 3] = st->t[i];
+  }
+}
+
+// trace: this pair's trace region (LmCall::trace), nullptr when tracing is off
 __device__ void lm_update(PairState* st, const double* sums, const GicpParamsDev& prm, int phase, int n_src,
-                          int* done_counter) {  // done_counter = &LmSched::done
+                          int* done_counter, b200reg_lm_trial* trace) {  // done_counter = &LmSched::done
   if (phase == PH_LINEARIZE) {
     int k = 0;
     for (int i = 0; i < 6; i++)
@@ -161,36 +181,44 @@ __device__ void lm_update(PairState* st, const double* sums, const GicpParamsDev
     double denom = 0;
     for (int i = 0; i < 6; i++) denom += st->d[i] * (st->lambda * st->d[i] - st->b[i]);
     const double rho = (st->y0 - yi) / denom;
+    // what the trace records of this trial: the next trial's lm_prepare_trial overwrites d, the decision moves lambda / nu
+    const int trial = st->inner_it;
+    const double lambda = st->lambda, nu = st->nu;
+    double d[6];
+    for (int i = 0; i < 6; i++) d[i] = st->d[i];
+    int decision;
     if (rho < 0) {
       if (delta_converged(st, prm)) {
+        decision = 2;
         lm_finish(st, 1);  // step_lm returns true without touching x0; the caller then sees converged
-        return;
+      } else {
+        st->lambda = st->nu * st->lambda;
+        st->nu = 2 * st->nu;
+        st->inner_it++;
+        if (st->inner_it >= prm.lm_max_iterations) {
+          decision = 3;
+          st->lm_failed = 1;  // "lm not converged!!"
+          lm_finish(st, 0);
+        } else {
+          decision = 0;
+          lm_prepare_trial(st);
+        }
       }
-      st->lambda = st->nu * st->lambda;
-      st->nu = 2 * st->nu;
-      st->inner_it++;
-      if (st->inner_it >= prm.lm_max_iterations) {
-        st->lm_failed = 1;  // "lm not converged!!"
-        lm_finish(st, 0);
-        return;
+    } else {
+      decision = 1;
+      for (int i = 0; i < 9; i++) st->R[i] = st->Rt[i];
+      for (int i = 0; i < 3; i++) st->t[i] = st->tt[i];
+      const double x = 2 * rho - 1;
+      st->lambda = st->lambda * fmax(1.0 / 3.0, 1 - x * x * x);
+      if (delta_converged(st, prm)) {
+        lm_finish(st, 1);
+      } else {
+        st->outer_it++;
+        if (st->outer_it >= prm.max_iterations) lm_finish(st, 0);
+        else st->phase = PH_LINEARIZE;
       }
-      lm_prepare_trial(st);
-      return;
     }
-    for (int i = 0; i < 9; i++) st->R[i] = st->Rt[i];
-    for (int i = 0; i < 3; i++) st->t[i] = st->tt[i];
-    const double x = 2 * rho - 1;
-    st->lambda = st->lambda * fmax(1.0 / 3.0, 1 - x * x * x);
-    if (delta_converged(st, prm)) {
-      lm_finish(st, 1);
-      return;
-    }
-    st->outer_it++;
-    if (st->outer_it >= prm.max_iterations) {
-      lm_finish(st, 0);
-      return;
-    }
-    st->phase = PH_LINEARIZE;
+    if (trace) lm_record(&trace[st->n_err - 1], st, trial, decision, yi, rho, lambda, nu, d);
   } else if (phase == PH_FITNESS) {
     st->fitness = n_src > 0 ? sums[0] / (double)n_src : 0.0;
     st->phase = PH_DONE;
@@ -642,7 +670,8 @@ __global__ void __launch_bounds__(CTRL_THREADS) k_gicp_control(const PairDev* pa
         for (int w = 0; w < CTRL_THREADS / 32; w++) s += s_red[w][k];
         sums[k] = s;
       }
-      lm_update(&states[sl.pair], sums, call->prm, sl.phase, N, &sched->done);
+      b200reg_lm_trial* trace = call->trace ? call->trace + (size_t)sl.pair * call->trace_stride : nullptr;
+      lm_update(&states[sl.pair], sums, call->prm, sl.phase, N, &sched->done, trace);
     }
   }
   // ---- end of the step: the last block to get here rebuilds the schedule from the pairs' new phases

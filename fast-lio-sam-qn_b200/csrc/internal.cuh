@@ -16,6 +16,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/b200reg.h"  // b200reg_lm_trial: the LM controller writes the ABI's trace records directly
+
 namespace b200 {
 
 constexpr int LEAF = 8;            // max points per leaf (8 x 16 B = one 128-B line); must be <= 15
@@ -111,7 +113,7 @@ struct PairState {
   int inner_it;  // LM trials done in this outer iteration
   int converged;
   int lm_failed;
-  int n_lin, n_err;
+  int n_lin, n_err;     // n_err also counts the pair's trace records: trial k goes to LmCall::trace slot k
   int nr_iterations;
   unsigned int arrive;  // (unused since the controller became its own kernel; kept for layout stability)
   int pad;
@@ -152,6 +154,10 @@ struct LmCall {
   int overrun;          // set by the device when max_steps was hit (a bug in the state machine, never expected)
   unsigned long long cond_handle;  // cudaGraphConditionalHandle of the while node, 0 when the step kernels are launched directly
   GicpParamsDev prm;
+  // LM trace (b200reg_ctx_set_lm_trace): pair p's trials go to trace[p * trace_stride ...]; nullptr = tracing off.  Per call,
+  // like everything here, so the executable graph does not change when tracing is switched.
+  b200reg_lm_trial* trace;
+  long long trace_stride;  // max_iterations * max(lm_max_iterations, 1): no pair makes more trials
 };
 
 struct PairDev {

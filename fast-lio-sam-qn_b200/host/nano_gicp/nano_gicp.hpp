@@ -16,10 +16,14 @@
 //   * covariances live on the device and are materialised on the host lazily by getSource/TargetCovariances() as
 //     Eigen::Matrix4d (4th row/column zero, like the reference's, nano_gicp_impl.hpp:354); setSource/TargetCovariances
 //     upload the caller's.
+//   * setDebugPrint(true) prints the reference's LM table to std::cout, row for row, but all of it when the solve has
+//     finished on the device (the rows come from the solve's trace, b200reg_lm_trace), not while it runs; lastLmTrace()
+//     returns the records themselves.
 #pragma once
 #include <array>
 #include <cmath>
 #include <cstdio>
+#include <iostream>
 #include <limits>
 #include <memory>
 #include <vector>
@@ -90,7 +94,7 @@ class NanoGICP {
   // ---- LsqRegistration (lsq_registration.hpp:84-92)
   void setRotationEpsilon(double e) { prm_.rotation_eps = e; }
   void setInitialLambdaFactor(double f) { prm_.lm_init_lambda_factor = f; }
-  void setDebugPrint(bool) {}
+  void setDebugPrint(bool lm_debug_print) { lm_debug_print_ = lm_debug_print; }
 
   // ---- inputs (nano_gicp_impl.hpp:120-139): pointer-identity early-out, index build, covariances cleared
   void setInputSource(const PointCloudSourceConstPtr& cloud) {
@@ -146,11 +150,19 @@ class NanoGICP {
     b200reg_host::to_rowmajor(guess, g);
     b200reg_cloud* s[1] = {src_.get()};
     b200reg_cloud* t[1] = {tgt_.get()};
-    const int rc = b200reg_gicp_align(b200reg_host::context(), 1, s, t, g, &prm_, &res_);
+    b200reg_ctx* ctx = b200reg_host::context();
+    lm_trace_.clear();
+    if (lm_debug_print_) b200reg_ctx_set_lm_trace(ctx, 1);
+    const int rc = b200reg_gicp_align(ctx, 1, s, t, g, &prm_, &res_);
+    if (lm_debug_print_) {
+      if (rc == 0) fetch_lm_trace(ctx);
+      b200reg_ctx_set_lm_trace(ctx, 0);
+    }
     if (rc != 0) {
       std::fprintf(stderr, "b200reg: gicp_align failed (%d): %s\n", rc, b200reg_last_error());
       return;
     }
+    if (lm_debug_print_) print_lm_trace();
     if (res_.lm_failed) std::fprintf(stderr, "lm not converged!!\n");  // lsq_registration_impl.hpp:106
     src_cov_ok_ = tgt_cov_ok_ = true;
     converged_ = res_.converged != 0;
@@ -194,6 +206,8 @@ class NanoGICP {
   }
   int nr_iterations() const { return res_.iterations; }
   const b200reg_result& lastResult() const { return res_; }
+  // every LM trial of the last align(), in execution order; empty unless setDebugPrint(true)
+  const std::vector<b200reg_lm_trial>& lastLmTrace() const { return lm_trace_; }
 
   // nano_gicp.hpp:121-122: search the clouds set by setInputSource / setInputTarget (radiusSearch takes a SQUARED radius)
   std::shared_ptr<nanoflann::KdTreeFLANN<PointSource>> source_kdtree_;
@@ -206,6 +220,35 @@ class NanoGICP {
     if (!cloud || cloud->size() == 0) return;
     using P = typename std::remove_reference<decltype(cloud->points[0])>::type;
     *slot = b200reg_host::make_device_cloud(reinterpret_cast<const float*>(cloud->points.data()), cloud->size(), sizeof(P));
+  }
+  void fetch_lm_trace(b200reg_ctx* ctx) {
+    int64_t off[2] = {0, 0};
+    b200reg_lm_trace(ctx, off, 0, nullptr);  // B200REG_ESTATE unless the pair made no trial: off[1] is the count either way
+    lm_trace_.resize(off[1]);
+    const int rc = b200reg_lm_trace(ctx, off, lm_trace_.size(), lm_trace_.data());
+    if (rc != 0) {
+      std::fprintf(stderr, "b200reg: lm_trace failed (%d): %s\n", rc, b200reg_last_error());
+      lm_trace_.clear();
+    }
+  }
+  // what LsqRegistration prints with lm_debug_print_ (lsq_registration_impl.hpp:95-99, 183-189), one row per trial
+  void print_lm_trace() const {
+    std::cout << "********************************************" << std::endl;
+    std::cout << "***************** optimize *****************" << std::endl;
+    std::cout << "********************************************" << std::endl;
+    char line[160];
+    for (const b200reg_lm_trial& r : lm_trace_) {
+      if (r.trial == 0) {
+        std::snprintf(line, sizeof(line), "--- LM optimization ---\n%5s %15s %15s %15s %15s %15s %5s\n", "i", "y0", "yi", "rho",
+                      "lambda", "|delta|", "dec");
+        std::cout << line;
+      }
+      double dn = 0;
+      for (int k = 0; k < 6; k++) dn += r.d[k] * r.d[k];
+      std::snprintf(line, sizeof(line), "%5d %15g %15g %15g %15g %15g %5c", r.trial, r.y0, r.yi, r.rho, r.lambda, std::sqrt(dn),
+                    r.rho > 0.0 ? 'x' : ' ');
+      std::cout << line << std::endl;
+    }
   }
   void destroy(b200reg_host::DeviceCloud* slot) { slot->reset(); }  // the device cloud goes when its last user (a tree) does
   void release() {
@@ -257,6 +300,8 @@ class NanoGICP {
   PointCloudTargetConstPtr target_;
   b200reg_host::DeviceCloud src_, tgt_;
   bool src_cov_ok_ = false, tgt_cov_ok_ = false, converged_ = false;
+  bool lm_debug_print_ = false;  // lsq_registration.hpp:92
+  std::vector<b200reg_lm_trial> lm_trace_;
   std::array<float, 16> final_;
   Matrix6d final_hessian_;
   int ransac_iterations_ = 0;

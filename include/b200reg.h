@@ -117,8 +117,28 @@ void b200reg_default_quatro_params(b200reg_quatro_params* p);
 const char* b200reg_last_error(void);                /* message of the calling thread's last failure               */
 void b200reg_set_last_error(const char* message);  /* used by the batch driver to hand a worker's message over     */
 const char* b200reg_version(void);
+/* One Levenberg-Marquardt trial of the Nano-GICP solve: one pass through the body of step_lm's
+ * `for (i < lm_max_iterations_)` loop (lsq_registration_impl.hpp:170-205), recorded when tracing is enabled
+ * (b200reg_ctx_set_lm_trace).  LsqRegistration::setDebugPrint prints one table row per such trial (:183-189). */
+typedef struct b200reg_lm_trial {
+  int32_t outer;       /* outer iteration: nr_iterations_ during the trial                                          */
+  int32_t trial;       /* step_lm's i: the first column of the reference's table                                    */
+  int32_t decision;    /* 1 accepted (x0 <- xi); 0 rejected (lambda <- nu lambda); 2 rejected but is_converged(delta)
+                          held, so the solve returns without moving x0 (:191-194); 3 rejected on the last allowed trial,
+                          "lm not converged!!" (:105-108)                                                              */
+  int32_t reserved;    /* 0                                                                                          */
+  double y0;           /* error of the linearization this trial belongs to                                           */
+  double yi;           /* compute_error at the trial pose                                                            */
+  double rho;          /* (y0 - yi) / d.(lambda d - b)                                                               */
+  double lambda;       /* the lambda the trial was solved with (the value the reference prints)                      */
+  double nu;           /* the nu in force during the trial                                                           */
+  double d[6];         /* the step (rotation, translation): |delta| = ||d||                                          */
+  double T[12];        /* x0 after the decision, row-major 3 x 4                                                     */
+} b200reg_lm_trial;
+
 /* sizeof() of the ABI structs as compiled into the library, so that a binding (ctypes, cgo, JNI ...) can check its own
- * layout at load time: 0 gicp_params, 1 result, 2 quatro_params, 3 quatro_info, 4 loop_config, 5 loop_factor.  0 = unknown. */
+ * layout at load time: 0 gicp_params, 1 result, 2 quatro_params, 3 quatro_info, 4 loop_config, 5 loop_factor,
+ * 6 lm_trial.  0 = unknown. */
 size_t b200reg_struct_size(int which);
 
 /* ---- context ---------------------------------------------------------------------- */
@@ -139,6 +159,21 @@ int b200reg_ctx_set_profiling(b200reg_ctx* ctx, int enable);
 int b200reg_ctx_reset_profile(b200reg_ctx* ctx);
 int b200reg_ctx_get_profile(b200reg_ctx* ctx, int family, const char** name, double* ms, double* algo_bytes,
                             int64_t* launches);
+
+/* LM trace (LsqRegistration::setDebugPrint, lsq_registration_impl.hpp:95-99, 183-189).  Off by default.  While enabled,
+ * every call that runs the LM solve (b200reg_gicp_align, b200reg_icp_alignment, b200reg_loop_closure,
+ * b200reg_perform_loop_closure) records each trial of each pair.  The device buffer holds count x max_iterations x
+ * max(lm_max_iterations, 1) records (no pair can have more, nothing is truncated) and lives for the call only; if it cannot
+ * be allocated the call returns B200REG_ECUDA with the bytes in the message.  Tracing changes no result and no launch.
+ * With tracing disabled nothing is recorded or allocated, and such a call discards the stored trace.                    */
+int b200reg_ctx_set_lm_trace(b200reg_ctx* ctx, int enable);
+/* The trace of the context's most recent call that ran the LM solve, as CSR over that call's pairs (the CALLER's pair
+ * indices; a pair whose fine stage did not run -- invalid Quatro, no loop candidate -- has no records): the trials of pair
+ * i are trials_out[offsets_out[i] .. offsets_out[i + 1]), in execution order; offsets_out has count + 1 entries.  If the
+ * records exceed `capacity` the call fills offsets_out, writes nothing else and returns B200REG_ESTATE.  offsets_out ==
+ * NULL: returns that call's pair count (>= 0) and writes nothing.  Before any traced solve, or after an untraced one:
+ * B200REG_ESTATE.                                                                                                       */
+int b200reg_lm_trace(b200reg_ctx* ctx, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out);
 
 /* ---- clouds: replaces KdTreeFLANN::setInputCloud / buildIndex
  *      (third_party/nano_gicp/include/nano_gicp/nanoflann.hpp:131-138) ----------------- */
