@@ -293,6 +293,8 @@ class Context:
         return [Cloud(self, C.c_void_p(outs[i]), ns[i]) for i in range(cnt)]
 
     def covariances(self, clouds, k=15, method=3):
+        """NanoGICP::calculate_covariances for every cloud: any k >= 1 (all of the cloud when k >= n, still divided by k);
+        method is the RegularizationMethod (0 NONE, 1 MIN_EIG, 2 NORMALIZED_MIN_EIG, 3 PLANE, 4 FROBENIUS)."""
         arr = (C.c_void_p * len(clouds))(*[c.h for c in clouds])
         _check(lib().b200reg_clouds_covariances_ex(self.h, len(clouds), arr, int(k), int(method)))
 

@@ -316,14 +316,16 @@ int b200reg_cloud_destroy(b200reg_ctx* c, b200reg_cloud* cl) {
   return B200REG_OK;
 }
 
+// The plain entry point keeps its 1..32 range; b200reg_clouds_covariances_ex takes any k >= 1.
 int b200reg_clouds_covariances(b200reg_ctx* c, int count, b200reg_cloud* const* clouds, int k) {
+  if (k < 1 || k > 32) return fail(B200REG_EINVAL, "k_correspondences must be in 1..32 (b200reg_clouds_covariances_ex takes any k >= 1)");
   return b200reg_clouds_covariances_ex(c, count, clouds, k, 3);
 }
 
 int b200reg_clouds_covariances_ex(b200reg_ctx* c, int count, b200reg_cloud* const* clouds, int k, int method) {
   if (!c || count <= 0 || !clouds) return fail(B200REG_EINVAL, "bad argument");
   if (method < 0 || method > 4) return fail(B200REG_EINVAL, "regularization must be 0..4 (NONE, MIN_EIG, NORMALIZED_MIN_EIG, PLANE, FROBENIUS)");
-  if (k < 1 || k > 32) return fail(B200REG_EINVAL, "k_correspondences must be in 1..32");
+  if (k < 1) return fail(B200REG_EINVAL, "k_correspondences must be >= 1");
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Scratch scratch(c);
@@ -341,9 +343,11 @@ int b200reg_clouds_covariances_ex(b200reg_ctx* c, int count, b200reg_cloud* cons
   if (descs.empty()) return B200REG_OK;
   CloudDev* d_descs = nullptr;
   CU(scratch.upload(&d_descs, descs.data(), sizeof(CloudDev) * descs.size()));
+  unsigned long long* d_slab = nullptr;  // lists beyond shared memory (k > 256): one per warp, bounded (launchers.cuh)
+  if (const size_t slab = covariance_large_slab_bytes((int)descs.size(), max_n, k)) CU(scratch.alloc((void**)&d_slab, slab));
   {
     ProfScope ps(c, CLS_COV);
-    int l = launch_covariances(d_descs, (int)descs.size(), max_n, k, method, s);
+    int l = launch_covariances(d_descs, (int)descs.size(), max_n, k, method, d_slab, s);
     if (l < 0) return fail(B200REG_EINVAL, "unsupported k");
     c->launches += l;
     for (auto& d : descs) c->prof_bytes[CLS_COV] += 64.0 * d.n;  // SURVEY §8(d) K2

@@ -19,23 +19,8 @@
 namespace b200 {
 
 // ---------------------------------------------------------------------------------------
-// small fp64 helpers
+// small fp64 helpers (sym3_inverse and the covariance epilogue are in smallmath.cuh)
 // ---------------------------------------------------------------------------------------
-// inverse of a symmetric 3x3 given as (xx,xy,xz,yy,yz,zz); result in the same packing
-__device__ __forceinline__ void sym3_inverse(const double a[6], double o[6]) {
-  double c00 = a[3] * a[5] - a[4] * a[4];
-  double c01 = a[2] * a[4] - a[1] * a[5];
-  double c02 = a[1] * a[4] - a[2] * a[3];
-  double det = a[0] * c00 + a[1] * c01 + a[2] * c02;
-  double id = 1.0 / det;
-  o[0] = c00 * id;
-  o[1] = c01 * id;
-  o[2] = c02 * id;
-  o[3] = (a[0] * a[5] - a[2] * a[2]) * id;
-  o[4] = (a[1] * a[2] - a[0] * a[4]) * id;
-  o[5] = (a[0] * a[3] - a[1] * a[1]) * id;
-}
-
 // R C R^T for symmetric C (packed) and row-major R; packed symmetric result
 __device__ __forceinline__ void rcrt(const double R[9], const double c[6], double o[6]) {
   const double C[3][3] = {{c[0], c[1], c[2]}, {c[1], c[3], c[4]}, {c[2], c[4], c[5]}};
@@ -317,12 +302,12 @@ __global__ void __launch_bounds__(256) k_gicp_init(const PairDev* pairs, PairSta
 }
 
 // ---------------------------------------------------------------------------------------
-// K2: 15-NN + covariance + PLANE regularisation (nano_gicp_impl.hpp:298-357).
-// For symmetric PSD input U diag(1,1,eps) V^T == I - (1-eps) n n^T with n the eigenvector of
-// the smallest eigenvalue (SURVEY.md App. A.2), so only n is computed.
+// K2: 15-NN + covariance + PLANE regularisation (nano_gicp_impl.hpp:298-357); the regularisation is
+// cov_regularize_store (smallmath.cuh).
 // ---------------------------------------------------------------------------------------
 // K is the CAPACITY of the result set; k <= K neighbours enter the covariance (the k nearest of the K nearest are the
-// k nearest), so every k in 1..32 is served by the next instantiated capacity.
+// k nearest), so every k in 1..32 is served by the next instantiated capacity.  k > 32 runs k_covariance_large
+// (knn_large.cu), one warp per point.
 // The result set is a max-heap in shared memory (KnnHeap, knn.cuh): the covariance needs the SET of neighbours, not their
 // order.  (A sorted list in registers, the earlier design, spent most of its instructions in the insertion chain.)
 template <int K>
@@ -379,51 +364,7 @@ __global__ void __launch_bounds__(STEP_THREADS, (K <= 16 ? 10 : 4)) k_covariance
   }
   const double ik = 1.0 / k;
   cxx *= ik; cxy *= ik; cxz *= ik; cyy *= ik; cyz *= ik; czz *= ik;
-  double* o = c.cov + (size_t)i * 6;
-  if (method == 3) {  // PLANE, the default (nano_gicp_impl.hpp:61, 341-343)
-    double n[3];
-    sym3_smallest_evec(cxx, cxy, cxz, cyy, cyz, czz, n);
-    const double w = 1.0 - 1e-3;
-    o[0] = 1.0 - w * n[0] * n[0];
-    o[1] = -w * n[0] * n[1];
-    o[2] = -w * n[0] * n[2];
-    o[3] = 1.0 - w * n[1] * n[1];
-    o[4] = -w * n[1] * n[2];
-    o[5] = 1.0 - w * n[2] * n[2];
-    return;
-  }
-  // cold path: the other RegularizationMethods (nano_gicp_impl.hpp:323-353)
-  if (method == 0) {  // NONE
-    o[0] = cxx; o[1] = cxy; o[2] = cxz; o[3] = cyy; o[4] = cyz; o[5] = czz;
-  } else if (method == 4) {  // FROBENIUS: ((C + 1e-3 I)^-1 / ||.||_F)^-1 = ||(C + 1e-3 I)^-1||_F (C + 1e-3 I)
-    const double cl[6] = {cxx + 1e-3, cxy, cxz, cyy + 1e-3, cyz, czz + 1e-3};
-    double ci[6];
-    sym3_inverse(cl, ci);
-    const double nrm = sqrt(ci[0] * ci[0] + ci[3] * ci[3] + ci[5] * ci[5] + 2.0 * (ci[1] * ci[1] + ci[2] * ci[2] + ci[4] * ci[4]));
-#pragma unroll
-    for (int a = 0; a < 6; a++) o[a] = nrm * cl[a];
-  } else {  // MIN_EIG / NORMALIZED_MIN_EIG: sum_i max(f(s_i), 1e-3) u_i u_i^T
-    const double a6[6] = {cxx, cxy, cxz, cyy, cyz, czz};
-    double wv[3], V[3][3];
-    sym3_eigen_jacobi(a6, wv, V);
-    double vals[3];
-    const double mx = fmax(wv[0], fmax(wv[1], wv[2]));
-    for (int a = 0; a < 3; a++) {
-      const double sgl = fmax(wv[a], 0.0);  // singular value of a PSD matrix
-      vals[a] = fmax(method == 2 ? sgl / mx : sgl, 1e-3);
-    }
-    double r[6] = {0, 0, 0, 0, 0, 0};
-    for (int a = 0; a < 3; a++) {
-      r[0] += vals[a] * V[0][a] * V[0][a];
-      r[1] += vals[a] * V[0][a] * V[1][a];
-      r[2] += vals[a] * V[0][a] * V[2][a];
-      r[3] += vals[a] * V[1][a] * V[1][a];
-      r[4] += vals[a] * V[1][a] * V[2][a];
-      r[5] += vals[a] * V[2][a] * V[2][a];
-    }
-#pragma unroll
-    for (int a = 0; a < 6; a++) o[a] = r[a];
-  }
+  cov_regularize_store(c.cov + (size_t)i * 6, cxx, cxy, cxz, cyy, cyz, czz, method);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -797,9 +738,10 @@ __global__ void __launch_bounds__(256) k_transform_out(CloudDev c, const float* 
 // ---------------------------------------------------------------------------------------
 // host launchers
 // ---------------------------------------------------------------------------------------
-int launch_covariances(const CloudDev* d_clouds, int count, int max_n, int k, int method, cudaStream_t s) {
+int launch_covariances(const CloudDev* d_clouds, int count, int max_n, int k, int method, unsigned long long* slab, cudaStream_t s) {
   dim3 grid((max_n + STEP_THREADS - 1) / STEP_THREADS, count);
-  if (k < 1 || k > 32 || method < 0 || method > 4) return -1;
+  if (k < 1 || method < 0 || method > 4) return -1;
+  if (k > 32) return launch_covariance_large(d_clouds, count, max_n, k, method, slab, s);
   if (k <= 8) k_covariance<8><<<grid, STEP_THREADS, 0, s>>>(d_clouds, k, method);
   else if (k <= 15) k_covariance<15><<<grid, STEP_THREADS, 0, s>>>(d_clouds, k, method);
   else if (k <= 20) k_covariance<20><<<grid, STEP_THREADS, 0, s>>>(d_clouds, k, method);

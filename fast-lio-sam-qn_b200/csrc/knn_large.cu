@@ -23,8 +23,14 @@
 // kernel does not walk the tree for it.
 // The answer is the k smallest keys of the cloud, a set that does not depend on the walk order: chunking, query order and
 // repeated calls return identical bytes.
+// k_covariance_large (b200reg_clouds_covariances_ex, k > 32) runs the same walk for every point of its clouds and sums the
+// moments of the list it leaves.
+#include <algorithm>
+#include <climits>
+
 #include "knn.cuh"
 #include "launchers.cuh"
+#include "smallmath.cuh"
 
 namespace b200 {
 
@@ -196,13 +202,106 @@ __global__ void __launch_bounds__(KL_THREADS) k_knn_large(CloudDev c, const floa
 }
 
 // ---------------------------------------------------------------------------------------
-// host launcher
+// k > 32 covariances (nano_gicp_impl.hpp:298-357): one warp per point
+// ---------------------------------------------------------------------------------------
+// Work item it = cloud * max_n + point covers every cloud of the call in one launch; items past a cloud's size are skipped,
+// and the items are strided over the grid's warps.  The neighbour list of a point is its m = min(k, n) nearest points of
+// its own cloud (itself included), found by kl_walk: ascending (d2, original index), all of the cloud once k >= n.  A warp
+// reuses one list for all its items: in shared memory when m <= KL_SMEM_K, else at slab + (global warp) * lstride.
+// The moments follow the oracle's operation order (oracle_gicp.cpp:214-232, the reference's rowwise().mean() and
+// / k_correspondences_), so the unregularised covariance is bit-identical to it wherever the lists agree: lanes 0..2 each
+// sum one coordinate in list order and divide by k; lanes 0..5 then each sum one product (xa - ma) (xb - mb) in list order
+// and divide by k -- fp64, no FMA, the divisor k even when fewer than k points exist.  (A lane-parallel tree sum would be
+// faster but would not be that order.)  Lane 0 regularises and stores.
+template <bool SMEM_LIST>
+__global__ void __launch_bounds__(KL_THREADS) k_covariance_large(const CloudDev* clouds, int max_n, long long items, int k, int method,
+                                                                 unsigned long long* slab, int lstride) {
+  __shared__ unsigned long long s_list[SMEM_LIST ? KL_WARPS * KL_SMEM_K : 1];
+  __shared__ unsigned long long s_stage[KL_WARPS][KL_STAGE];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long gw = (long long)blockIdx.x * KL_WARPS + warp;
+  unsigned long long* list = SMEM_LIST ? s_list + warp * KL_SMEM_K : slab + gw * lstride;
+  // the covariance term of lane t < 6: (xx, xy, xz, yy, yz, zz)
+  const int ta = lane < 3 ? 0 : lane < 5 ? 1 : 2, tb = lane < 3 ? lane : lane < 5 ? lane - 2 : 2;
+  const double dk = (double)k;
+  for (long long it = gw; it < items; it += (long long)gridDim.x * KL_WARPS) {
+    const CloudDev& c = clouds[it / max_n];
+    const int i = (int)(it % max_n);
+    if (i >= c.n) continue;  // the whole warp
+    const int m = min(k, c.n);
+    const float4 q = c.pts[i];
+    for (int j = lane; j < m; j += 32) list[j] = KL_PAD;
+    __syncwarp();
+    if (!(isnan(q.x) || isnan(q.y) || isnan(q.z))) kl_walk(c, q.x, q.y, q.z, m, list, s_stage[warp]);
+    __syncwarp();
+    // original index -> sorted position, in place; padding (no neighbour) keeps index -1
+    for (int j = lane; j < m; j += 32) {
+      const unsigned o = (unsigned)list[j];
+      if (o != 0xFFFFFFFFu) list[j] = (unsigned)c.rank[o];
+    }
+    __syncwarp();
+    const float* __restrict__ pf = reinterpret_cast<const float*>(c.pts);
+    double mean = 0.0;
+    if (lane < 3) {
+      for (int j = 0; j < m; j++) {
+        const unsigned p = (unsigned)list[j];
+        if (p != 0xFFFFFFFFu) mean = __dadd_rn(mean, (double)__ldg(&pf[4 * (size_t)p + lane]));
+      }
+      mean = __ddiv_rn(mean, dk);
+    }
+    const double mx = __shfl_sync(KL_FULL, mean, 0), my = __shfl_sync(KL_FULL, mean, 1), mz = __shfl_sync(KL_FULL, mean, 2);
+    double acc = 0.0;
+    if (lane < 6) {
+      const double ma = ta == 0 ? mx : ta == 1 ? my : mz, mb = tb == 0 ? mx : tb == 1 ? my : mz;
+      for (int j = 0; j < m; j++) {
+        const unsigned p = (unsigned)list[j];
+        if (p == 0xFFFFFFFFu) continue;
+        const double da = __dsub_rn((double)__ldg(&pf[4 * (size_t)p + ta]), ma);
+        const double db = __dsub_rn((double)__ldg(&pf[4 * (size_t)p + tb]), mb);
+        acc = __dadd_rn(acc, __dmul_rn(da, db));
+      }
+      acc = __ddiv_rn(acc, dk);
+    }
+    double cv[6];
+#pragma unroll
+    for (int t = 0; t < 6; t++) cv[t] = __shfl_sync(KL_FULL, acc, t);
+    if (lane == 0) cov_regularize_store(c.cov + (size_t)i * 6, cv[0], cv[1], cv[2], cv[3], cv[4], cv[5], method);
+    __syncwarp();  // every lane has read the list before the next item refills it
+  }
+}
+
+// ---------------------------------------------------------------------------------------
+// host launchers
 // ---------------------------------------------------------------------------------------
 int launch_knn_large(const CloudDev& c, const float* d_q, int nq, int qstride, int k, unsigned long long* slab, int* idx, float* d2,
                      cudaStream_t s) {
   const int grid = (nq + KL_WARPS - 1) / KL_WARPS;
   if (k <= KL_SMEM_K) k_knn_large<true><<<grid, KL_THREADS, 0, s>>>(c, d_q, nq, qstride, k, slab, idx, d2);
   else k_knn_large<false><<<grid, KL_THREADS, 0, s>>>(c, d_q, nq, qstride, k, slab, idx, d2);
+  return 1;
+}
+
+// k_covariance_large's grid: one warp per item, capped for slab lists so that the slab stays within KL_COV_SLAB_BYTES
+// (but holds at least one block's lists).
+static int cov_large_blocks(int count, int max_n, int k) {
+  const long long items = (long long)count * max_n, lstride = std::min(k, max_n);
+  long long blocks = (items + KL_WARPS - 1) / KL_WARPS;
+  if (lstride > KL_SMEM_K) blocks = std::min(blocks, std::max(1LL, (long long)(KL_COV_SLAB_BYTES / (KL_WARPS * lstride * 8))));
+  return (int)std::min(blocks, (long long)INT_MAX);
+}
+
+size_t covariance_large_slab_bytes(int count, int max_n, int k) {
+  const int lstride = std::min(k, max_n);
+  if (lstride <= KL_SMEM_K) return 0;
+  return (size_t)cov_large_blocks(count, max_n, k) * KL_WARPS * lstride * 8;
+}
+
+int launch_covariance_large(const CloudDev* d_clouds, int count, int max_n, int k, int method, unsigned long long* slab,
+                            cudaStream_t s) {
+  const int lstride = std::min(k, max_n), grid = cov_large_blocks(count, max_n, k);
+  const long long items = (long long)count * max_n;
+  if (lstride <= KL_SMEM_K) k_covariance_large<true><<<grid, KL_THREADS, 0, s>>>(d_clouds, max_n, items, k, method, slab, lstride);
+  else k_covariance_large<false><<<grid, KL_THREADS, 0, s>>>(d_clouds, max_n, items, k, method, slab, lstride);
   return 1;
 }
 

@@ -13,8 +13,9 @@ int radix_sort_result_buf(int key_bits);
 int launch_radix_sort(const CloudDev* d_clouds, int count, int max_n, int key_bits, cudaStream_t s);
 int launch_index_build(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s);
 
-// gicp.cu
-int launch_covariances(const CloudDev* d_clouds, int count, int max_n, int k, int method, cudaStream_t s);
+// gicp.cu.  launch_covariances: k <= 32 one thread per point; k > 32 goes to launch_covariance_large and needs
+// covariance_large_slab_bytes(count, max_n, k) of device scratch in slab (nullptr when that is 0)
+int launch_covariances(const CloudDev* d_clouds, int count, int max_n, int k, int method, unsigned long long* slab, cudaStream_t s);
 void launch_gicp_init(const PairDev* pairs, PairState* states, const double* d_guess, LmCall* call, LmSched* sched, cudaStream_t s);
 void launch_gicp_search(const PairDev* pairs, const PairState* states, int blocks, const LmCall* call, const LmSched* sched, cudaStream_t s);
 void launch_gicp_accum(const PairDev* pairs, const PairState* states, int blocks, const LmSched* sched, cudaStream_t s);
@@ -61,6 +62,14 @@ int launch_radius_gather(const uint32_t* perm, int m, const int* e_idx, const fl
 constexpr int KL_SMEM_K = 256;
 int launch_knn_large(const CloudDev& c, const float* d_q, int nq, int qstride, int k, unsigned long long* slab, int* idx, float* d2,
                      cudaStream_t s);
+// Covariances for k > 32, one warp per point, every cloud of the call in one launch.  A warp's neighbour list holds
+// min(k, max_n) keys; lists longer than KL_SMEM_K live in a slab with one list per warp of the grid, not per point, so the
+// launcher caps the grid to keep the slab at or below max(KL_COV_SLAB_BYTES, one 4-warp block's lists = 32 * min(k, max_n)
+// bytes) whatever the cloud sizes.  covariance_large_slab_bytes is that slab's exact size (0 for the shared-memory tier).
+constexpr size_t KL_COV_SLAB_BYTES = size_t(128) << 20;
+size_t covariance_large_slab_bytes(int count, int max_n, int k);
+int launch_covariance_large(const CloudDev* d_clouds, int count, int max_n, int k, int method, unsigned long long* slab,
+                            cudaStream_t s);
 
 // assemble.cu
 void launch_pack_xyzi(const float* d_raw, int stride, int n, float4* d_out, cudaStream_t s);

@@ -1,4 +1,4 @@
-// smallmath.cuh -- tiny fp64 device helpers shared by gicp.cu and quatro.cu.
+// smallmath.cuh -- tiny fp64 device helpers shared by gicp.cu, knn_large.cu and quatro.cu.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -93,6 +93,74 @@ static __device__ __noinline__ void sym3_eigen_jacobi(const double a[6], double 
     }
   }
   w[0] = A[0][0]; w[1] = A[1][1]; w[2] = A[2][2];
+}
+
+// inverse of a symmetric 3x3 given as (xx,xy,xz,yy,yz,zz); result in the same packing
+__device__ __forceinline__ void sym3_inverse(const double a[6], double o[6]) {
+  double c00 = a[3] * a[5] - a[4] * a[4];
+  double c01 = a[2] * a[4] - a[1] * a[5];
+  double c02 = a[1] * a[4] - a[2] * a[3];
+  double det = a[0] * c00 + a[1] * c01 + a[2] * c02;
+  double id = 1.0 / det;
+  o[0] = c00 * id;
+  o[1] = c01 * id;
+  o[2] = c02 * id;
+  o[3] = (a[0] * a[5] - a[2] * a[2]) * id;
+  o[4] = (a[1] * a[2] - a[0] * a[4]) * id;
+  o[5] = (a[0] * a[3] - a[1] * a[1]) * id;
+}
+
+// RegularizationMethod (nano_gicp_impl.hpp:323-353) of the covariance (cxx, cxy, cxz, cyy, cyz, czz), stored packed at o.
+// method: 0 NONE, 1 MIN_EIG, 2 NORMALIZED_MIN_EIG, 3 PLANE, 4 FROBENIUS.  The epilogue of both covariance kernels
+// (k_covariance in gicp.cu, k_covariance_large in knn_large.cu).
+// PLANE: for symmetric PSD input U diag(1,1,eps) V^T == I - (1-eps) n n^T with n the eigenvector of the smallest
+// eigenvalue (SURVEY.md App. A.2), so only n is computed.
+__device__ __forceinline__ void cov_regularize_store(double* o, double cxx, double cxy, double cxz, double cyy, double cyz,
+                                                     double czz, int method) {
+  if (method == 3) {  // PLANE, the default (nano_gicp_impl.hpp:61, 341-343)
+    double n[3];
+    sym3_smallest_evec(cxx, cxy, cxz, cyy, cyz, czz, n);
+    const double w = 1.0 - 1e-3;
+    o[0] = 1.0 - w * n[0] * n[0];
+    o[1] = -w * n[0] * n[1];
+    o[2] = -w * n[0] * n[2];
+    o[3] = 1.0 - w * n[1] * n[1];
+    o[4] = -w * n[1] * n[2];
+    o[5] = 1.0 - w * n[2] * n[2];
+    return;
+  }
+  // cold path: the other RegularizationMethods (nano_gicp_impl.hpp:323-353)
+  if (method == 0) {  // NONE
+    o[0] = cxx; o[1] = cxy; o[2] = cxz; o[3] = cyy; o[4] = cyz; o[5] = czz;
+  } else if (method == 4) {  // FROBENIUS: ((C + 1e-3 I)^-1 / ||.||_F)^-1 = ||(C + 1e-3 I)^-1||_F (C + 1e-3 I)
+    const double cl[6] = {cxx + 1e-3, cxy, cxz, cyy + 1e-3, cyz, czz + 1e-3};
+    double ci[6];
+    sym3_inverse(cl, ci);
+    const double nrm = sqrt(ci[0] * ci[0] + ci[3] * ci[3] + ci[5] * ci[5] + 2.0 * (ci[1] * ci[1] + ci[2] * ci[2] + ci[4] * ci[4]));
+#pragma unroll
+    for (int a = 0; a < 6; a++) o[a] = nrm * cl[a];
+  } else {  // MIN_EIG / NORMALIZED_MIN_EIG: sum_i max(f(s_i), 1e-3) u_i u_i^T
+    const double a6[6] = {cxx, cxy, cxz, cyy, cyz, czz};
+    double wv[3], V[3][3];
+    sym3_eigen_jacobi(a6, wv, V);
+    double vals[3];
+    const double mx = fmax(wv[0], fmax(wv[1], wv[2]));
+    for (int a = 0; a < 3; a++) {
+      const double sgl = fmax(wv[a], 0.0);  // singular value of a PSD matrix
+      vals[a] = fmax(method == 2 ? sgl / mx : sgl, 1e-3);
+    }
+    double r[6] = {0, 0, 0, 0, 0, 0};
+    for (int a = 0; a < 3; a++) {
+      r[0] += vals[a] * V[0][a] * V[0][a];
+      r[1] += vals[a] * V[0][a] * V[1][a];
+      r[2] += vals[a] * V[0][a] * V[2][a];
+      r[3] += vals[a] * V[1][a] * V[1][a];
+      r[4] += vals[a] * V[1][a] * V[2][a];
+      r[5] += vals[a] * V[2][a] * V[2][a];
+    }
+#pragma unroll
+    for (int a = 0; a < 6; a++) o[a] = r[a];
+  }
 }
 
 }  // namespace b200

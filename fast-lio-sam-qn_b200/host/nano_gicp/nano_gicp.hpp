@@ -10,7 +10,8 @@
 //   * the class does not derive from pcl::Registration (nothing in fast_lio_sam_qn/src uses it polymorphically);
 //   * setNumThreads is accepted and ignored; RANSAC* / EuclideanFitnessEpsilon setters are stored and never read,
 //     exactly like the reference's LSQ path (SURVEY.md §8b);
-//   * all five RegularizationMethods are built (PLANE is the default, nano_gicp_impl.hpp:61); k may be 1..32;
+//   * all five RegularizationMethods are built (PLANE is the default, nano_gicp_impl.hpp:61); setCorrespondenceRandomness takes
+//     any k >= 1 (k > 32 computes the covariances one warp per point, b200reg_clouds_covariances_ex);
 //   * source_kdtree_/target_kdtree_ are nanoflann::KdTreeFLANN facades (nanoflann.hpp in this directory) over the SAME device
 //     cloud and index the class builds for registration: no second upload, no second build;
 //   * covariances live on the device and are materialised on the host lazily by getSource/TargetCovariances() as

@@ -49,7 +49,7 @@ typedef struct b200reg_cloud b200reg_cloud;
 /* Mirrors NanoGICPConfig (fast_lio_sam_qn/include/loop_closure.h:25-36) + the LsqRegistration
  * constructor defaults (third_party/nano_gicp/include/nano_gicp/impl/lsq_registration_impl.hpp:49-63). */
 typedef struct b200reg_gicp_params {
-  int32_t k_correspondences;     /* setCorrespondenceRandomness, loop_closure.cpp:10 (15)   */
+  int32_t k_correspondences;     /* setCorrespondenceRandomness, loop_closure.cpp:10 (15); any k >= 1 */
   int32_t max_iterations;        /* setMaximumIterations, loop_closure.cpp:11 (32)          */
   double max_corr_dist;          /* setMaxCorrespondenceDistance, loop_closure.cpp:13 (52.5)*/
   double transformation_eps;     /* setTransformationEpsilon, loop_closure.cpp:14 (0.01)    */
@@ -185,13 +185,19 @@ int b200reg_cloud_destroy(b200reg_ctx* ctx, b200reg_cloud* cloud);
 size_t b200reg_cloud_size(const b200reg_cloud* cloud);
 
 /* NanoGICP::calculateSourceCovariances / calculateTargetCovariances
- * (third_party/nano_gicp/include/nano_gicp/impl/nano_gicp_impl.hpp:151-159, 298-357), batched. */
+ * (third_party/nano_gicp/include/nano_gicp/impl/nano_gicp_impl.hpp:151-159, 298-357), batched.  k in 1..32 here;
+ * b200reg_clouds_covariances_ex takes any k >= 1. */
 int b200reg_clouds_covariances(b200reg_ctx* ctx, int count, b200reg_cloud* const* clouds, int k);
 /* NanoGICP::setSourceCovariances / setTargetCovariances (nano_gicp.hpp:91-93, nano_gicp_impl.hpp:142-150): the caller's
  * per-point covariances (n x 9 doubles: the row-major 3x3 block of each Matrix4d, ORIGINAL point order) replace the
  * computed ones; align() then does not recompute them (nano_gicp_impl.hpp:162-167) until the input cloud changes.   */
 int b200reg_set_covariances(b200reg_ctx* ctx, b200reg_cloud* cloud, const double* cov9, size_t n);
-/* Same with an explicit RegularizationMethod (setRegularizationMethod, nano_gicp.hpp:84); the plain call uses PLANE. */
+/* Same with an explicit RegularizationMethod (setRegularizationMethod, nano_gicp.hpp:84); the plain call uses PLANE.
+ * Any k >= 1 (setCorrespondenceRandomness): each point's k nearest points of its own cloud, itself included; all of the
+ * cloud when k >= n, the mean and covariance still divided by k.  k <= 32 runs one thread per point; k > 32 one warp per
+ * point, O(k) per point, with the moments summed in neighbour order ((d2, original index), fp64, no FMA).  Its neighbour
+ * lists live in shared memory up to 256 entries and beyond that in device scratch of one list per resident warp, at most
+ * max(128 MiB, 32 * min(k, largest cloud) bytes) per call whatever the cloud sizes.                                  */
 int b200reg_clouds_covariances_ex(b200reg_ctx* ctx, int count, b200reg_cloud* const* clouds, int k, int method);
 
 /* ---- registration ----------------------------------------------------------------- */
