@@ -4,66 +4,9 @@
 
 namespace b200 {
 
-// Eigenvector of the smallest eigenvalue of a symmetric 3x3, fp64, non-iterative:
-// eigenvalue by the trigonometric closed form on the matrix scaled to unit max entry, eigenvector as the
-// best-conditioned cross product of two rows of (A - lambda I), then ONE inverse-iteration-free polish by
-// re-orthogonalising against the residual.  (A cyclic-Jacobi version was measured first: its fp64 div/sqrt chains
-// were ~30% of k_covariance's instructions.)  Accuracy ~1e-13 relative for the plane-like neighbourhoods GICP uses;
-// when the two smallest eigenvalues coincide any vector of that eigenspace is returned, as with an SVD.
-__device__ __forceinline__ void sym3_smallest_evec(double a00, double a01, double a02, double a11, double a12,
-                                                   double a22, double n[3]) {
-  const double mx = fmax(fmax(fmax(fabs(a00), fabs(a01)), fmax(fabs(a02), fabs(a11))), fmax(fabs(a12), fabs(a22)));
-  if (mx == 0.0) {
-    n[0] = 0.0; n[1] = 0.0; n[2] = 1.0;
-    return;
-  }
-  const double is = 1.0 / mx;
-  a00 *= is; a01 *= is; a02 *= is; a11 *= is; a12 *= is; a22 *= is;
-  const double off = a01 * a01 + a02 * a02 + a12 * a12;
-  double lam;
-  if (off == 0.0) {
-    lam = fmin(a00, fmin(a11, a22));
-  } else {
-    const double q = (a00 + a11 + a22) * (1.0 / 3.0);
-    const double b00 = a00 - q, b11 = a11 - q, b22 = a22 - q;
-    const double p = sqrt((b00 * b00 + b11 * b11 + b22 * b22 + 2.0 * off) * (1.0 / 6.0));
-    const double ip = 1.0 / p;
-    const double c00 = b00 * ip, c01 = a01 * ip, c02 = a02 * ip, c11 = b11 * ip, c12 = a12 * ip, c22 = b22 * ip;
-    double r = 0.5 * (c00 * (c11 * c22 - c12 * c12) - c01 * (c01 * c22 - c12 * c02) + c02 * (c01 * c12 - c11 * c02));
-    r = fmin(1.0, fmax(-1.0, r));
-    const double phi = acos(r) * (1.0 / 3.0);
-    lam = q + 2.0 * p * cos(phi + 2.0943951023931954923);  // smallest root
-  }
-  // rows of (A - lam I); the eigenvector is orthogonal to all three
-  const double r0x = a00 - lam, r0y = a01, r0z = a02;
-  const double r1x = a01, r1y = a11 - lam, r1z = a12;
-  const double r2x = a02, r2y = a12, r2z = a22 - lam;
-  const double c0x = r0y * r1z - r0z * r1y, c0y = r0z * r1x - r0x * r1z, c0z = r0x * r1y - r0y * r1x;
-  const double c1x = r0y * r2z - r0z * r2y, c1y = r0z * r2x - r0x * r2z, c1z = r0x * r2y - r0y * r2x;
-  const double c2x = r1y * r2z - r1z * r2y, c2y = r1z * r2x - r1x * r2z, c2z = r1x * r2y - r1y * r2x;
-  const double d0 = c0x * c0x + c0y * c0y + c0z * c0z, d1 = c1x * c1x + c1y * c1y + c1z * c1z,
-               d2 = c2x * c2x + c2y * c2y + c2z * c2z;
-  double vx = c0x, vy = c0y, vz = c0z, dm = d0;
-  if (d1 > dm) { vx = c1x; vy = c1y; vz = c1z; dm = d1; }
-  if (d2 > dm) { vx = c2x; vy = c2y; vz = c2z; dm = d2; }
-  if (dm == 0.0) {  // (A - lam I) has rank <= 1: pick any vector orthogonal to its dominant row
-    double rx = r0x, ry = r0y, rz = r0z;
-    double rm = r0x * r0x + r0y * r0y + r0z * r0z;
-    const double m1 = r1x * r1x + r1y * r1y + r1z * r1z, m2 = r2x * r2x + r2y * r2y + r2z * r2z;
-    if (m1 > rm) { rx = r1x; ry = r1y; rz = r1z; rm = m1; }
-    if (m2 > rm) { rx = r2x; ry = r2y; rz = r2z; rm = m2; }
-    if (rm == 0.0) { n[0] = 0.0; n[1] = 0.0; n[2] = 1.0; return; }
-    if (fabs(rx) <= fabs(ry) && fabs(rx) <= fabs(rz)) { vx = 0.0; vy = -rz; vz = ry; }
-    else if (fabs(ry) <= fabs(rz)) { vx = -rz; vy = 0.0; vz = rx; }
-    else { vx = -ry; vy = rx; vz = 0.0; }
-    dm = vx * vx + vy * vy + vz * vz;
-  }
-  const double inv = rsqrt(dm);
-  n[0] = vx * inv; n[1] = vy * inv; n[2] = vz * inv;
-}
-
 // Full eigen-decomposition of a symmetric 3x3 by cyclic Jacobi (fp64): eigenvalues in w (unsorted), eigenvectors in
-// the columns of V.  Only the non-default regularisation methods need it (cold path).
+// the columns of V.  The non-default regularisation methods and sym3_smallest_evec's near-degenerate case need it (cold
+// paths).
 static __device__ __noinline__ void sym3_eigen_jacobi(const double a[6], double w[3], double V[3][3]) {
   double A[3][3] = {{a[0], a[1], a[2]}, {a[1], a[3], a[4]}, {a[2], a[4], a[5]}};
   for (int i = 0; i < 3; i++)
@@ -93,6 +36,79 @@ static __device__ __noinline__ void sym3_eigen_jacobi(const double a[6], double 
     }
   }
   w[0] = A[0][0]; w[1] = A[1][1]; w[2] = A[2][2];
+}
+
+// Eigenvector of the smallest eigenvalue of a symmetric 3x3, fp64, non-iterative:
+// eigenvalue by the trigonometric closed form on the matrix scaled to unit max entry, eigenvector as the
+// best-conditioned cross product of two rows of (A - lambda I), then ONE inverse-iteration-free polish by
+// re-orthogonalising against the residual.  (A cyclic-Jacobi version was measured first: its fp64 div/sqrt chains
+// were ~30% of k_covariance's instructions.)  Accuracy ~1e-13 relative for the plane-like neighbourhoods GICP uses;
+// when the two smallest eigenvalues coincide any vector of that eigenspace is returned, as with an SVD.
+// Where the two smallest eigenvalues are g apart with g << p (the spread; near-collinear neighbourhoods: poles, edges),
+// r -> 1 and acos has infinite slope there: the closed-form lambda errs by ~eps p^2 / g and the cross products turn that
+// into an eigenvector error ~eps (p/g)^2, where the problem itself only allows ~eps p / g (an fp64 restatement of this
+// code errs by 3e-5 rad on near-collinear points of a raw scan; one Rayleigh-quotient refinement of lambda was measured
+// to leave errors of 0.4 rad on a 2e-4 m-thick edge, where lambda's error exceeds g).  So below phi = 1e-3
+// (g / p ~ 3.5e-3) the vector comes from the backward-stable cyclic Jacobi instead
+// (tests/test_gpu_fpfh_dense.py checks the normals against that eigen-gap bound).
+__device__ __forceinline__ void sym3_smallest_evec(double a00, double a01, double a02, double a11, double a12,
+                                                   double a22, double n[3]) {
+  const double mx = fmax(fmax(fmax(fabs(a00), fabs(a01)), fmax(fabs(a02), fabs(a11))), fmax(fabs(a12), fabs(a22)));
+  if (mx == 0.0) {
+    n[0] = 0.0; n[1] = 0.0; n[2] = 1.0;
+    return;
+  }
+  const double is = 1.0 / mx;
+  a00 *= is; a01 *= is; a02 *= is; a11 *= is; a12 *= is; a22 *= is;
+  const double off = a01 * a01 + a02 * a02 + a12 * a12;
+  double lam;
+  if (off == 0.0) {
+    lam = fmin(a00, fmin(a11, a22));
+  } else {
+    const double q = (a00 + a11 + a22) * (1.0 / 3.0);
+    const double b00 = a00 - q, b11 = a11 - q, b22 = a22 - q;
+    const double p = sqrt((b00 * b00 + b11 * b11 + b22 * b22 + 2.0 * off) * (1.0 / 6.0));
+    const double ip = 1.0 / p;
+    const double c00 = b00 * ip, c01 = a01 * ip, c02 = a02 * ip, c11 = b11 * ip, c12 = a12 * ip, c22 = b22 * ip;
+    double r = 0.5 * (c00 * (c11 * c22 - c12 * c12) - c01 * (c01 * c22 - c12 * c02) + c02 * (c01 * c12 - c11 * c02));
+    r = fmin(1.0, fmax(-1.0, r));
+    const double phi = acos(r) * (1.0 / 3.0);
+    if (phi < 1e-3) {  // the two smallest eigenvalues nearly coincide: see above
+      const double a6[6] = {a00, a01, a02, a11, a12, a22};
+      double w[3], V[3][3];
+      sym3_eigen_jacobi(a6, w, V);
+      const int k = w[0] <= w[1] ? (w[0] <= w[2] ? 0 : 2) : (w[1] <= w[2] ? 1 : 2);
+      n[0] = V[0][k]; n[1] = V[1][k]; n[2] = V[2][k];
+      return;
+    }
+    lam = q + 2.0 * p * cos(phi + 2.0943951023931954923);  // smallest root
+  }
+  // rows of (A - lam I); the eigenvector is orthogonal to all three
+  const double r0x = a00 - lam, r0y = a01, r0z = a02;
+  const double r1x = a01, r1y = a11 - lam, r1z = a12;
+  const double r2x = a02, r2y = a12, r2z = a22 - lam;
+  const double c0x = r0y * r1z - r0z * r1y, c0y = r0z * r1x - r0x * r1z, c0z = r0x * r1y - r0y * r1x;
+  const double c1x = r0y * r2z - r0z * r2y, c1y = r0z * r2x - r0x * r2z, c1z = r0x * r2y - r0y * r2x;
+  const double c2x = r1y * r2z - r1z * r2y, c2y = r1z * r2x - r1x * r2z, c2z = r1x * r2y - r1y * r2x;
+  const double d0 = c0x * c0x + c0y * c0y + c0z * c0z, d1 = c1x * c1x + c1y * c1y + c1z * c1z,
+               d2 = c2x * c2x + c2y * c2y + c2z * c2z;
+  double vx = c0x, vy = c0y, vz = c0z, dm = d0;
+  if (d1 > dm) { vx = c1x; vy = c1y; vz = c1z; dm = d1; }
+  if (d2 > dm) { vx = c2x; vy = c2y; vz = c2z; dm = d2; }
+  if (dm == 0.0) {  // (A - lam I) has rank <= 1: pick any vector orthogonal to its dominant row
+    double rx = r0x, ry = r0y, rz = r0z;
+    double rm = r0x * r0x + r0y * r0y + r0z * r0z;
+    const double m1 = r1x * r1x + r1y * r1y + r1z * r1z, m2 = r2x * r2x + r2y * r2y + r2z * r2z;
+    if (m1 > rm) { rx = r1x; ry = r1y; rz = r1z; rm = m1; }
+    if (m2 > rm) { rx = r2x; ry = r2y; rz = r2z; rm = m2; }
+    if (rm == 0.0) { n[0] = 0.0; n[1] = 0.0; n[2] = 1.0; return; }
+    if (fabs(rx) <= fabs(ry) && fabs(rx) <= fabs(rz)) { vx = 0.0; vy = -rz; vz = ry; }
+    else if (fabs(ry) <= fabs(rz)) { vx = -rz; vy = 0.0; vz = rx; }
+    else { vx = -ry; vy = rx; vz = 0.0; }
+    dm = vx * vx + vy * vy + vz * vz;
+  }
+  const double inv = rsqrt(dm);
+  n[0] = vx * inv; n[1] = vy * inv; n[2] = vz * inv;
 }
 
 // inverse of a symmetric 3x3 given as (xx,xy,xz,yy,yz,zz); result in the same packing
