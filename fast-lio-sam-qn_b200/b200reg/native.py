@@ -451,17 +451,22 @@ class Context:
         total = int(offsets[-1])
         return offsets, idx[:total], d2[:total]
 
-    def quatro_solve_tap(self, src_xyz, dst_xyz, params=None, wide=False):
-        """The TEASER++ solve of the advancedMatching path on given correspondences (row i of src_xyz joined to row i of
-        dst_xyz) -> info dict with "clique" (ascending correspondence indices).  wide: the path of sets beyond ADV_MAXC."""
+    TAP_PATHS = {"global": 0, "wide": 1, "shared": 2}
+
+    def quatro_solve_tap(self, src_xyz, dst_xyz, params=None, wide=False, path=None):
+        """The TEASER++ solve on given correspondences (row i of src_xyz joined to row i of dst_xyz) -> info dict with
+        "clique" (ascending correspondence indices).  path: "shared" (optimizedMatching's solver, at most 512
+        correspondences), "global" (advancedMatching's, at most 8192) or "wide" (advancedMatching's beyond 8192); without
+        it, wide=True picks "wide" and wide=False "global"."""
         S = np.ascontiguousarray(np.asarray(src_xyz)[:, :3], np.float32)
         D = np.ascontiguousarray(np.asarray(dst_xyz)[:, :3], np.float32)
         assert S.shape == D.shape
+        code = self.TAP_PATHS[path if path is not None else ("wide" if wide else "global")]
         prm = params or default_quatro_params()
         info = QuatroInfo()
         clique = np.empty(len(S), np.int32)
         _check(lib().b200reg_quatro_solve_tap(self.h, len(S), S.ctypes.data_as(C.c_void_p), D.ctypes.data_as(C.c_void_p),
-                                              int(bool(wide)), C.byref(prm), C.byref(info), clique.ctypes.data_as(C.c_void_p)))
+                                              code, C.byref(prm), C.byref(info), clique.ctypes.data_as(C.c_void_p)))
         out = info.as_dict()
         out["clique"] = clique[:out["clique_size"]].copy()
         return out

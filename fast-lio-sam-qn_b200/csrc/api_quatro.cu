@@ -454,43 +454,85 @@ int b200reg_quatro_solve_tap(b200reg_ctx* c, int n, const float* src_xyz, const 
                              const b200reg_quatro_params* prm, b200reg_quatro_info* info, int32_t* clique_out) {
   if (!c || n < 1 || n >= BIG_NMAX || !src_xyz || !dst_xyz || !prm || !info) return fail(B200REG_EINVAL, "bad argument");
   if (!wide && n > BIGC) return fail(B200REG_EINVAL, "wide = 0 solves at most B200REG_ADV_CORR_CAPACITY correspondences");
+  if (wide == 2 && n > MAXC) return fail(B200REG_EINVAL, "wide = 2 solves at most B200REG_CORR_CAPACITY correspondences");
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Scratch scratch(c);
-  std::vector<double> S(3 * (size_t)n), D(3 * (size_t)n);
-  for (size_t k = 0; k < 3 * (size_t)n; k++) {
-    S[k] = src_xyz[k];  // k_big_gather's float -> double
-    D[k] = dst_xyz[k];
-  }
-  // the workspace b200reg_quatro_align gives a set of this size on each path
-  const int cap = wide ? (n + 1023) / 1024 * 1024 : std::max(1024, pow2_at_least(n));
-  Layout l;
-  const size_t o_big = l.take(sizeof(BigSolveWs)), o_cnt = l.take(8 * 4), o_T = l.take(16 * 8), o_pair = l.take(sizeof(MatchDev));
-  const BigWsLayout wl(l, cap, 0);
-  char* slab = nullptr;
-  CU(scratch.alloc((void**)&slab, l.size));
-  const BigSolveWs w = wl.bind(slab);
-  MatchDev m{};
-  m.counters = (int*)(slab + o_cnt);
-  m.T = (double*)(slab + o_T);
-  m.big = (BigSolveWs*)(slab + o_big);
   const int counters[8] = {0, n, n, 0, 0, 0, 0, 0};
-  double T[16];
-  for (int k = 0; k < 16; k++) T[k] = (k % 5 == 0) ? 1.0 : 0.0;
-  CU(cudaMemcpyAsync(w.S, S.data(), S.size() * 8, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(w.D, D.data(), D.size() * 8, cudaMemcpyHostToDevice, s));
-  CU(cudaMemsetAsync(w.deg, 0, (size_t)n * 4, s));
-  CU(cudaMemcpyAsync(m.counters, counters, sizeof counters, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(m.T, T, sizeof T, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(m.big, &w, sizeof w, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(slab + o_pair, &m, sizeof m, cudaMemcpyHostToDevice, s));
-  c->launches += launch_big_graph_solve((const MatchDev*)(slab + o_pair), 1, quatro_params_dev(prm, true), wide ? n : 0, s);
+  MatchDev m{};
+  const MatchDev* d_pair = nullptr;
+  const int* d_clique = nullptr;
+  if (wide == 2) {
+    // k_teaser_solve, the solver of optimizedMatching's sets, reads its pair as b200reg_quatro_align leaves it: fi = the
+    // source points, fj = the destination points, both in original order (identity rank), correspondence i = (i, i)
+    std::vector<float4> pts(2 * (size_t)n);
+    std::vector<int> ident(n), corr(2 * (size_t)n);
+    for (int i = 0; i < n; i++) {
+      float w;
+      memcpy(&w, &i, 4);  // the original index, as the index build stores it
+      pts[i] = make_float4(src_xyz[3 * i], src_xyz[3 * i + 1], src_xyz[3 * i + 2], w);
+      pts[n + i] = make_float4(dst_xyz[3 * i], dst_xyz[3 * i + 1], dst_xyz[3 * i + 2], w);
+      ident[i] = i;
+      corr[2 * i] = corr[2 * i + 1] = i;
+    }
+    Layout l;
+    const size_t o_pts = l.take(pts.size() * 16), o_rank = l.take((size_t)n * 4), o_oc = l.take(corr.size() * 4),
+                 o_cnt = l.take(8 * 4), o_T = l.take(16 * 8), o_clq = l.take((size_t)n * 4), o_pair = l.take(sizeof(MatchDev));
+    char* slab = nullptr;
+    CU(scratch.alloc((void**)&slab, l.size));
+    m.fi.n = m.fj.n = n;
+    m.fi.pts = (float4*)(slab + o_pts);
+    m.fj.pts = m.fi.pts + n;
+    m.fi.rank = m.fj.rank = (int*)(slab + o_rank);
+    m.swapped = 0;
+    m.out_corr = (int*)(slab + o_oc);
+    m.counters = (int*)(slab + o_cnt);
+    m.T = (double*)(slab + o_T);
+    m.clique = (int*)(slab + o_clq);
+    d_clique = m.clique;
+    d_pair = (const MatchDev*)(slab + o_pair);
+    CU(cudaMemcpyAsync(m.fi.pts, pts.data(), pts.size() * 16, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(m.fi.rank, ident.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(m.out_corr, corr.data(), corr.size() * 4, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(m.counters, counters, sizeof counters, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(slab + o_pair, &m, sizeof m, cudaMemcpyHostToDevice, s));
+    c->launches += launch_teaser_solve(d_pair, 1, quatro_params_dev(prm, false), s);
+  } else {
+    std::vector<double> S(3 * (size_t)n), D(3 * (size_t)n);
+    for (size_t k = 0; k < 3 * (size_t)n; k++) {
+      S[k] = src_xyz[k];  // k_big_gather's float -> double
+      D[k] = dst_xyz[k];
+    }
+    // the workspace b200reg_quatro_align gives a set of this size on each path
+    const int cap = wide ? (n + 1023) / 1024 * 1024 : std::max(1024, pow2_at_least(n));
+    Layout l;
+    const size_t o_big = l.take(sizeof(BigSolveWs)), o_cnt = l.take(8 * 4), o_T = l.take(16 * 8), o_pair = l.take(sizeof(MatchDev));
+    const BigWsLayout wl(l, cap, 0);
+    char* slab = nullptr;
+    CU(scratch.alloc((void**)&slab, l.size));
+    const BigSolveWs w = wl.bind(slab);
+    m.counters = (int*)(slab + o_cnt);
+    m.T = (double*)(slab + o_T);
+    m.big = (BigSolveWs*)(slab + o_big);
+    d_clique = w.clique;
+    d_pair = (const MatchDev*)(slab + o_pair);
+    double T[16];
+    for (int k = 0; k < 16; k++) T[k] = (k % 5 == 0) ? 1.0 : 0.0;
+    CU(cudaMemcpyAsync(w.S, S.data(), S.size() * 8, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(w.D, D.data(), D.size() * 8, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(w.deg, 0, (size_t)n * 4, s));
+    CU(cudaMemcpyAsync(m.counters, counters, sizeof counters, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(m.T, T, sizeof T, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(m.big, &w, sizeof w, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(slab + o_pair, &m, sizeof m, cudaMemcpyHostToDevice, s));
+    c->launches += launch_big_graph_solve(d_pair, 1, quatro_params_dev(prm, true), wide ? n : 0, s);
+  }
   CU(cudaGetLastError());
   int got[8];
   CU(cudaMemcpyAsync(got, m.counters, sizeof got, cudaMemcpyDeviceToHost, s));
   CU(cudaMemcpyAsync(info->T, m.T, 128, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
-  if (clique_out && got[4] > 0) CU(cudaMemcpyAsync(clique_out, w.clique, (size_t)got[4] * 4, cudaMemcpyDeviceToHost, s));
+  if (clique_out && got[4] > 0) CU(cudaMemcpyAsync(clique_out, d_clique, (size_t)got[4] * 4, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
   info->valid = got[3];
   info->n_mutual = n;

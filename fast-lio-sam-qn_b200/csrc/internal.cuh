@@ -214,6 +214,7 @@ struct MatchDev {
   int* out_corr;       // [2 * corr_cap] final (src, dst) pairs (corr_cap = MAXC, or BigSolveWs::cap for advancedMatching)
   double* T;           // [16] row-major result
   struct BigSolveWs* big;  // global-memory solver workspace (advancedMatching only; nullptr otherwise)
+  int* clique;         // [MAXC] or nullptr: k_teaser_solve lists the clique here, ascending (b200reg_quatro_solve_tap)
 };
 
 // Global-memory workspace of the multi-kernel TEASER++ solve used when the correspondence set is not capped at MAXC

@@ -694,7 +694,12 @@ __global__ void __launch_bounds__(1024) k_mutual(const MatchDev* pairs, float th
   if (threadIdx.x == 0) P.counters[1] = carry;
 }
 
-// Matcher::normalizePoints: per-cloud mean (fp64 fixed-shape tree sum, cast to fp32) and the larger max radius
+// Matcher::normalizePoints: per-cloud mean (fp64 fixed-shape tree sum, cast to fp32) and the larger max radius.
+// A deliberate deviation: the reference sums in fp32 in original point order (matcher.cc:70-76).  Kilometres from the
+// map origin the two means differ by centimetres, which rescales every normalised length by ~1e-4 through the max radius
+// but moves a length RATIO only by fp32 rounding (p - mean is exact there, Sterbenz).  The tuple test compares ratios
+// only; tests/test_tuple_reference.py measures that no trial of it flips (20 pairs shifted by (3000, -2000, 50) m: mean
+// gaps up to 19 mm, no verdict changed).
 __global__ void __launch_bounds__(1024) k_cloud_sum(const MatchDev* pairs) {
   const MatchDev& P = pairs[blockIdx.y];
   const int which = blockIdx.z;
@@ -760,7 +765,9 @@ __device__ __forceinline__ float len3(const float a[3], const float b[3]) {
 __global__ void __launch_bounds__(256) k_tuple_trials(const MatchDev* pairs, QuatroParamsDev prm) {
   const MatchDev& P = pairs[blockIdx.y];
   const int ncorr = P.counters[1];
-  if (ncorr == 0) return;
+  // tuple_scale == 0: no trial runs.  optimizedMatching then keeps nothing (its tuple block is the only writer of corres_,
+  // matcher.cc:461), so k_tuple_select finds no key; advancedMatching keeps every pair (k_adv_select's keepall).
+  if (ncorr == 0 || prm.tuple_scale == 0.f) return;
   const long long trials = (long long)ncorr * 100;
   const float mxi = (float)(P.stats[0] / P.fi.n), myi = (float)(P.stats[1] / P.fi.n), mzi = (float)(P.stats[2] / P.fi.n);
   const float mxj = (float)(P.stats[3] / P.fj.n), myj = (float)(P.stats[4] / P.fj.n), mzj = (float)(P.stats[5] / P.fj.n);
@@ -1092,6 +1099,8 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
       if ((Cm[v >> 5] >> (v & 31)) & 1u) sm.clique[m++] = v;
     sm.m = m;
     P.counters[4] = m;
+    if (P.clique)
+      for (int k = 0; k < m; k++) P.clique[k] = sm.clique[k];
   }
   __syncthreads();
   const int m = sm.m;
@@ -1863,6 +1872,11 @@ cudaError_t quatro_init_device() {
   return cudaFuncSetAttribute(k_adv_select, cudaFuncAttributeMaxDynamicSharedMemorySize, BIGC * 8);
 }
 
+int launch_teaser_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, cudaStream_t s) {
+  k_teaser_solve<<<count, SV_THREADS, solve_smem_bytes(), s>>>(d_pairs, prm);
+  return 1;
+}
+
 int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, int max_nj, const QuatroParamsDev& prm, cudaStream_t s) {
   int l = 0;
   k_match_init<<<dim3((max_ni + 255) / 256, count), 256, 0, s>>>(d_pairs); l++;
@@ -1875,8 +1889,7 @@ int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, in
   k_tuple_trials<<<dim3(128, count), 256, 0, s>>>(d_pairs, prm); l++;
   if (!prm.advanced) {
     k_tuple_select<<<count, 1024, 0, s>>>(d_pairs, prm); l++;
-    k_teaser_solve<<<count, SV_THREADS, sizeof(SolveSmem), s>>>(d_pairs, prm); l++;
-    return l;
+    return l + launch_teaser_solve(d_pairs, count, prm, s);
   }
   k_adv_select<<<count, 1024, BIGC * 8, s>>>(d_pairs, prm); l++;
   k_big_gather<<<dim3(BIGC / 256, count), 256, 0, s>>>(d_pairs); l++;

@@ -413,12 +413,15 @@ int b200reg_knn_bruteforce(b200reg_ctx* ctx, const b200reg_cloud* cloud, const f
 int b200reg_radius_search(b200reg_ctx* ctx, const b200reg_cloud* cloud, const float* queries, size_t nq,
                           size_t qstride_bytes, double sq_radius, int sorted, int64_t* offsets_out, size_t capacity,
                           int32_t* idx_out, float* d2_out);
-/* The TEASER++ QUATRO solve that follows advancedMatching, on n given correspondences: correspondence i joins
- * src_xyz[3i..3i+2] to dst_xyz[3i..3i+2] (host floats).  TIM graph, core-number order, greedy clique, GNC-TLS yaw and
- * TLS translation, exactly as b200reg_quatro_align runs them.  wide == 0 takes the path of sets up to
- * B200REG_ADV_CORR_CAPACITY (n must not exceed it); wide != 0 the path of larger sets, for any 1 <= n < 2^20.  Both
- * give the same answer.  info: T, valid, clique_size, gnc_iterations (n_mutual = n_corr = n).  clique_out (optional,
- * n ints): the clique's correspondence indices, ascending.                                                      */
+/* The TEASER++ QUATRO solve on n given correspondences: correspondence i joins src_xyz[3i..3i+2] to dst_xyz[3i..3i+2]
+ * (host floats).  TIM graph, core-number order, greedy clique, GNC-TLS yaw and TLS translation, exactly as
+ * b200reg_quatro_align runs them.  `wide` picks the solver:
+ *   0  the global-memory solver of advancedMatching sets up to B200REG_ADV_CORR_CAPACITY (n must not exceed it);
+ *   2  the shared-memory solver of optimizedMatching sets (the deployment's), n <= B200REG_CORR_CAPACITY;
+ *   any other value: the solver of advancedMatching sets beyond B200REG_ADV_CORR_CAPACITY, any 1 <= n < 2^20.
+ * All three give the same clique and iteration count, and T up to the order of their fp64 sums.  info: T, valid,
+ * clique_size, gnc_iterations (n_mutual = n_corr = n).  clique_out (optional, n ints): the clique's correspondence
+ * indices, ascending.                                                                                           */
 int b200reg_quatro_solve_tap(b200reg_ctx* ctx, int n, const float* src_xyz, const float* dst_xyz, int wide,
                              const b200reg_quatro_params* params, b200reg_quatro_info* info, int32_t* clique_out);
 /* normals (n x 3, NaN where fewer than 3 neighbours) and FPFH (n x 33), original point order.            */

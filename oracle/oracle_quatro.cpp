@@ -389,11 +389,9 @@ static std::vector<Corr> optimized_matching(const float* src, int N, int sstride
   // tuple test (matcher.cc:461-538) with the counter-based generator
   std::vector<Corr> out;
   const int ncorr = (int)corres.size();
-  if (ncorr == 0) return out;
-  if (tuple_scale == 0.f) {
-    for (auto& c : corres) out.push_back(swapped ? Corr{c.second, c.first} : Corr{c.first, c.second});
-    return out;
-  }
+  // tuple_scale == 0 skips the tuple block, the only writer of corres_ (matcher.cc:461-543): nothing is kept, and
+  // quatro::align returns invalid with the identity (quatro_module.cc:63-66)
+  if (ncorr == 0 || tuple_scale == 0.f) return out;
   std::vector<unsigned char> included(ncorr, 0);
   const long trials = (long)ncorr * 100;
   auto len = [&](int c, int a, int b) {
