@@ -6,7 +6,7 @@ from concurrent.futures import ThreadPoolExecutor
 PKG = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(PKG, "csrc")
 REPO = os.path.dirname(PKG)
-SOURCES = ["api.cu", "api_gicp.cu", "api_quatro.cu", "api_keyframes.cu", "index_build.cu", "gicp.cu", "quatro.cu", "assemble.cu", "batch.cu", "radius.cu", "knn_large.cu"]
+SOURCES = ["api.cu", "api_gicp.cu", "api_quatro.cu", "api_keyframes.cu", "api_loop_clouds.cu", "index_build.cu", "gicp.cu", "quatro.cu", "assemble.cu", "batch.cu", "radius.cu", "knn_large.cu"]
 EXTRA = {"quatro.cu": ["-fmad=false"],    # fixed fp32 operation order for the FPFH / matcher arithmetic
          "assemble.cu": ["-fmad=false"]}  # transformPcd / VoxelGrid / candidate distances as the (FMA-free) reference computes them
 HEADERS = ["api.cuh", "launchers.cuh", "internal.cuh", "knn.cuh", "smallmath.cuh", "fpfh_basis.cuh", os.path.join(REPO, "include", "b200reg.h")]

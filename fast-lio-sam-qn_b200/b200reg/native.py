@@ -96,9 +96,11 @@ EXPORTS = [
     "b200reg_batch_wait", "b200reg_batch_wait_all", "b200reg_batch_launch_count", "b200reg_batch_depth",
     "b200reg_comm_unique_id", "b200reg_comm_init", "b200reg_comm_destroy", "b200reg_comm_rank", "b200reg_comm_world",
     "b200reg_allgather_results", "b200reg_radius_search", "b200reg_quatro_align_ex", "b200reg_quatro_solve_tap",
-    "b200reg_ctx_set_lm_trace", "b200reg_lm_trace",
+    "b200reg_ctx_set_lm_trace", "b200reg_lm_trace", "b200reg_ctx_set_loop_clouds", "b200reg_loop_clouds",
 ]
 ESTATE = -4  # B200REG_ESTATE
+# B200REG_CLOUD_*: the loop clouds (Context.set_loop_clouds / Context.loop_clouds)
+CLOUD_SOURCE, CLOUD_TARGET, CLOUD_COARSE, CLOUD_FINAL = 1, 2, 4, 8
 
 
 def _point_at_bundled_nccl():
@@ -250,6 +252,25 @@ class Context:
         _check(lib().b200reg_lm_trace(self.h, offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(trials)),
                                       trials.ctypes.data_as(C.c_void_p)))
         return [trials[offsets[i]:offsets[i + 1]] for i in range(n)]
+
+    def set_loop_clouds(self, mask):
+        """Capture the clouds loopTimerFunc publishes (an OR of CLOUD_SOURCE, CLOUD_TARGET, CLOUD_COARSE, CLOUD_FINAL; 0 turns
+        capture off) in the following icp_alignment / loop_closure / perform_loop_closure calls; results do not change."""
+        _check(lib().b200reg_ctx_set_loop_clouds(self.h, int(mask)))
+
+    def loop_clouds(self, kind):
+        """The clouds of one kind from the last capturing call: one (n, 4) float32 array (x, y, z, intensity) per pair of
+        that call, in its pair order; empty where the reference has no such cloud (include/b200reg.h)."""
+        n = lib().b200reg_loop_clouds(self.h, int(kind), None, C.c_size_t(0), None)
+        _check(min(n, 0))
+        offsets = np.empty(n + 1, np.int64)
+        rc = lib().b200reg_loop_clouds(self.h, int(kind), offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None)  # offsets only
+        if rc != ESTATE:
+            _check(rc)
+        pts = np.empty((int(offsets[-1]), 4), np.float32)
+        _check(lib().b200reg_loop_clouds(self.h, int(kind), offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(pts)),
+                                         pts.ctypes.data_as(C.c_void_p)))
+        return [pts[offsets[i]:offsets[i + 1]] for i in range(n)]
 
     # -- the path's one collective: all-gather of the result records over NCCL (SURVEY §8e) --------
     def comm_init(self, unique_id, rank, world):

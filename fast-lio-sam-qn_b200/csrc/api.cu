@@ -56,14 +56,14 @@ b200reg_result default_result() {
 }
 
 int create_pair_clouds(b200reg_ctx* c, int count, const float* const* src_xyz, const size_t* src_n, const float* const* tgt_xyz,
-                       const size_t* tgt_n, size_t stride_bytes, int on_device, CloudBag& bag, b200reg_cloud** src_out,
-                       b200reg_cloud** tgt_out) {
+                       const size_t* tgt_n, size_t stride_bytes, int on_device, bool keep_intensity, CloudBag& bag,
+                       b200reg_cloud** src_out, b200reg_cloud** tgt_out) {
   std::vector<const float*> ptrs(src_xyz, src_xyz + count);
   ptrs.insert(ptrs.end(), tgt_xyz, tgt_xyz + count);
   std::vector<size_t> ns(src_n, src_n + count);
   ns.insert(ns.end(), tgt_n, tgt_n + count);
   std::vector<b200reg_cloud*> cl(2 * count, nullptr);
-  const int rc = b200reg_clouds_create(c, 2 * count, ptrs.data(), ns.data(), stride_bytes, on_device, cl.data());
+  const int rc = clouds_create(c, 2 * count, ptrs.data(), ns.data(), stride_bytes, on_device, keep_intensity, cl.data());
   if (rc) return rc;
   bag.cl.insert(bag.cl.end(), cl.begin(), cl.end());
   std::copy(cl.begin(), cl.begin() + count, src_out);
@@ -209,6 +209,13 @@ size_t b200reg_cloud_size(const b200reg_cloud* cl) { return cl ? (size_t)cl->dev
 // ------------------------------------------------------------------------------------------
 int b200reg_clouds_create(b200reg_ctx* c, int count, const float* const* xyz, const size_t* n, size_t stride_bytes,
                           int on_device, b200reg_cloud** out) {
+  return clouds_create(c, count, xyz, n, stride_bytes, on_device, false, out);
+}
+
+}  // extern "C"
+
+int b200::clouds_create(b200reg_ctx* c, int count, const float* const* xyz, const size_t* n, size_t stride_bytes, int on_device,
+                        bool keep_intensity, b200reg_cloud** out) {
   if (!c || count <= 0 || !xyz || !n || !out) return fail(B200REG_EINVAL, "bad argument");
   if (stride_bytes < 12 || stride_bytes % 4) return fail(B200REG_EINVAL, "stride_bytes must be a multiple of 4, >= 12");
   for (int i = 0; i < count; i++)
@@ -242,9 +249,11 @@ int b200reg_clouds_create(b200reg_ctx* c, int count, const float* const* xyz, co
     Layout pl;
     const size_t o_pts = pl.take((size_t)d.n * sizeof(float4)), o_tn = pl.take(4 * nn * sizeof(float4)),
                  o_cov = pl.take((size_t)6 * d.n * sizeof(double)), o_rank = pl.take((size_t)d.n * sizeof(int));
+    const size_t o_int = keep_intensity ? pl.take((size_t)d.n * sizeof(float)) : 0;
     char* slab = nullptr;
     CU(cudaMallocFromPoolAsync((void**)&slab, pl.size, c->pool, s));
     cl->slab = slab;
+    if (keep_intensity) cl->inten = (float*)(slab + o_int);
     d.pts = (float4*)(slab + o_pts);
     d.tnodes = (float4*)(slab + o_tn);
     d.cov = (double*)(slab + o_cov);
@@ -292,6 +301,15 @@ int b200reg_clouds_create(b200reg_ctx* c, int count, const float* const* xyz, co
     for (int i = 0; i < count; i++) c->prof_bytes[CLS_BUILD] += 36.0 * descs[i].n;  // SURVEY §8(d) K1
   }
   CU(cudaGetLastError());
+  if (keep_intensity) {  // from the raw records, while they are still there
+    std::vector<float*> inten(count);
+    for (int i = 0; i < count; i++) inten[i] = bag.cl[i]->inten;
+    float** d_inten = nullptr;
+    CU(scratch.upload(&d_inten, inten.data(), sizeof(float*) * count));
+    launch_gather_intensity(d_descs, count, max_n, d_inten, s);
+    c->launches++;
+    CU(cudaGetLastError());
+  }
   for (b200reg_cloud* cl : bag.cl) {  // the temporaries are gone once the build has run
     CloudDev& d = cl->dev;
     d.raw = nullptr;
@@ -305,6 +323,8 @@ int b200reg_clouds_create(b200reg_ctx* c, int count, const float* const* xyz, co
   bag.cl.clear();
   return B200REG_OK;
 }
+
+extern "C" {
 
 int b200reg_cloud_destroy(b200reg_ctx* c, b200reg_cloud* cl) {
   if (!cl) return B200REG_OK;

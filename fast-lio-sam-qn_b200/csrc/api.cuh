@@ -59,6 +59,14 @@ struct b200reg_ctx {
     std::vector<int64_t> offsets;  // pairs + 1
     std::vector<b200reg_lm_trial> trials;
   } lm_trace;
+  // loop clouds (b200reg_ctx_set_loop_clouds / b200reg_loop_clouds): the kinds the capturing calls record, and the clouds of
+  // the most recent such call, CSR over its pairs per kind (slot = log2 of the kind's bit), on the host
+  struct LoopClouds {
+    int mask = 0;
+    int stored = 0;  // kinds held; 0 before a capturing call and after an uncaptured one
+    std::vector<int64_t> offsets[4];  // pairs + 1 each
+    std::vector<float4> pts[4];       // (x, y, z, intensity)
+  } loop_clouds;
   // the path's one collective (b200reg_comm_*): NCCL communicator of this rank
   ncclComm_t comm = nullptr;
   int rank = -1, world = 1;
@@ -83,6 +91,7 @@ struct b200reg_cloud {
   int cov_method = 3;
   bool has_fpfh = false;
   double normal_r = 0, fpfh_r = 0;
+  float* inten = nullptr;  // [n] intensities, original order, in `slab`: only clouds created inside a capturing call keep them
 };
 
 namespace b200 {
@@ -157,11 +166,15 @@ struct Layout {
 // RegistrationOutput's defaults (loop_closure.h:64-70): identity transforms, score_ = DBL_MAX, not valid
 b200reg_result default_result();
 
+// b200reg_clouds_create; keep_intensity: each cloud also keeps the intensities of its records (b200reg_cloud::inten)
+int clouds_create(b200reg_ctx* c, int count, const float* const* xyz, const size_t* n, size_t stride_bytes, int on_device,
+                  bool keep_intensity, b200reg_cloud** out);
+
 // The clouds of `count` pairs, built in one batch: the source clouds come first, then the targets.  They go to src_out /
 // tgt_out and are owned by `bag`.
 int create_pair_clouds(b200reg_ctx* c, int count, const float* const* src_xyz, const size_t* src_n, const float* const* tgt_xyz,
-                       const size_t* tgt_n, size_t stride_bytes, int on_device, CloudBag& bag, b200reg_cloud** src_out,
-                       b200reg_cloud** tgt_out);
+                       const size_t* tgt_n, size_t stride_bytes, int on_device, bool keep_intensity, CloudBag& bag,
+                       b200reg_cloud** src_out, b200reg_cloud** tgt_out);
 
 // orig[p] = the original index of the point at sorted position p (the int bits of pts[p].w).  Synchronises the stream, so
 // the downloads the caller queued before have landed too.  pts_out, if given, receives the sorted points.
@@ -174,9 +187,37 @@ void lm_arena_free(b200reg_ctx* c);  // api_gicp.cu
 // others get no records.  Does nothing but keep the trace invalid when tracing is off.  (api_gicp.cu)
 void lm_trace_remap(b200reg_ctx* c, int count, const std::vector<int>& where);
 
-// LoopClosure::coarseToFineAlignment on cloud handles (api_quatro.cu)
+// LoopClosure::coarseToFineAlignment on cloud handles (api_quatro.cu).  fine_tf16 (optional, count x 16): the fine stage's
+// own fp32 final transformation of each pair whose coarse stage is valid (the transform of align()'s output cloud)
 int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst,
                              const b200reg_quatro_params* qp, const b200reg_gicp_params* gp, b200reg_result* out,
-                             b200reg_quatro_info* quatro_out);
+                             b200reg_quatro_info* quatro_out, float* fine_tf16);
+
+// The loop clouds of one call of b200reg_icp_alignment, b200reg_loop_closure or b200reg_perform_loop_closure, over the
+// CALLER's pairs (api_loop_clouds.cu).  The constructor discards the stored clouds.  The call then hands over what its
+// stages ran on, numbered as the stages saw their pairs: stage pair k is the caller's pair where[k], and this is the one
+// place that renumbers them (an empty `where`: stage pair k is the caller's pair k).
+//   clouds()  the source and target clouds, as soon as they exist: sizes the device slab for every row that can be present,
+//             so that a failed allocation costs no registration;
+//   finish()  the coarse stage's infos (nullptr: the call has no Quatro stage; the fine stage ran where they are valid) and
+//             the fine stage's fp32 transforms (16 per stage pair): writes every row in one launch and stores the result.
+// With capture off every step returns at once: no allocation, no launch.
+class LoopCapture {
+ public:
+  LoopCapture(b200reg_ctx* c, int count);
+  bool on() const { return mask_ != 0; }
+  int clouds(const std::vector<int>& where, b200reg_cloud* const* src, b200reg_cloud* const* dst, bool src_tgt_rows,
+             bool coarse_rows);
+  int finish(const b200reg_quatro_info* qi, const float* fine_tf16);
+
+ private:
+  b200reg_ctx* c_;
+  int count_, mask_;
+  Scratch scratch_;
+  std::vector<int> where_;
+  std::vector<const b200reg_cloud*> src_, dst_;  // per stage pair
+  bool src_tgt_rows_ = false;
+  float4* slab_[4] = {nullptr, nullptr, nullptr, nullptr};
+};
 
 }  // namespace b200

@@ -327,15 +327,26 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
   return B200REG_OK;
 }
 
+// the solve of icpAlignment over built clouds, with its loop clouds: FINAL is align()'s output cloud of every pair
+static int icp_solve(b200reg_ctx* c, LoopCapture& cap, int count, b200reg_cloud* const* sc, b200reg_cloud* const* tc,
+                     const b200reg_gicp_params* params, b200reg_result* out) {
+  int rc = cap.clouds({}, sc, tc, false, false);
+  if (!rc) rc = b200reg_gicp_align(c, count, sc, tc, nullptr, params, out);
+  if (rc || !cap.on()) return rc;
+  std::vector<float> fine_tf(16 * (size_t)count);
+  for (int i = 0; i < count; i++) memcpy(&fine_tf[16 * (size_t)i], out[i].Tf, sizeof(out[i].Tf));
+  return cap.finish(nullptr, fine_tf.data());
+}
+
 // one chunk of pairs, raw records already on the device
-static int icp_alignment_device(b200reg_ctx* c, int count, const float* const* src_xyz, const size_t* src_n,
+static int icp_alignment_device(b200reg_ctx* c, LoopCapture& cap, int count, const float* const* src_xyz, const size_t* src_n,
                                 const float* const* tgt_xyz, const size_t* tgt_n, size_t stride_bytes,
                                 const b200reg_gicp_params* params, b200reg_result* out) {
   CloudBag bag(c);
   std::vector<b200reg_cloud*> sc(count), tc(count);
-  int rc = create_pair_clouds(c, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, 1, bag, sc.data(), tc.data());
+  int rc = create_pair_clouds(c, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, 1, cap.on(), bag, sc.data(), tc.data());
   if (!rc) rc = b200reg_clouds_covariances_ex(c, 2 * count, bag.cl.data(), params->k_correspondences, params->regularization);
-  if (!rc) rc = b200reg_gicp_align(c, count, sc.data(), tc.data(), nullptr, params, out);
+  if (!rc) rc = icp_solve(c, cap, count, sc.data(), tc.data(), params, out);
   return rc;
 }
 
@@ -348,7 +359,8 @@ int b200reg_icp_alignment(b200reg_ctx* c, int count, const float* const* src_xyz
   for (int i = 0; i < count; i++)
     if (!src_xyz[i] || !tgt_xyz[i] || src_n[i] == 0 || tgt_n[i] == 0) return fail(B200REG_EINVAL, "empty cloud");
   CU(cudaSetDevice(c->device));
-  if (on_device) return icp_alignment_device(c, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, params, out);
+  LoopCapture cap(c, count);
+  if (on_device) return icp_alignment_device(c, cap, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, params, out);
   // Host buffers: all uploads are queued on the copy stream up front, chunk by chunk; the compute stream processes
   // chunk k as soon as its records have landed, so the PCIe time of chunk k+1 hides behind the kernels of chunk k.
   cudaStream_t s = c->stream;
@@ -402,11 +414,11 @@ int b200reg_icp_alignment(b200reg_ctx* c, int count, const float* const* src_xyz
   for (int k0 = 0; k0 < count && !rc; k0 += per, chunk++) {
     const int m = std::min(count, k0 + per) - k0;
     CU(cudaStreamWaitEvent(s, landed[chunk], 0));
-    rc = create_pair_clouds(c, m, &sp[k0], &src_n[k0], &tp[k0], &tgt_n[k0], stride_bytes, 1, bag, &sc[k0], &tc[k0]);
+    rc = create_pair_clouds(c, m, &sp[k0], &src_n[k0], &tp[k0], &tgt_n[k0], stride_bytes, 1, cap.on(), bag, &sc[k0], &tc[k0]);
     // the chunk's clouds are the last 2 m in the bag
     if (!rc) rc = b200reg_clouds_covariances_ex(c, 2 * m, &bag.cl[bag.cl.size() - 2 * m], params->k_correspondences, params->regularization);
   }
-  if (!rc) rc = b200reg_gicp_align(c, count, sc.data(), tc.data(), nullptr, params, out);
+  if (!rc) rc = icp_solve(c, cap, count, sc.data(), tc.data(), params, out);
   return rc;  // clouds, events and the copy stream are released / drained by the scope guards
 }
 

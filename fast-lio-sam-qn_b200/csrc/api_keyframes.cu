@@ -37,6 +37,10 @@ static int kf_alloc(b200reg_keyframes* kf, size_t n, size_t min_slab, float4** o
   return B200REG_OK;
 }
 
+static int assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
+                           const b200reg_loop_config* cfg, const int32_t* n_keyframes, bool keep_intensity, b200reg_cloud** src_out,
+                           b200reg_cloud** dst_out);
+
 extern "C" {
 
 void b200reg_default_loop_config(b200reg_loop_config* cfg) {
@@ -308,6 +312,15 @@ int b200reg_assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, co
 int b200reg_assemble_clouds_at(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
                                const b200reg_loop_config* cfg, const int32_t* n_keyframes, b200reg_cloud** src_out,
                                b200reg_cloud** dst_out) {
+  return assemble_clouds(c, kf, count, src_idx, dst_idx, cfg, n_keyframes, false, src_out, dst_out);
+}
+
+}  // extern "C"
+
+// b200reg_assemble_clouds_at; keep_intensity: the clouds keep the voxel-mean intensities (b200reg_cloud::inten)
+static int assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
+                           const b200reg_loop_config* cfg, const int32_t* n_keyframes, bool keep_intensity, b200reg_cloud** src_out,
+                           b200reg_cloud** dst_out) {
   if (!c || !kf || count <= 0 || !src_idx || !dst_idx || !cfg || !n_keyframes || !src_out || !dst_out)
     return fail(B200REG_EINVAL, "bad argument");
   for (int i = 0; i < count; i++)
@@ -404,7 +417,7 @@ int b200reg_assemble_clouds_at(b200reg_ctx* c, b200reg_keyframes* kf, int count,
     ns[j] = overflow ? (size_t)jobs[j].total : (size_t)counters[4 * j];
   }
   std::vector<b200reg_cloud*> clouds(njobs, nullptr);
-  int rc = b200reg_clouds_create(c, njobs, ptrs.data(), ns.data(), 16, 1, clouds.data());
+  int rc = clouds_create(c, njobs, ptrs.data(), ns.data(), 16, 1, keep_intensity, clouds.data());
   for (int i = 0; i < count && !rc; i++) {
     src_out[i] = clouds[i];
     dst_out[i] = clouds[count + i];
@@ -412,9 +425,12 @@ int b200reg_assemble_clouds_at(b200reg_ctx* c, b200reg_keyframes* kf, int count,
   return rc;
 }
 
+extern "C" {
+
 int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
                                  const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out) {
   if (!c || !kf || count <= 0 || !query_idx || !closest_idx || !cfg || !out) return fail(B200REG_EINVAL, "bad argument");
+  LoopCapture cap(c, count);
   std::vector<int32_t> qs, cs;
   std::vector<int> where;
   for (int i = 0; i < count; i++) {
@@ -428,7 +444,7 @@ int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int coun
   }
   if (qs.empty()) {
     lm_trace_remap(c, count, where);
-    return B200REG_OK;
+    return cap.finish(nullptr, nullptr);
   }
   const int m = (int)qs.size();
   // at the time query q was the latest keyframe the vector held q + 1 keyframes (fast_lio_sam_qn.cpp:205-219); a batch
@@ -436,20 +452,27 @@ int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int coun
   std::vector<int32_t> nks(m);
   for (int k = 0; k < m; k++) nks[k] = qs[k] + 1;
   std::vector<b200reg_cloud*> sc(m, nullptr), dc(m, nullptr);
-  int rc = b200reg_assemble_clouds_at(c, kf, m, qs.data(), cs.data(), cfg, nks.data(), sc.data(), dc.data());
+  int rc = assemble_clouds(c, kf, m, qs.data(), cs.data(), cfg, nks.data(), cap.on(), sc.data(), dc.data());
   if (rc) return rc;
   CloudBag bag(c);
   bag.cl = sc;
   bag.cl.insert(bag.cl.end(), dc.begin(), dc.end());
+  if ((rc = cap.clouds(where, sc.data(), dc.data(), true, cfg->enable_quatro != 0))) return rc;
   std::vector<b200reg_result> res(m);
   std::vector<b200reg_quatro_info> qi(m);
-  if (cfg->enable_quatro) rc = coarse_to_fine_on_clouds(c, m, sc.data(), dc.data(), &cfg->quatro, &cfg->gicp, res.data(), qi.data());
-  else rc = b200reg_gicp_align(c, m, sc.data(), dc.data(), nullptr, &cfg->gicp, res.data());
+  std::vector<float> fine_tf(16 * (size_t)m);  // the fine stage's transform of align()'s output cloud
+  if (cfg->enable_quatro) {
+    rc = coarse_to_fine_on_clouds(c, m, sc.data(), dc.data(), &cfg->quatro, &cfg->gicp, res.data(), qi.data(), fine_tf.data());
+  } else {
+    rc = b200reg_gicp_align(c, m, sc.data(), dc.data(), nullptr, &cfg->gicp, res.data());
+    for (int k = 0; k < m && !rc; k++) memcpy(&fine_tf[16 * (size_t)k], res[k].Tf, sizeof(res[k].Tf));
+  }
   for (int k = 0; k < m && !rc; k++) {
     out[where[k]] = res[k];
     if (quatro_out && cfg->enable_quatro) quatro_out[where[k]] = qi[k];
   }
   if (!rc) lm_trace_remap(c, count, where);
+  if (!rc) rc = cap.finish(cfg->enable_quatro ? qi.data() : nullptr, fine_tf.data());
   return rc;
 }
 

@@ -9,7 +9,7 @@
 namespace b200 {
 int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst,
                              const b200reg_quatro_params* qp, const b200reg_gicp_params* gp, b200reg_result* out,
-                             b200reg_quatro_info* quatro_out) {
+                             b200reg_quatro_info* quatro_out, float* fine_tf16) {
   cudaStream_t s = c->stream;
   Scratch scratch(c);
   std::vector<b200reg_quatro_info> qi(count);
@@ -65,6 +65,7 @@ int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* sr
     if (rc) return rc;
     for (int k = 0; k < nv; k++) {
       const int i = vidx[k];
+      if (fine_tf16) memcpy(&fine_tf16[16 * (size_t)i], gres[k].Tf, sizeof(gres[k].Tf));
       b200reg_result r = gres[k];
       // reg_output.pose_between_eig_ = fine (float -> double) * quatro_tf_  (loop_closure.cpp:156)
       double F[16], Q[16];
@@ -548,10 +549,16 @@ int b200reg_loop_closure(b200reg_ctx* c, int count, const float* const* src_xyz,
                          const b200reg_gicp_params* gp, b200reg_result* out, b200reg_quatro_info* quatro_out) {
   if (!c || count <= 0 || !src_xyz || !src_n || !tgt_xyz || !tgt_n || !qp || !gp || !out) return fail(B200REG_EINVAL, "bad argument");
   CU(cudaSetDevice(c->device));
+  LoopCapture cap(c, count);
   CloudBag bag(c);
   std::vector<b200reg_cloud*> sc(count), tc(count);
-  int rc = create_pair_clouds(c, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, on_device, bag, sc.data(), tc.data());
-  if (!rc) rc = coarse_to_fine_on_clouds(c, count, sc.data(), tc.data(), qp, gp, out, quatro_out);
+  int rc = create_pair_clouds(c, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, on_device, cap.on(), bag, sc.data(), tc.data());
+  if (!rc) rc = cap.clouds({}, sc.data(), tc.data(), false, true);
+  std::vector<b200reg_quatro_info> own(quatro_out ? 0 : count);  // the capture reads the coarse stage's infos
+  b200reg_quatro_info* qi = quatro_out ? quatro_out : own.data();
+  std::vector<float> fine_tf(cap.on() ? 16 * (size_t)count : 0);
+  if (!rc) rc = coarse_to_fine_on_clouds(c, count, sc.data(), tc.data(), qp, gp, out, qi, cap.on() ? fine_tf.data() : nullptr);
+  if (!rc) rc = cap.finish(qi, fine_tf.data());
   return rc;
 }
 

@@ -192,6 +192,40 @@ __global__ void __launch_bounds__(256) k_pack_xyzi(const float* raw, int stride,
   const float* p = raw + (size_t)i * stride;
   out[i] = make_float4(p[0], p[1], p[2], stride >= 8 ? p[4] : p[3]);
 }
+// Intensities of the raw records a cloud was built from, ORIGINAL order (clouds created inside a call that captures its loop
+// clouds): k_pack_xyzi's rule -- float 3 for 4..7-float records, float 4 from pcl::PointXYZI's 8 on -- and 0 for bare xyz
+__global__ void __launch_bounds__(256) k_gather_intensity(const CloudDev* clouds, float* const* inten) {
+  const CloudDev& c = clouds[blockIdx.y];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c.n) return;
+  const float* p = c.raw + (size_t)i * c.raw_stride;
+  inten[blockIdx.y][i] = c.raw_stride >= 8 ? p[4] : c.raw_stride >= 4 ? p[3] : 0.f;
+}
+
+// Every row of one call's loop clouds (b200reg_loop_clouds) in one launch; the transforms are k_transform_raw's and
+// k_transform_out's own (internal.cuh), so COARSE and FINAL are their bytes
+__global__ void __launch_bounds__(256) k_capture_rows(const CaptureRow* rows, int nrows) {
+  for (int r = blockIdx.y; r < nrows; r += gridDim.y) {
+    const CaptureRow& R = rows[r];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < R.n; i += gridDim.x * blockDim.x) {
+      const float4 p = R.pts[i];
+      const int o = __float_as_int(p.w);
+      float3 q = make_float3(p.x, p.y, p.z);
+      if (R.coarse) q = transform_pcd_point(R.Tq, q.x, q.y, q.z);
+      if (R.fine) q = transform_out_point(R.Tf, q.x, q.y, q.z);
+      R.out[o] = make_float4(q.x, q.y, q.z, R.inten[o]);
+    }
+  }
+}
+
+void launch_gather_intensity(const CloudDev* d_clouds, int count, int max_n, float* const* d_inten, cudaStream_t s) {
+  k_gather_intensity<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_clouds, d_inten);
+}
+
+void launch_capture_rows(const CaptureRow* d_rows, int nrows, int max_n, cudaStream_t s) {
+  k_capture_rows<<<dim3((max_n + 255) / 256, min(nrows, 65535)), 256, 0, s>>>(d_rows, nrows);
+}
+
 void launch_pack_xyzi(const float* d_raw, int stride, int n, float4* d_out, cudaStream_t s) {
   k_pack_xyzi<<<(n + 255) / 256, 256, 0, s>>>(d_raw, stride, n, d_out);
 }

@@ -729,10 +729,11 @@ __global__ void __launch_bounds__(256) k_transform_out(CloudDev c, const float* 
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= c.n) return;
   const float4 p = c.pts[i];
-  const int o = __float_as_int(p.w);
-#pragma unroll
-  for (int r = 0; r < 3; r++)
-    out3[(size_t)o * 3 + r] = __fadd_rn(__fmul_rn(Tf[4 * r], p.x), __fadd_rn(__fmul_rn(Tf[4 * r + 1], p.y), __fadd_rn(__fmul_rn(Tf[4 * r + 2], p.z), Tf[4 * r + 3])));
+  const size_t o = (size_t)__float_as_int(p.w) * 3;
+  const float3 q = transform_out_point(Tf, p.x, p.y, p.z);
+  out3[o] = q.x;
+  out3[o + 1] = q.y;
+  out3[o + 2] = q.z;
 }
 
 // ---------------------------------------------------------------------------------------

@@ -198,6 +198,35 @@ struct AssembleJob {  // one output cloud of setSrcAndDstCloud
   SortBufs sort;
 };
 
+// ---- the transforms behind the output clouds, one definition each -----------------------------------------------------
+// transformPcd (utilities.hpp:164-175): Matrix4d (row-major here), double math, cast to float.  The reference's FMA-free
+// order holds in the files compiled with -fmad=false (quatro.cu: k_transform_raw; assemble.cu: the loop-cloud capture).
+__device__ __forceinline__ float3 transform_pcd_point(const double* T, float px, float py, float pz) {
+  const double x = px, y = py, z = pz;
+  return make_float3((float)(T[0] * x + T[1] * y + T[2] * z + T[3]), (float)(T[4] * x + T[5] * y + T[6] * z + T[7]),
+                     (float)(T[8] * x + T[9] * y + T[10] * z + T[11]));
+}
+// pcl::transformPointCloud with align()'s fp32 final transformation (lsq_registration_impl.hpp:114), explicit rounding
+__device__ __forceinline__ float3 transform_out_point(const float* Tf, float x, float y, float z) {
+  float o[3];
+#pragma unroll
+  for (int r = 0; r < 3; r++)
+    o[r] = __fadd_rn(__fmul_rn(Tf[4 * r], x), __fadd_rn(__fmul_rn(Tf[4 * r + 1], y), __fadd_rn(__fmul_rn(Tf[4 * r + 2], z), Tf[4 * r + 3])));
+  return make_float3(o[0], o[1], o[2]);
+}
+
+// One row of the loop-cloud capture (b200reg_loop_clouds): a cloud in ORIGINAL point order as (x, y, z, intensity), taken
+// through transformPcd(Tq) when `coarse` is set and then through the fine stage's fp32 Tf when `fine` is set.
+struct CaptureRow {
+  const float4* pts;   // the cloud's sorted points, w = original index
+  const float* inten;  // [n] intensities, original order
+  float4* out;         // [n] this row in the call's slab
+  int n;
+  int coarse, fine;
+  double Tq[12];       // row-major 3 x 4
+  float Tf[12];
+};
+
 // ---- Quatro matcher / solver workspace ---------------------------------------------------
 // per-pair device workspace of the matcher / solver
 struct MatchDev {

@@ -81,5 +81,9 @@ int launch_fetch_closest(const double* d_pos, const double* d_stamp, const int* 
                          int* d_out, cudaStream_t s);
 int launch_assemble_voxelize(const AssembleJob* d_jobs, const CloudDev* d_sort, int count, int max_total, const KeyframeDev* d_kfs,
                              const double* d_poses, float inv_leaf, cudaStream_t s);
+// loop-cloud capture: intensities of freshly uploaded clouds (raw records still valid) into d_inten[i][n_i]; then every
+// CaptureRow of a call (max_n = the longest row)
+void launch_gather_intensity(const CloudDev* d_clouds, int count, int max_n, float* const* d_inten, cudaStream_t s);
+void launch_capture_rows(const CaptureRow* d_rows, int nrows, int max_n, cudaStream_t s);
 
 }  // namespace b200

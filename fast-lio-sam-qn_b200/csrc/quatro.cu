@@ -1833,14 +1833,8 @@ __global__ void __launch_bounds__(256) k_transform_raw(const CloudDev* clouds, c
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= src.n) return;
   const float4 p = src.pts[i];
-  const double* T = T16s + 16 * blockIdx.y;
-  const double x = p.x, y = p.y, z = p.z;
-  float4 o;
-  o.x = (float)(T[0] * x + T[1] * y + T[2] * z + T[3]);
-  o.y = (float)(T[4] * x + T[5] * y + T[6] * z + T[7]);
-  o.z = (float)(T[8] * x + T[9] * y + T[10] * z + T[11]);
-  o.w = 1.f;
-  outs[blockIdx.y][__float_as_int(p.w)] = o;
+  const float3 q = transform_pcd_point(T16s + 16 * blockIdx.y, p.x, p.y, p.z);
+  outs[blockIdx.y][__float_as_int(p.w)] = make_float4(q.x, q.y, q.z, 1.f);
 }
 
 // ------------------------------------------------------------------------------------------------

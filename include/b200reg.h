@@ -175,6 +175,40 @@ int b200reg_ctx_set_lm_trace(b200reg_ctx* ctx, int enable);
  * B200REG_ESTATE.                                                                                                       */
 int b200reg_lm_trace(b200reg_ctx* ctx, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out);
 
+/* Loop clouds: the four clouds loopTimerFunc publishes after each loop attempt (fast_lio_sam_qn.cpp:245-248), as the batched
+ * calls b200reg_icp_alignment, b200reg_loop_closure and b200reg_perform_loop_closure produce them.  Every point is four
+ * floats (x, y, z, intensity), pcl::PointXYZI without its padding; intensity is carried through every step.
+ *   SOURCE  LoopClosure::getSourceCloud (loop_closure.cpp:185): the assembled, voxelised source -- b200reg_cloud_points of it,
+ *           in voxel-index order, intensity the voxel mean (fp32 running sums in ascending point order; the unfiltered
+ *           merged cloud when the voxel grid's int32 guard trips, as PCL returns it).  b200reg_perform_loop_closure only.
+ *   TARGET  getTargetCloud (:186): the same for the target.  b200reg_perform_loop_closure only.
+ *   COARSE  getCoarseAlignedCloud (:152): transformPcd(source, quatro_out[i].T) -- double math cast to float, the source's
+ *           order -- for pairs whose Quatro stage is valid; empty otherwise, as the reference clears it (:142).
+ *   FINAL   getFinalAlignedCloud (:124; lsq_registration_impl.hpp:114): NanoGICP::align's output cloud, the fine source
+ *           (COARSE in Quatro mode, else the source) through the fine stage's fp32 transform, byte-equal to
+ *           b200reg_transform_cloud; present whenever the fine stage ran, converged or not.  Where it did not run the row is
+ *           empty (the reference would keep the previous tick's cloud; a batch has no previous tick).
+ * The raw-buffer calls take the intensity from their records as b200reg_keyframes_add does: float 3 for strides of 16 to
+ * 31 bytes, float 4 from 32 bytes (pcl::PointXYZI), 0 for 12-byte records.                                             */
+#define B200REG_CLOUD_SOURCE 1
+#define B200REG_CLOUD_TARGET 2
+#define B200REG_CLOUD_COARSE 4
+#define B200REG_CLOUD_FINAL 8
+/* Capture the kinds in `mask` (an OR of B200REG_CLOUD_*; 0, the default, turns capture off) in the following calls of the
+ * three entry points above; no other entry point touches the stored clouds.  A call with capture on replaces the stored
+ * clouds, one with capture off discards them.  Capture changes no result, trace or solve.  Its device slab (16 bytes per
+ * point per kind: 512 pairs x 100k points x 4 kinds is about 3.3 GB) lives for the call only and is sized before Quatro
+ * for every row that can be present; if it cannot be allocated the call returns B200REG_ECUDA with the bytes in the
+ * message.  With capture off nothing is allocated or launched.                                                         */
+int b200reg_ctx_set_loop_clouds(b200reg_ctx* ctx, int mask);
+/* The clouds of one kind from the context's most recent capturing call, as CSR over that call's pairs (the CALLER's pair
+ * order): pair i's points are xyzi_out[4 * offsets_out[i] .. 4 * offsets_out[i + 1]), in the order above; offsets_out has
+ * count + 1 entries; pairs without such a cloud (no loop candidate, invalid Quatro ...) have empty rows.  If the points
+ * exceed `capacity` the call fills offsets_out, writes nothing else and returns B200REG_ESTATE.  offsets_out == NULL:
+ * returns that call's pair count (>= 0) and writes nothing.  A kind that call did not capture, or no capturing call since
+ * the last uncaptured one: B200REG_ESTATE.  A kind that is not one B200REG_CLOUD_* bit: B200REG_EINVAL.              */
+int b200reg_loop_clouds(b200reg_ctx* ctx, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out);
+
 /* ---- clouds: replaces KdTreeFLANN::setInputCloud / buildIndex
  *      (third_party/nano_gicp/include/nano_gicp/nanoflann.hpp:131-138) ----------------- */
 /* Upload `count` clouds (host or device pointers) and build their spatial indices in one
