@@ -305,6 +305,25 @@ __global__ void __launch_bounds__(256) k_gicp_init(const PairDev* pairs, PairSta
 // K2: 15-NN + covariance + PLANE regularisation (nano_gicp_impl.hpp:298-357); the regularisation is
 // cov_regularize_store (smallmath.cuh).
 // ---------------------------------------------------------------------------------------
+// Seed the heap with the K points around position i in Morton order (cheap, coalesced, usually most of the true
+// neighbours: the traversal then starts with a tight bound and only ever inserts improvements) and walk the tree.
+template <typename Heap, int K>
+__device__ __forceinline__ void cov_knn(const CloudDev& c, int i, float4 q, Heap& res) {
+  int lo = max(0, i - K / 2), hi = min(c.n - 1, lo + K - 1);
+  lo = max(0, hi - (K - 1));
+#pragma unroll
+  for (int j = 0; j < K; j++) {
+    if (lo + j <= hi) {
+      const float4 p = __ldg(&c.pts[lo + j]);
+      res.set(j, dist2_rn(q.x, q.y, q.z, p.x, p.y, p.z), lo + j);
+    } else {
+      res.set(j, 3.402823466e+38f, -1);
+    }
+  }
+  res.heapify();
+  knn_walk<Heap>(c, q.x, q.y, q.z, res, lo, hi);
+}
+
 // K is the CAPACITY of the result set; k <= K neighbours enter the covariance (the k nearest of the K nearest are the
 // k nearest), so every k in 1..32 is served by the next instantiated capacity.  k > 32 runs k_covariance_large
 // (knn_large.cu), one warp per point.
@@ -318,26 +337,19 @@ __global__ void __launch_bounds__(STEP_THREADS, (K <= 16 ? 10 : 4)) k_covariance
   __shared__ int s_hp[K][STEP_THREADS];
   if (i >= c.n) return;
   const float4 q = c.pts[i];
-  // seed with the K points around i in Morton order (cheap, coalesced, usually most of the true neighbours): the
-  // traversal then starts with a tight bound and only ever inserts improvements
-  int lo = max(0, i - K / 2), hi = min(c.n - 1, lo + K - 1);
-  lo = max(0, hi - (K - 1));
   int nb[K];  // neighbour positions for the covariance
   {
     KnnHeap<K, STEP_THREADS> res;
     res.hd = &s_hd[0][threadIdx.x];
     res.hp = &s_hp[0][threadIdx.x];
-#pragma unroll
-    for (int j = 0; j < K; j++) {
-      if (lo + j <= hi) {
-        const float4 p = __ldg(&c.pts[lo + j]);
-        res.set(j, dist2_rn(q.x, q.y, q.z, p.x, p.y, p.z), lo + j);
-      } else {
-        res.set(j, 3.402823466e+38f, -1);
-      }
+    cov_knn<KnnHeap<K, STEP_THREADS>, K>(c, i, q, res);
+    if (res.ev == res.worst()) {  // cold: an entry tied at the final cut may have been evicted for a higher index (KnnHeap);
+                                  // the exact search rewrites the same shared-memory columns, which the pops below read
+      KnnHeap<K, STEP_THREADS, true> ex;
+      ex.hd = res.hd;
+      ex.hp = res.hp;
+      cov_knn<KnnHeap<K, STEP_THREADS, true>, K>(c, i, q, ex);
     }
-    res.heapify();
-    knn_walk<KnnHeap<K, STEP_THREADS>>(c, q.x, q.y, q.z, res, lo, hi);
     int m = K;
     while (m > k) m = res.pop(m, c.pts);  // k < K: drop the K - k farthest
 #pragma unroll

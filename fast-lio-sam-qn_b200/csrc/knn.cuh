@@ -106,11 +106,12 @@ struct KnnSet {
 // a candidate at EXACTLY the current worst distance -- and is resolved there, cold: among the entries tied at that
 // distance the one with the highest original index is the true worst; the candidate overwrites it in place (same
 // distance: the heap stays a heap) iff its own index is lower.
-template <int K, int stride>
+template <int K, int stride, bool EXACT = false>
 struct KnnHeap {
   float* hd;   // column base: slot j at hd[j * stride] (stride = threads per block, a compile-time constant)
   int* hp;
   float wd;    // cached root distance
+  float ev;    // distance of the entry evicted last (-1: none); see offer
   // a leaf candidate's distance is recomputed from the (L1-resident) point instead of being selected out of eight registers
   __device__ __forceinline__ float leaf_distance(const float (&)[LEAF], int, const float4* __restrict__ pts, int pos, float qx, float qy,
                                                  float qz) const {
@@ -150,6 +151,7 @@ struct KnnHeap {
 #pragma unroll 1
     for (int i = K / 2 - 1; i >= 0; i--) sift(i, d(i), p(i), K);
     wd = d(0);
+    ev = -1.f;
   }
   // sift from the root of a PERFECT tree (K = 2^m - 1: every internal slot has two children), levels unrolled: no bounds
   // checks, the first level's slots are immediates
@@ -168,6 +170,26 @@ struct KnnHeap {
     }
     set(i, cd, cp);
   }
+  // Among the first m slots, move the entry that is worst under the full (d2, original index) order to the root: of the
+  // entries tied at the root's distance, the one with the highest original index (same distance: the heap stays a heap).
+  __device__ __forceinline__ void root_to_true_worst(int m, const float4* __restrict__ pts) {
+    const float top = d(0);
+    int victim = 0, vidx = orig_index(pts, p(0));
+#pragma unroll 1
+    for (int j = 1; j < m; j++)
+      if (d(j) == top) {
+        const int oi = orig_index(pts, p(j));
+        if (oi > vidx) {
+          vidx = oi;
+          victim = j;
+        }
+      }
+    if (victim != 0) {
+      const int t = p(0);
+      hp[0] = p(victim);
+      hp[victim * stride] = t;
+    }
+  }
   // candidate with cd <= worst()
   __device__ __forceinline__ void offer(float cd, int cp, const float4* __restrict__ pts) {
     if (cd == wd) {  // cold: the (d2, original index) rule among everything tied at the worst distance
@@ -184,6 +206,16 @@ struct KnnHeap {
       if (orig_index(pts, cp) < worst_idx) hp[worst_slot * stride] = cp;
       return;
     }
+    // The root is evicted.  If another entry ties with it (then a child of the root does), the one to evict is the highest
+    // original index among them, not whichever entry the distance-only heap put at the root.  EXACT does that at every
+    // eviction; the hot instantiation only records the distance evicted last (evictions only ever lower it), and the
+    // caller redoes the search with EXACT when that equals the final worst distance -- the only case in which an entry of
+    // the final tie group can have been dropped (exact ties at the cut: lattices, duplicates).
+    if (EXACT) {
+      if (d(1) == wd || d(2) == wd) root_to_true_worst(K, pts);
+    } else {
+      ev = wd;
+    }
     if (K == 15) sift_root_perfect<3>(cd, cp);
     else if (K == 31) sift_root_perfect<4>(cd, cp);
     else sift(0, cd, cp, K);
@@ -192,18 +224,7 @@ struct KnnHeap {
   // Remove the worst entry under the full (d2, original index) order from a heap holding m entries; returns m - 1.
   // Only used when fewer neighbours than the capacity are wanted (k < K): cold.
   __device__ __forceinline__ int pop(int m, const float4* __restrict__ pts) {
-    const float top = d(0);
-    int victim = 0, vidx = orig_index(pts, p(0));
-#pragma unroll 1
-    for (int j = 1; j < m; j++)
-      if (d(j) == top) {
-        const int oi = orig_index(pts, p(j));
-        if (oi > vidx) {
-          vidx = oi;
-          victim = j;
-        }
-      }
-    if (victim != 0) hp[victim * stride] = p(0);  // same distance: swap the positions, the root is now the true worst
+    root_to_true_worst(m, pts);  // the root's entry is dropped
     const float ld = d(m - 1);
     const int lp = p(m - 1);
     sift(0, ld, lp, m - 1);

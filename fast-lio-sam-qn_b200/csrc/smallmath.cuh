@@ -163,7 +163,10 @@ __device__ __forceinline__ void cov_regularize_store(double* o, double cxx, doub
     const double mx = fmax(wv[0], fmax(wv[1], wv[2]));
     for (int a = 0; a < 3; a++) {
       const double sgl = fmax(wv[a], 0.0);  // singular value of a PSD matrix
-      vals[a] = fmax(method == 2 ? sgl / mx : sgl, 1e-3);
+      const double f = method == 2 ? sgl / mx : sgl;
+      // std::max(f, 1e-3) as the reference's (s / s.maxCoeff()).array().max(1e-3): at a zero covariance (k = 1, or k copies
+      // of one point) NORMALIZED_MIN_EIG gives 0 / 0 and the NaN is kept (fmax would return 1e-3)
+      vals[a] = f < 1e-3 ? 1e-3 : f;
     }
     double r[6] = {0, 0, 0, 0, 0, 0};
     for (int a = 0; a < 3; a++) {

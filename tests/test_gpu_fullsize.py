@@ -64,6 +64,9 @@ def test_covariances_100k_match_oracle(ctx, ref_oracle, synth):
     o, knn = oracle.covariances(dst, 15, return_knn=True)
     err = np.abs(g - o).reshape(len(dst), -1).max(1)
     assert np.median(err) < 1e-12 and np.quantile(err, 0.999) < 1e-6, (np.median(err), np.quantile(err, 0.999))
+    import gicp_ref
+    r, _ = gicp_ref.Cov(dst, 15).check(g, 3)  # every point within the fp64 restatement's PLANE bound
+    assert np.all(r <= 1), (float(np.max(r)), int((r > 1).sum()))
     gi, gd = ctx.knn(cl, dst[::7], 15)
     assert np.array_equal(gi, knn[::7]), "15-NN index lists must be bit-exact at 100k"
     cl.destroy()

@@ -290,6 +290,7 @@ def test_cuda_gicp_equals_oracle_golden(ctx, synth):
 
 def test_any_k_correspondences(ctx, oracle, pair5k):
     """setCorrespondenceRandomness(k) for k outside the tuned 15/20 (the NanoGICP default ctor uses 20)."""
+    import gicp_ref
     src, dst, _ = pair5k
     for k in (5, 12, 20, 27):
         cl, = ctx.create_clouds([dst])
@@ -298,6 +299,8 @@ def test_any_k_correspondences(ctx, oracle, pair5k):
         o = oracle.covariances(dst, k)
         err = np.abs(g - o).reshape(len(dst), -1).max(1)
         assert np.median(err) < 1e-11 and np.quantile(err, 0.995) < 1e-5, (k, np.median(err))
+        r, _ = gicp_ref.Cov(dst, k).check(g, 3)  # every point within the fp64 restatement's PLANE bound
+        assert np.all(r <= 1), (k, float(np.max(r)))
         gi, gd = ctx.knn(cl, src[:500], k)
         oi, od = oracle.knn(dst, src[:500], k)
         assert np.array_equal(gi, oi) and np.array_equal(gd, od)
@@ -413,7 +416,9 @@ def test_all_regularization_methods(ctx, oracle, synth, pair5k):
     """setRegularizationMethod: NONE, MIN_EIG, NORMALIZED_MIN_EIG, PLANE, FROBENIUS (nano_gicp_impl.hpp:323-353)."""
     import b200reg
     from oracle.oracle import GicpParams
+    import gicp_ref
     src, dst, Texp = pair5k
+    ref = gicp_ref.Cov(dst, 15)
     cl, = ctx.create_clouds([dst])
     for method in (0, 1, 2, 3, 4):
         ctx.covariances([cl], 15, method)
@@ -422,6 +427,8 @@ def test_all_regularization_methods(ctx, oracle, synth, pair5k):
         scale = np.abs(o).reshape(len(o), -1).max(1) + 1e-12
         err = np.abs(g - o).reshape(len(o), -1).max(1) / scale
         assert np.median(err) < 1e-10 and np.quantile(err, 0.995) < 1e-5, (method, np.median(err), np.quantile(err, 0.995))
+        r, _ = ref.check(g, method)  # and every point within the fp64 restatement's bound (tests/gicp_ref.py)
+        assert np.all(r <= 1), (method, float(np.max(r)), int((r > 1).sum()))
     cl.destroy()
     # the registration honours the method end to end (MIN_EIG here)
     prm = b200reg.default_params()
