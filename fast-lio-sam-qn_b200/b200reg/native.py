@@ -394,8 +394,8 @@ class Context:
         if not want_corr:
             _check(lib().b200reg_quatro_align(self.h, cnt, sa, da, C.byref(prm), info, None))
             return [i.as_dict() for i in info]
-        # enough for any answer: optimizedMatching keeps at most MAXC pairs, advancedMatching's pairs are one-to-one
-        cap = sum(MAXC if prm.use_optimized_matching else min(s.n, d.n) for s, d in zip(srcs, dsts))
+        # enough for any answer: optimizedMatching keeps at most max_corres + 3 pairs, advancedMatching's pairs are one-to-one
+        cap = sum(max(MAXC, prm.max_corres + 3) if prm.use_optimized_matching else min(s.n, d.n) for s, d in zip(srcs, dsts))
         offsets = np.empty(cnt + 1, np.int64)
         corr = np.empty((max(cap, 1), 2), np.int32)
         _check(lib().b200reg_quatro_align_ex(self.h, cnt, sa, da, C.byref(prm), info, offsets.ctypes.data_as(C.c_void_p),

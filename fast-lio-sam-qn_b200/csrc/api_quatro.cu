@@ -162,12 +162,16 @@ static QuatroParamsDev quatro_params_dev(const b200reg_quatro_params* prm, bool 
 // corr_csr: `capacity` pairs, or NULL).  Every pair is matched and, if its set holds at most BIGC correspondences,
 // solved in one batched pass.  A larger advancedMatching set is then solved on its own in one workspace shared by all
 // such pairs of the call (sized for the largest), one pair after another, so device memory stays bounded by the largest.
+// optimizedMatching keeps at most max_corres + 3 <= BIGC: k_teaser_solve solves the sets of at most MAXC in that pass,
+// and the larger ones are solved afterwards in one batched pass of the global-memory chain.
 static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst, const b200reg_quatro_params* prm,
                       b200reg_quatro_info* out, int32_t* corr_fixed, int64_t* offsets_out, size_t capacity, int32_t* corr_csr) {
   if (!c || count <= 0 || !src || !dst || !prm || !out) return fail(B200REG_EINVAL, "bad argument");
   if (prm->estimate_scale) return fail(B200REG_EINVAL, "estimate_scale is not supported (the deployment sets it false)");
   const bool advanced = !prm->use_optimized_matching;  // Matcher::advancedMatching (matcher.cc:118-356)
-  if (!advanced && (prm->max_corres < 1 || prm->max_corres > MAXC - 3)) return fail(B200REG_EINVAL, "max_corres must be in 1..509");
+  if (!advanced && (prm->max_corres < 1 || prm->max_corres > OPT_MAX_CORRES)) return fail(B200REG_EINVAL, "max_corres must be in 1..8189");
+  // optimizedMatching's out_corr: MAXC pairs, or max_corres + 3 when that is more
+  const int opt_cap = advanced ? 0 : std::max(MAXC, prm->max_corres + 3);
   const int corr_stride = advanced ? BIGC : MAXC;  // B200REG_ADV_CORR_CAPACITY / B200REG_CORR_CAPACITY
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
@@ -200,7 +204,7 @@ static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* sr
     int cap = 1024;
     while (advanced && cap < (int)nj && cap < BIGC) cap <<= 1;
     const size_t o_cor = l.take(2 * nj * 4), o_tk = l.take(nj * 4), o_cnt = l.take(8 * 4), o_st = l.take(8 * 8),
-                 o_oc = l.take(2 * (size_t)(advanced ? cap : MAXC) * 4), o_T = l.take(16 * 8);
+                 o_oc = l.take(2 * (size_t)(advanced ? cap : opt_cap) * 4), o_T = l.take(16 * 8);
     const size_t o_big = advanced ? l.take(sizeof(BigSolveWs)) : 0;
     const BigWsLayout wl(l, advanced ? cap : 0, 0);  // empty when !advanced
     char* slab = nullptr;
@@ -264,6 +268,21 @@ static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* sr
       max_wide = std::max(max_wide, n);
       max_src = std::max(max_src, pairs[i].swapped ? pairs[i].fj.n : pairs[i].fi.n);
     }
+  // optimizedMatching sets beyond MAXC: k_teaser_solve left them unsolved
+  std::vector<int> big;
+  int max_big = 0;
+  for (int i = 0; i < count && !advanced; i++)
+    if (counters[8 * i + 2] > MAXC) {
+      const int n = counters[8 * i + 2];
+      if (corr_fixed) {
+        char msg[200];
+        snprintf(msg, sizeof msg, "optimizedMatching kept %d correspondences for pair %d; corr_out holds %d per pair "
+                 "(b200reg_quatro_align_ex returns any number)", n, i, MAXC);
+        return fail(B200REG_ESTATE, msg);
+      }
+      big.push_back(i);
+      max_big = std::max(max_big, n);
+    }
   std::vector<int64_t> offsets;
   if (offsets_out) {
     offsets.assign(count + 1, 0);
@@ -278,6 +297,42 @@ static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* sr
       for (int i = 0; i < count; i++)
         if (counters[8 * i + 6] == 0 && counters[8 * i + 2] > 0)
           CU(cudaMemcpyAsync(corr_csr + 2 * offsets[i], pairs[i].out_corr, (size_t)counters[8 * i + 2] * 8, cudaMemcpyDeviceToHost, s));
+  }
+  // each optimizedMatching set beyond MAXC gets a workspace for its own size, and all of them are solved in one batched
+  // pass; each pair's view reads its own out_corr and writes its own counters and T
+  std::vector<MatchDev> big_views(big.size());
+  std::vector<BigSolveWs> big_ws(big.size());
+  if (!big.empty()) {
+    const int nb = (int)big.size();
+    Layout l;
+    const size_t o_views = l.take(sizeof(MatchDev) * nb), o_ws = l.take(sizeof(BigSolveWs) * nb);
+    std::vector<BigWsLayout> wls;
+    wls.reserve(nb);
+    for (int i : big) wls.emplace_back(l, std::max(1024, pow2_at_least(counters[8 * i + 2])), 0);
+    char* slab = nullptr;
+    if (scratch.alloc((void**)&slab, l.size) != cudaSuccess) {
+      cudaGetLastError();
+      char msg[200];
+      snprintf(msg, sizeof msg, "optimizedMatching kept up to %d correspondences; solving them needs a workspace of %zu bytes, "
+               "which could not be allocated", max_big, l.size);
+      return fail(B200REG_ECUDA, msg);
+    }
+    for (int k = 0; k < nb; k++) {
+      big_ws[k] = wls[k].bind(slab);
+      big_views[k] = pairs[big[k]];
+      big_views[k].big = (BigSolveWs*)(slab + o_ws) + k;
+    }
+    CU(cudaMemcpyAsync(slab + o_ws, big_ws.data(), sizeof(BigSolveWs) * nb, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(slab + o_views, big_views.data(), sizeof(MatchDev) * nb, cudaMemcpyHostToDevice, s));
+    {
+      ProfScope ps(c, CLS_MATCH);
+      c->launches += launch_big_solve((const MatchDev*)(slab + o_views), nb, max_big, q, s);
+    }
+    CU(cudaGetLastError());
+    for (int i : big) {
+      CU(cudaMemcpyAsync(&counters[8 * i], pairs[i].counters, 32, cudaMemcpyDeviceToHost, s));
+      CU(cudaMemcpyAsync(out[i].T, pairs[i].T, 128, cudaMemcpyDeviceToHost, s));
+    }
   }
   if (!wide.empty()) {
     const int cap = (max_wide + 1023) / 1024 * 1024;

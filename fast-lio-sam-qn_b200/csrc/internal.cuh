@@ -240,14 +240,16 @@ struct MatchDev {
   unsigned* tkey;      // [nj] first (trial*4 + slot) at which correspondence r would be added
   int* counters;       // [0] unused, [1] ncorr, [2] n_out, [3] valid, [4] clique size, [5] gnc iterations
   double* stats;       // [0..2] sum fi, [3..5] sum fj, then floats: mean fi(3) mean fj(3) scale (as float bits in doubles)
-  int* out_corr;       // [2 * corr_cap] final (src, dst) pairs (corr_cap = MAXC, or BigSolveWs::cap for advancedMatching)
+  int* out_corr;       // [2 * corr_cap] final (src, dst) pairs (corr_cap = max(MAXC, max_corres + 3) for
+                       // optimizedMatching, BigSolveWs::cap for advancedMatching)
   double* T;           // [16] row-major result
   struct BigSolveWs* big;  // global-memory solver workspace (advancedMatching only; nullptr otherwise)
   int* clique;         // [MAXC] or nullptr: k_teaser_solve lists the clique here, ascending (b200reg_quatro_solve_tap)
 };
 
 // Global-memory workspace of the multi-kernel TEASER++ solve used when the correspondence set is not capped at MAXC
-// (Matcher::advancedMatching, matcher.cc:118-356).  cap is a multiple of 1024, words = cap / 32, p2 = the power of two
+// (Matcher::advancedMatching, matcher.cc:118-356) or exceeds it (optimizedMatching with max_corres > MAXC - 3).
+// cap is a multiple of 1024, words = cap / 32, p2 = the power of two
 // >= cap (the bitonic sorts' length).  big_ws_layout (api_quatro.cu) is the one place that sizes it.
 struct BigSolveWs {
   int cap, words, p2;
@@ -275,10 +277,21 @@ struct QuatroParamsDev {
   int advanced;        // 1: Matcher::advancedMatching (cross check, 3-edge tuple test, no cap); 0: optimizedMatching
 };
 
-constexpr int MAXC = 512;  // capacity of the final correspondence set (max_corres + 3 <= MAXC)
+constexpr int MAXC = 512;  // largest set k_teaser_solve holds in shared memory (B200REG_CORR_CAPACITY)
 constexpr int BIGC = 8192; // largest advancedMatching set solved per pair in one batched pass (B200REG_ADV_CORR_CAPACITY);
                            // larger sets are solved one pair at a time in a workspace sized for them
 constexpr int BIG_NMAX = 1 << 20;  // sets must stay below this: k_big_core packs vertex indices into 20 bits
+// optimizedMatching keeps at most max_corres + 3 correspondences (the tuple test stops after the trial that passes
+// max_corres), so with max_corres <= OPT_MAX_CORRES every set fits one batched pass of the global-memory chain
+constexpr int OPT_MAX_CORRES = BIGC - 3;
+
+// k_tuple_select's sort length (its dynamic shared memory holds this many 8-byte keys): the power of two that holds
+// max_corres + 3 keys, at least 1024
+__host__ __device__ inline int tuple_sort_len(int max_corres) {
+  int p = 1024;
+  while (p < max_corres + 3) p <<= 1;
+  return p;
+}
 
 // ---- ordered-int encoding of floats for atomicMin/atomicMax ------------------------
 __device__ __forceinline__ int f2ord(float f) {

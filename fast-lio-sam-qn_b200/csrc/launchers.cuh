@@ -30,10 +30,14 @@ void launch_transform_out(const CloudDev& c, const float* d_Tf, float* d_out3, c
 // quatro.cu
 cudaError_t quatro_init_device();
 int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2, float fpfh_r2, cudaStream_t s);
+// optimizedMatching: k_teaser_solve solves the sets of at most MAXC and leaves larger ones (counters[2] > MAXC) to
+// launch_big_solve
 int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, int max_nj, const QuatroParamsDev& prm, cudaStream_t s);
 // k_teaser_solve alone (one block of solve_smem_bytes() per pair): counters[2] correspondences listed in out_corr
 size_t solve_smem_bytes();
 int launch_teaser_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, cudaStream_t s);
+// k_big_gather + launch_big_graph_solve(n_wide = 0): pairs of at most max_n <= BIGC correspondences, `big` bound
+int launch_big_solve(const MatchDev* d_pairs, int count, int max_n, const QuatroParamsDev& prm, cudaStream_t s);
 int launch_adv_wide(const MatchDev* d_pair, int n, const QuatroParamsDev& prm, cudaStream_t s);
 int launch_big_graph_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, int n_wide, cudaStream_t s);
 void launch_transform_raw(const CloudDev* d_clouds, const double* d_T16s, int count, int max_n, float4* const* d_outs, cudaStream_t s);

@@ -797,13 +797,15 @@ __global__ void __launch_bounds__(256) k_tuple_trials(const MatchDev* pairs, Qua
 }
 
 // serial semantics recovered: the loop stops after the first trial that leaves more than max_corres unique
-// correspondences; the survivors are emitted in insertion order.  One block per pair.
+// correspondences; the survivors are emitted in insertion order.  One block per pair; at most max_corres + 3 survive
+// (each trial adds up to three), and the sort holds tuple_sort_len(max_corres) >= max_corres + 3 keys.
 __global__ void __launch_bounds__(1024) k_tuple_select(const MatchDev* pairs, QuatroParamsDev prm) {
+  extern __shared__ __align__(16) unsigned long long keys[];  // [tuple_sort_len(prm.max_corres)]
   const MatchDev& P = pairs[blockIdx.x];
   const int ncorr = P.counters[1];
+  const int L = tuple_sort_len(prm.max_corres);
   __shared__ unsigned hist[256];
   __shared__ unsigned prefix, remaining, tstar;
-  __shared__ unsigned long long keys[1024];
   __shared__ int nsel;
   if (ncorr == 0) {
     if (threadIdx.x == 0) P.counters[2] = 0;
@@ -856,32 +858,34 @@ __global__ void __launch_bounds__(1024) k_tuple_select(const MatchDev* pairs, Qu
     if (k == 0xFFFFFFFFu) continue;
     if (ts == 0xFFFFFFFFu || (k >> 2) <= ts) {
       const int s = atomicAdd(&nsel, 1);
-      if (s < 1024) keys[s] = ((unsigned long long)k << 32) | (unsigned)r;
+      if (s < L) keys[s] = ((unsigned long long)k << 32) | (unsigned)r;
     }
   }
   __syncthreads();
-  const int n = min(nsel, MAXC);
-  for (int s = threadIdx.x; s < 1024; s += 1024)
+  const int n = min(nsel, L);
+  for (int s = threadIdx.x; s < L; s += 1024)
     if (s >= nsel) keys[s] = 0xFFFFFFFFFFFFFFFFull;
   __syncthreads();
-  for (int k = 2; k <= 1024; k <<= 1)
+  for (int k = 2; k <= L; k <<= 1)
     for (int j = k >> 1; j > 0; j >>= 1) {
-      const int i = threadIdx.x, l = i ^ j;
-      if (l > i) {
-        const unsigned long long a = keys[i], b = keys[l];
-        const bool up = (i & k) == 0;
-        if ((a > b) == up) {
-          keys[i] = b;
-          keys[l] = a;
+      for (int i = threadIdx.x; i < L; i += 1024) {
+        const int l = i ^ j;
+        if (l > i) {
+          const unsigned long long a = keys[i], b = keys[l];
+          const bool up = (i & k) == 0;
+          if ((a > b) == up) {
+            keys[i] = b;
+            keys[l] = a;
+          }
         }
       }
       __syncthreads();
     }
-  if ((int)threadIdx.x < n) {
-    const int r = (int)(keys[threadIdx.x] & 0xFFFFFFFFu);
+  for (int s = threadIdx.x; s < n; s += 1024) {
+    const int r = (int)(keys[s] & 0xFFFFFFFFu);
     const int i = P.corres[2 * r], j = P.corres[2 * r + 1];
-    P.out_corr[2 * threadIdx.x] = P.swapped ? j : i;      // always (src, dst) (matcher.cc:527-535)
-    P.out_corr[2 * threadIdx.x + 1] = P.swapped ? i : j;
+    P.out_corr[2 * s] = P.swapped ? j : i;      // always (src, dst) (matcher.cc:527-535)
+    P.out_corr[2 * s + 1] = P.swapped ? i : j;
   }
   if (threadIdx.x == 0) P.counters[2] = n;
 }
@@ -941,7 +945,9 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
     P.counters[4] = 0;
     P.counters[5] = 0;
   }
-  if (n == 0) return;
+  // a set beyond MAXC (optimizedMatching with max_corres > 509) does not fit here: quatro_align_impl hands it to the
+  // global-memory chain (k_big_gather, launch_big_graph_solve)
+  if (n == 0 || n > MAXC) return;
   const CloudDev& src = P.swapped ? P.fj : P.fi;
   const CloudDev& dst = P.swapped ? P.fi : P.fj;
   for (int i = tid; i < n; i += SV_THREADS) {
@@ -1863,6 +1869,8 @@ cudaError_t quatro_init_device() {
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(k_big_greedy_wide, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM);
   if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(k_tuple_select, cudaFuncAttributeMaxDynamicSharedMemorySize, tuple_sort_len(OPT_MAX_CORRES) * 8);
+  if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(k_adv_select, cudaFuncAttributeMaxDynamicSharedMemorySize, BIGC * 8);
 }
 
@@ -1882,12 +1890,18 @@ int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, in
   k_mutual<<<count, 1024, 0, s>>>(d_pairs, prm.thr2, prm.advanced); l++;
   k_tuple_trials<<<dim3(128, count), 256, 0, s>>>(d_pairs, prm); l++;
   if (!prm.advanced) {
-    k_tuple_select<<<count, 1024, 0, s>>>(d_pairs, prm); l++;
+    k_tuple_select<<<count, 1024, (size_t)tuple_sort_len(prm.max_corres) * 8, s>>>(d_pairs, prm); l++;
     return l + launch_teaser_solve(d_pairs, count, prm, s);
   }
   k_adv_select<<<count, 1024, BIGC * 8, s>>>(d_pairs, prm); l++;
-  k_big_gather<<<dim3(BIGC / 256, count), 256, 0, s>>>(d_pairs); l++;
-  return l + launch_big_graph_solve(d_pairs, count, prm, 0, s);
+  return l + launch_big_solve(d_pairs, count, BIGC, prm, s);
+}
+
+// the global-memory TEASER++ solve of sets of at most BIGC correspondences (out_corr listed, counters[2] set, each
+// pair's `big` workspace bound), max_n the largest set of the batch: gather, then one batched pass
+int launch_big_solve(const MatchDev* d_pairs, int count, int max_n, const QuatroParamsDev& prm, cudaStream_t s) {
+  k_big_gather<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_pairs);
+  return 1 + launch_big_graph_solve(d_pairs, count, prm, 0, s);
 }
 
 // one pair whose advancedMatching set outgrew k_adv_select (n > BIGC correspondences, counters[6] = n): select into the

@@ -10,7 +10,9 @@ template <typename PointType>
 class quatro {
  public:
   quatro() { b200reg_default_quatro_params(&prm_); }
-  // fast_lio_sam_qn/src/loop_closure.cpp:18-27 passes all ten arguments
+  // fast_lio_sam_qn/src/loop_closure.cpp:18-27 passes all ten arguments.  num_max_corres: 1..8189 with optimized
+  // matching (at most num_max_corres + 3 correspondences are kept and solved); a larger value makes align() print the
+  // refusal to stderr and return Identity / invalid
   quatro(const double& fpfh_normal_radi, const double& fpfh_radi, const double noise_bound, const double& rot_gnc_fact,
          const double& rot_cost_thr, const int& rot_max_iter, const bool& estimat_scale, const bool& use_optimized_matching = true,
          const double& distance_threshold = 30.0, const int& num_max_corres = 200) {

@@ -93,7 +93,7 @@ typedef struct b200reg_quatro_params {
   double rot_gnc_factor;       /* 1.4                                                                 */
   double rot_cost_thr;         /* 1e-4                                                                */
   int32_t rot_max_iter;        /* 50                                                                  */
-  int32_t max_corres;          /* num_max_corres (200); must be <= 509                                */
+  int32_t max_corres;          /* num_max_corres (200); optimizedMatching: 1..8189 (B200REG_ADV_CORR_CAPACITY - 3) */
   double distance_threshold;   /* FEATURE-space gate of optimizedMatching (matcher.cc:422/444) (35)   */
   double tuple_scale;          /* 0.95 (quatro_module.cc:61)                                          */
   uint64_t seed;               /* replaces srand(time(NULL)) (matcher.cc:465) by a counter-based RNG  */
@@ -260,7 +260,9 @@ int b200reg_clouds_fpfh(b200reg_ctx* ctx, int count, b200reg_cloud* const* cloud
  * pair, CAP = B200REG_CORR_CAPACITY (optimized) or B200REG_ADV_CORR_CAPACITY (advanced).  advancedMatching sets of any
  * size (below 2^20) are solved; a set larger than B200REG_ADV_CORR_CAPACITY does not fit corr_out, so with a non-NULL
  * corr_out such a set fails the call with B200REG_ESTATE (nothing is truncated silently), and with corr_out NULL the
- * call solves it.  b200reg_quatro_align_ex returns the correspondences of any size.
+ * call solves it.  optimizedMatching keeps at most max_corres + 3 correspondences (up to 8192); the same rule holds at
+ * its CAP: with max_corres > 509 a set of more than B200REG_CORR_CAPACITY fails a call with a non-NULL corr_out with
+ * B200REG_ESTATE, naming the pair and the count.  b200reg_quatro_align_ex returns the correspondences of any size.
  * Pairs with at most B200REG_ADV_CORR_CAPACITY correspondences are solved together; larger sets are solved one pair at
  * a time in one device workspace sized for the largest (about n^2 / 4 bytes for n correspondences: 1 GB at n = 65536).
  * If that workspace cannot be allocated the call returns B200REG_ECUDA with the bytes needed in the message.     */
