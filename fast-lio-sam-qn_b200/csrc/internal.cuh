@@ -250,7 +250,7 @@ struct MatchDev {
 // Global-memory workspace of the multi-kernel TEASER++ solve used when the correspondence set is not capped at MAXC
 // (Matcher::advancedMatching, matcher.cc:118-356) or exceeds it (optimizedMatching with max_corres > MAXC - 3).
 // cap is a multiple of 1024, words = cap / 32, p2 = the power of two
-// >= cap (the bitonic sorts' length).  big_ws_layout (api_quatro.cu) is the one place that sizes it.
+// >= cap (the bitonic sorts' length).  BigWsLayout (api_quatro.cu) is the one place that sizes it.
 struct BigSolveWs {
   int cap, words, p2;
   double* S;                 // [cap * 3] source points of the correspondences

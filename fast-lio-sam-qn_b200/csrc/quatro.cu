@@ -796,6 +796,32 @@ __global__ void __launch_bounds__(256) k_tuple_trials(const MatchDev* pairs, Qua
   }
 }
 
+// bitonic sort network over `len` slots (a power of two) by the NT threads of a block, ending with a barrier.
+// cmp_swap(i, l, up) with i < l puts slots i and l in ascending order when up, descending otherwise.
+template <int NT, class CmpSwap>
+__device__ __forceinline__ void block_bitonic(int len, CmpSwap cmp_swap) {
+  for (int k = 2; k <= len; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = threadIdx.x; i < len; i += NT) {
+        const int l = i ^ j;
+        if (l > i) cmp_swap(i, l, (i & k) == 0);
+      }
+      __syncthreads();
+    }
+}
+
+// compare-exchange of packed u64 keys (the sorts of the matcher's selections and of the clique order)
+struct KeyCmpSwap {
+  unsigned long long* key;
+  __device__ __forceinline__ void operator()(int i, int l, bool up) const {
+    const unsigned long long a = key[i], b = key[l];
+    if ((a > b) == up) {
+      key[i] = b;
+      key[l] = a;
+    }
+  }
+};
+
 // serial semantics recovered: the loop stops after the first trial that leaves more than max_corres unique
 // correspondences; the survivors are emitted in insertion order.  One block per pair; at most max_corres + 3 survive
 // (each trial adds up to three), and the sort holds tuple_sort_len(max_corres) >= max_corres + 3 keys.
@@ -866,21 +892,7 @@ __global__ void __launch_bounds__(1024) k_tuple_select(const MatchDev* pairs, Qu
   for (int s = threadIdx.x; s < L; s += 1024)
     if (s >= nsel) keys[s] = 0xFFFFFFFFFFFFFFFFull;
   __syncthreads();
-  for (int k = 2; k <= L; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = threadIdx.x; i < L; i += 1024) {
-        const int l = i ^ j;
-        if (l > i) {
-          const unsigned long long a = keys[i], b = keys[l];
-          const bool up = (i & k) == 0;
-          if ((a > b) == up) {
-            keys[i] = b;
-            keys[l] = a;
-          }
-        }
-      }
-      __syncthreads();
-    }
+  block_bitonic<1024>(L, KeyCmpSwap{keys});
   for (int s = threadIdx.x; s < n; s += 1024) {
     const int r = (int)(keys[s] & 0xFFFFFFFFu);
     const int i = P.corres[2 * r], j = P.corres[2 * r + 1];
@@ -893,6 +905,211 @@ __global__ void __launch_bounds__(1024) k_tuple_select(const MatchDev* pairs, Qu
 // ------------------------------------------------------------------------------------------------
 // Q5 TEASER++ solve (QUATRO rotation, PMC_HEU-style clique), one block per pair
 // ------------------------------------------------------------------------------------------------
+// Two implementations share the stages below: k_teaser_solve (one 256-thread block per pair, everything in shared
+// memory, sets of at most MAXC) and the k_big_* chain (global-memory BigSolveWs, 1024-thread blocks, any size).  They
+// differ in storage, block size, core peeling and clique search.  quatro.cu is built with -fmad=false, so the order of
+// operations written here fixes the result; the thread-strided partial sums take the block size as their stride, which
+// is why the two paths' reductions round differently.  Helpers that hold a barrier are called by every thread of the
+// block.
+
+// block reduction in a fixed order: butterfly inside each warp, then over the NT / 32 warp results, lanes beyond them
+// contributing `identity` (two barriers per reduction; a shared-memory tree cost nine, and the GNC loop does six
+// reductions per iteration).  red holds NT / 32 values.
+template <int NT, class T, class Op>
+__device__ __forceinline__ T block_reduce(T v, T* red, Op op, T identity) {
+  for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
+  __syncthreads();  // the previous reduction's readers are done with red
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  T r = (threadIdx.x & 31) < NT / 32 ? red[threadIdx.x & 31] : identity;
+  for (int o = 16; o > 0; o >>= 1) r = op(r, __shfl_xor_sync(0xffffffffu, r, o));
+  return r;
+}
+struct SumOp {
+  __device__ __forceinline__ double operator()(double a, double b) const { return a + b; }
+};
+struct MaxOp {
+  __device__ __forceinline__ double operator()(double a, double b) const { return fmax(a, b); }
+};
+
+// compare-exchange of TLS interval ends by (value, original slot), i.e. std::stable_sort by value.  hidx is k + 1 at
+// the lower end of interval k (slot 2k), -(k + 1) at its upper end (slot 2k + 1) and 0 in the padding, which sorts last.
+struct IntervalCmpSwap {
+  double* val;
+  int* idx;
+  __device__ __forceinline__ void operator()(int i, int l, bool up) const {
+    const double a = val[i], b = val[l];
+    const int ia = idx[i], ib = idx[l];
+    const int sa = ia > 0 ? 2 * (ia - 1) : 2 * (-ia - 1) + 1, sb = ib > 0 ? 2 * (ib - 1) : 2 * (-ib - 1) + 1;
+    const bool gt = a > b || (a == b && (ia == 0 ? 1 << 30 : sa) > (ib == 0 ? 1 << 30 : sb));
+    if (gt == up) {
+      val[i] = b; val[l] = a;
+      idx[i] = ib; idx[l] = ia;
+    }
+  }
+};
+
+// TIM scale-consistency edge between correspondences i and j: | ||b_ij|| - ||a_ij|| | <= 2 * noise_bound = beta
+// (cbar2 = 1, quatro_module.cc:40).  Symmetric bit for bit ((x - y)^2 == (y - x)^2).
+__device__ __forceinline__ bool tim_edge(const double* si, const double* di, const double* sj, const double* dj, double beta) {
+  double a = 0, b = 0;
+#pragma unroll
+  for (int d = 0; d < 3; d++) {
+    const double da = sj[d] - si[d], db = dj[d] - di[d];
+    a += da * da;
+    b += db * db;
+  }
+  return fabs(sqrt(a) - sqrt(b)) <= beta;
+}
+
+// before anything is known: T = identity, not valid, no clique, no GNC iterations (thread i of the pair's threads)
+__device__ __forceinline__ void reset_result(const MatchDev& P, int i) {
+  if (i < 16) P.T[i] = (i % 5 == 0) ? 1.0 : 0.0;
+  if (i == 0) {
+    P.counters[3] = 0;
+    P.counters[4] = 0;
+    P.counters[5] = 0;
+  }
+}
+
+// the valid answer: yaw rotation R2 (row-major 2 x 2), translation t (one thread)
+__device__ __forceinline__ void write_result(const MatchDev& P, const double* R2, const double* t, int iters) {
+  P.T[0] = R2[0]; P.T[1] = R2[1]; P.T[2] = 0; P.T[3] = t[0];
+  P.T[4] = R2[2]; P.T[5] = R2[3]; P.T[6] = 0; P.T[7] = t[1];
+  P.T[8] = 0; P.T[9] = 0; P.T[10] = 1; P.T[11] = t[2];
+  P.T[12] = 0; P.T[13] = 0; P.T[14] = 0; P.T[15] = 1;
+  P.counters[3] = 1;
+  P.counters[5] = iters;
+}
+
+// block-wide state of the GNC-TLS rotation, in shared memory
+struct GncState {
+  double mu, prev_cost, R2[4];
+  int stop;
+};
+
+// GNC-TLS with a weighted 2-D (yaw-only) Kabsch step on the chain TIMs of the clique's m members.  S and D hold the
+// correspondences' points with stride 3; w and res hold m - 1 values, red NT / 32.  Leaves the rotation in g.R2 and
+// returns the number of iterations.
+template <int NT>
+__device__ int gnc_tls_yaw(const double* S, const double* D, const int* clique, int m, double* w, double* res, double* red,
+                           GncState& g, const QuatroParamsDev& prm) {
+  const int tid = threadIdx.x;
+  const int nt = m - 1;
+  double nb2 = prm.noise_bound * prm.noise_bound;
+  if (nb2 < 1e-16) nb2 = 1e-2;
+  for (int k = tid; k < nt; k += NT) w[k] = 1.0;
+  if (tid == 0) {
+    g.mu = 1.0;
+    g.prev_cost = INFINITY;
+    g.stop = 0;
+    g.R2[0] = 1; g.R2[1] = 0; g.R2[2] = 0; g.R2[3] = 1;
+  }
+  __syncthreads();
+  int iters = 0;
+  for (int it = 0; it < prm.max_iter; it++) {
+    iters = it + 1;
+    double h0 = 0, h1 = 0, h2 = 0, h3 = 0;
+    for (int k = tid; k < nt; k += NT) {
+      const int c0 = clique[k], c1 = clique[k + 1];
+      const double ax = S[3 * c1] - S[3 * c0], ay = S[3 * c1 + 1] - S[3 * c0 + 1];
+      const double bx = D[3 * c1] - D[3 * c0], by = D[3 * c1 + 1] - D[3 * c0 + 1];
+      const double wk = w[k];
+      h0 += ax * wk * bx; h1 += ax * wk * by; h2 += ay * wk * bx; h3 += ay * wk * by;
+    }
+    h0 = block_reduce<NT>(h0, red, SumOp(), 0.0);
+    h1 = block_reduce<NT>(h1, red, SumOp(), 0.0);
+    h2 = block_reduce<NT>(h2, red, SumOp(), 0.0);
+    h3 = block_reduce<NT>(h3, red, SumOp(), 0.0);
+    const double th = atan2(h1 - h2, h0 + h3);
+    const double cs = cos(th), sn = sin(th);
+    double mx = 0;
+    for (int k = tid; k < nt; k += NT) {
+      const int c0 = clique[k], c1 = clique[k + 1];
+      const double ax = S[3 * c1] - S[3 * c0], ay = S[3 * c1 + 1] - S[3 * c0 + 1], az = S[3 * c1 + 2] - S[3 * c0 + 2];
+      const double bx = D[3 * c1] - D[3 * c0], by = D[3 * c1 + 1] - D[3 * c0 + 1], bz = D[3 * c1 + 2] - D[3 * c0 + 2];
+      const double rx = bx - (cs * ax - sn * ay), ry = by - (sn * ax + cs * ay), rz = bz - az;
+      const double r = rx * rx + ry * ry + rz * rz;
+      res[k] = r;
+      mx = fmax(mx, r);
+    }
+    mx = block_reduce<NT>(mx, red, MaxOp(), 0.0);  // of non-negative values
+    if (tid == 0) {
+      g.R2[0] = cs; g.R2[1] = -sn; g.R2[2] = sn; g.R2[3] = cs;
+      if (it == 0) {
+        g.mu = 1.0 / (2.0 * mx / nb2 - 1.0);
+        if (g.mu <= 0) g.stop = 1;
+      }
+    }
+    __syncthreads();
+    if (g.stop) break;
+    const double mu = g.mu;
+    const double th1 = (mu + 1) / mu * nb2, th2 = mu / (mu + 1) * nb2;
+    double cost = 0;
+    for (int k = tid; k < nt; k += NT) {
+      const double r = res[k];
+      cost += w[k] * r;
+      w[k] = r >= th1 ? 0.0 : (r <= th2 ? 1.0 : sqrt(nb2 * mu * (mu + 1) / r) - mu);
+    }
+    cost = block_reduce<NT>(cost, red, SumOp(), 0.0);
+    if (tid == 0) {
+      const double diff = fabs(cost - g.prev_cost);
+      g.mu = mu * prm.gnc_factor;
+      g.prev_cost = cost;
+      if (diff < prm.cost_thr) g.stop = 1;
+    }
+    __syncthreads();
+    if (g.stop) break;
+  }
+  __syncthreads();
+  return iters;
+}
+
+// the 2m interval ends of axis d's TLS vote, [x_k - range, x_k + range] for x_k = D[c_k][d] - (R2 S[c_k])[d] over the
+// clique members c_k, sorted by (value, slot) over len slots (the power of two >= 2m, at least 2); x_k goes to res[k]
+template <int NT>
+__device__ void tls_sorted_intervals(const double* S, const double* D, const int* clique, int m, const double* R2, int d, double range,
+                                     int len, double* res, double* hval, int* hidx) {
+  const int tid = threadIdx.x;
+  for (int k = tid; k < len; k += NT) {
+    hval[k] = INFINITY;
+    hidx[k] = 0;
+  }
+  __syncthreads();
+  for (int k = tid; k < m; k += NT) {
+    const int c = clique[k];
+    const double rs = d == 0 ? R2[0] * S[3 * c] + R2[1] * S[3 * c + 1] : (d == 1 ? R2[2] * S[3 * c] + R2[3] * S[3 * c + 1] : S[3 * c + 2]);
+    const double x = D[3 * c + d] - rs;
+    res[k] = x;
+    hval[2 * k] = x - range; hidx[2 * k] = k + 1;
+    hval[2 * k + 1] = x + range; hidx[2 * k + 1] = -k - 1;
+  }
+  __syncthreads();
+  block_bitonic<NT>(len, IntervalCmpSwap{hval, hidx});
+}
+
+// the serial consensus sweep of the TLS estimate over the sorted interval ends of m values: add(eps, X) enters
+// (eps = 1) or leaves (eps = -1) the interval of value X; best is the estimate of the cheapest consensus set so far
+struct TlsSweep {
+  double range, w, ris, dxw = 0, dwc = 0, sxi = 0, sxq = 0, best_cost = INFINITY, best = 0;
+  int card = 0;
+  __device__ __forceinline__ TlsSweep(double range_, int m) : range(range_), w(1.0 / (range_ * range_)), ris(range_ * m) {}
+  __device__ __forceinline__ void add(int eps, double X) {
+    card += eps;
+    dwc += eps * w;
+    dxw += eps * w * X;
+    ris -= eps * range;
+    sxi += eps * X;
+    sxq += eps * X * X;
+    const double xh = dxw / dwc;
+    const double cost = (card * xh * xh + sxq - 2 * sxi * xh) + ris;
+    if (cost < best_cost) {
+      best_cost = cost;
+      best = xh;
+    }
+  }
+};
+
 constexpr int SV_THREADS = 256;
 constexpr int SV_WORDS = MAXC / 32;
 
@@ -908,29 +1125,36 @@ struct SolveSmem {
   double hval[2 * MAXC];
   int hidx[2 * MAXC];
   int m, best_r;
-  double R2[4], mu, prev_cost, t[3];
-  int stop;
+  GncState gnc;
+  double t[3];
 };
 
-// block reductions in a fixed order: butterfly inside each warp, then over the SV_THREADS / 32 warp results (two
-// barriers per reduction; a shared-memory tree cost nine, and the GNC loop does six reductions per iteration)
-__device__ __forceinline__ double block_sum(SolveSmem& sm, double v) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();  // the previous reduction's readers are done with sm.red
-  if ((threadIdx.x & 31) == 0) sm.red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double r = (threadIdx.x & 31) < SV_THREADS / 32 ? sm.red[threadIdx.x & 31] : 0.0;
-  for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
-  return r;
-}
-__device__ __forceinline__ double block_max(SolveSmem& sm, double v) {  // of non-negative values
-  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) sm.red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double r = (threadIdx.x & 31) < SV_THREADS / 32 ? sm.red[threadIdx.x & 31] : 0.0;
-  for (int o = 16; o > 0; o >>= 1) r = fmax(r, __shfl_xor_sync(0xffffffffu, r, o));
-  return r;
+// the greedy clique grown from rank r in k_teaser_solve's rank-space adjacency ("first vertex of P in the global order"
+// is the lowest set bit).  Cm != nullptr collects the members as bits of their original correspondence index.
+__device__ __forceinline__ int greedy_clique(const SolveSmem& sm, int r, unsigned* Cm) {
+  unsigned Pm[SV_WORDS];
+  for (int w = 0; w < SV_WORDS; w++) Pm[w] = sm.radj[r][w];
+  if (Cm) {
+    const int v = sm.order[r];
+    Cm[v >> 5] |= 1u << (v & 31);
+  }
+  int size = 1;
+  for (;;) {
+    int u = -1;
+    for (int w = 0; w < SV_WORDS; w++)
+      if (Pm[w]) {
+        u = w * 32 + __ffs(Pm[w]) - 1;
+        break;
+      }
+    if (u < 0) break;
+    size++;
+    if (Cm) {
+      const int v = sm.order[u];
+      Cm[v >> 5] |= 1u << (v & 31);
+    }
+    for (int w = 0; w < SV_WORDS; w++) Pm[w] &= sm.radj[u][w];
+  }
+  return size;
 }
 
 __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pairs, QuatroParamsDev prm) {
@@ -939,12 +1163,7 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
   const MatchDev& P = pairs[blockIdx.x];
   const int n = P.counters[2];
   const int tid = threadIdx.x;
-  if (tid < 16) P.T[tid] = (tid % 5 == 0) ? 1.0 : 0.0;
-  if (tid == 0) {
-    P.counters[3] = 0;
-    P.counters[4] = 0;
-    P.counters[5] = 0;
-  }
+  reset_result(P, tid);
   // a set beyond MAXC (optimizedMatching with max_corres > 509) does not fit here: quatro_align_impl hands it to the
   // global-memory chain (k_big_gather, launch_big_graph_solve)
   if (n == 0 || n > MAXC) return;
@@ -960,19 +1179,11 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
     }
   }
   __syncthreads();
-  // TIM scale-consistency graph: | ||b_ij|| - ||a_ij|| | <= 2 * noise_bound (cbar2 = 1, quatro_module.cc:40)
   const double beta = 2.0 * prm.noise_bound;
   for (int e = tid; e < n * n; e += SV_THREADS) {
     const int i = e / n, j = e % n;
     if (j <= i) continue;
-    double a = 0, b = 0;
-#pragma unroll
-    for (int d = 0; d < 3; d++) {
-      const double da = sm.S[j][d] - sm.S[i][d], db = sm.D[j][d] - sm.D[i][d];
-      a += da * da;
-      b += db * db;
-    }
-    if (fabs(sqrt(a) - sqrt(b)) <= beta) {
+    if (tim_edge(sm.S[i], sm.D[i], sm.S[j], sm.D[j], beta)) {
       atomicOr(&sm.adj[i][j >> 5], 1u << (j & 31));
       atomicOr(&sm.adj[j][i >> 5], 1u << (i & 31));
     }
@@ -1021,21 +1232,7 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
     sm.skey[i] = i < n ? (((unsigned long long)(MAXC - sm.core[i]) << 40) | ((unsigned long long)(MAXC - sm.deg[i]) << 20) | (unsigned)i)
                        : 0xFFFFFFFFFFFFFFFFull;
   __syncthreads();
-  for (int k = 2; k <= MAXC; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < MAXC; i += SV_THREADS) {
-        const int l = i ^ j;
-        if (l > i) {
-          const unsigned long long a = sm.skey[i], b = sm.skey[l];
-          const bool up = (i & k) == 0;
-          if ((a > b) == up) {
-            sm.skey[i] = b;
-            sm.skey[l] = a;
-          }
-        }
-      }
-      __syncthreads();
-    }
+  block_bitonic<SV_THREADS>(MAXC, KeyCmpSwap{sm.skey});
   for (int r = tid; r < n; r += SV_THREADS) {
     const int v = (int)(sm.skey[r] & 0xFFFFF);
     sm.order[r] = v;
@@ -1053,23 +1250,7 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
   }
   __syncthreads();
   // greedy clique from every start vertex (independent => one thread each)
-  for (int r = tid; r < n; r += SV_THREADS) {
-    unsigned Pm[SV_WORDS];
-    for (int w = 0; w < SV_WORDS; w++) Pm[w] = sm.radj[r][w];
-    int size = 1;
-    for (;;) {
-      int u = -1;
-      for (int w = 0; w < SV_WORDS; w++)
-        if (Pm[w]) {
-          u = w * 32 + __ffs(Pm[w]) - 1;
-          break;
-        }
-      if (u < 0) break;
-      size++;
-      for (int w = 0; w < SV_WORDS; w++) Pm[w] &= sm.radj[u][w];
-    }
-    sm.csize[r] = size;
-  }
+  for (int r = tid; r < n; r += SV_THREADS) sm.csize[r] = greedy_clique(sm, r, nullptr);
   __syncthreads();
   if (tid == 0) {
     int best = 0, br = 0;
@@ -1079,27 +1260,9 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
         br = r;
       }
     // replay the winner and list its members (ascending ORIGINAL correspondence index)
-    unsigned Pm[SV_WORDS], Cm[SV_WORDS];
-    for (int w = 0; w < SV_WORDS; w++) {
-      Pm[w] = sm.radj[br][w];
-      Cm[w] = 0;
-    }
-    {
-      const int v = sm.order[br];
-      Cm[v >> 5] |= 1u << (v & 31);
-    }
-    for (;;) {
-      int u = -1;
-      for (int w = 0; w < SV_WORDS; w++)
-        if (Pm[w]) {
-          u = w * 32 + __ffs(Pm[w]) - 1;
-          break;
-        }
-      if (u < 0) break;
-      const int v = sm.order[u];
-      Cm[v >> 5] |= 1u << (v & 31);
-      for (int w = 0; w < SV_WORDS; w++) Pm[w] &= sm.radj[u][w];
-    }
+    unsigned Cm[SV_WORDS];
+    for (int w = 0; w < SV_WORDS; w++) Cm[w] = 0;
+    greedy_clique(sm, br, Cm);
     int m = 0;
     for (int v = 0; v < n; v++)
       if ((Cm[v >> 5] >> (v & 31)) & 1u) sm.clique[m++] = v;
@@ -1111,148 +1274,28 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
   __syncthreads();
   const int m = sm.m;
   if (m <= 1) return;  // solution_.valid stays false
-  const int nt = m - 1;
-  // GNC-TLS with a weighted 2-D (yaw-only) Kabsch step on the chain TIMs
-  double nb2 = prm.noise_bound * prm.noise_bound;
-  if (nb2 < 1e-16) nb2 = 1e-2;
-  for (int k = tid; k < nt; k += SV_THREADS) sm.w[k] = 1.0;
-  if (tid == 0) {
-    sm.mu = 1.0;
-    sm.prev_cost = INFINITY;
-    sm.stop = 0;
-    sm.R2[0] = 1; sm.R2[1] = 0; sm.R2[2] = 0; sm.R2[3] = 1;
-  }
-  __syncthreads();
-  int iters = 0;
-  for (int it = 0; it < prm.max_iter; it++) {
-    iters = it + 1;
-    double h0 = 0, h1 = 0, h2 = 0, h3 = 0;
-    for (int k = tid; k < nt; k += SV_THREADS) {
-      const int c0 = sm.clique[k], c1 = sm.clique[k + 1];
-      const double ax = sm.S[c1][0] - sm.S[c0][0], ay = sm.S[c1][1] - sm.S[c0][1];
-      const double bx = sm.D[c1][0] - sm.D[c0][0], by = sm.D[c1][1] - sm.D[c0][1];
-      const double w = sm.w[k];
-      h0 += ax * w * bx; h1 += ax * w * by; h2 += ay * w * bx; h3 += ay * w * by;
-    }
-    h0 = block_sum(sm, h0); h1 = block_sum(sm, h1); h2 = block_sum(sm, h2); h3 = block_sum(sm, h3);
-    const double th = atan2(h1 - h2, h0 + h3);
-    const double cs = cos(th), sn = sin(th);
-    double mx = 0;
-    for (int k = tid; k < nt; k += SV_THREADS) {
-      const int c0 = sm.clique[k], c1 = sm.clique[k + 1];
-      const double ax = sm.S[c1][0] - sm.S[c0][0], ay = sm.S[c1][1] - sm.S[c0][1], az = sm.S[c1][2] - sm.S[c0][2];
-      const double bx = sm.D[c1][0] - sm.D[c0][0], by = sm.D[c1][1] - sm.D[c0][1], bz = sm.D[c1][2] - sm.D[c0][2];
-      const double rx = bx - (cs * ax - sn * ay), ry = by - (sn * ax + cs * ay), rz = bz - az;
-      sm.res[k] = rx * rx + ry * ry + rz * rz;
-      mx = fmax(mx, sm.res[k]);
-    }
-    mx = block_max(sm, mx);
-    if (tid == 0) {
-      sm.R2[0] = cs; sm.R2[1] = -sn; sm.R2[2] = sn; sm.R2[3] = cs;
-      if (it == 0) {
-        sm.mu = 1.0 / (2.0 * mx / nb2 - 1.0);
-        if (sm.mu <= 0) sm.stop = 1;
-      }
-    }
-    __syncthreads();
-    if (sm.stop) break;
-    const double mu = sm.mu;
-    const double th1 = (mu + 1) / mu * nb2, th2 = mu / (mu + 1) * nb2;
-    double cost = 0;
-    for (int k = tid; k < nt; k += SV_THREADS) {
-      const double r = sm.res[k];
-      cost += sm.w[k] * r;
-      sm.w[k] = r >= th1 ? 0.0 : (r <= th2 ? 1.0 : sqrt(nb2 * mu * (mu + 1) / r) - mu);
-    }
-    cost = block_sum(sm, cost);
-    if (tid == 0) {
-      const double diff = fabs(cost - sm.prev_cost);
-      sm.mu = mu * prm.gnc_factor;
-      sm.prev_cost = cost;
-      if (diff < prm.cost_thr) sm.stop = 1;
-    }
-    __syncthreads();
-    if (sm.stop) break;
-  }
-  __syncthreads();
+  const int iters = gnc_tls_yaw<SV_THREADS>(&sm.S[0][0], &sm.D[0][0], sm.clique, m, sm.w, sm.res, sm.red, sm.gnc, prm);
   // translation: per-axis TLS adaptive voting over dst_i - R src_i on the clique members
   const double range = prm.noise_bound;
   int sn = 2;  // sort size: the power of two that holds the 2m interval ends (not always 2 * MAXC)
   while (sn < 2 * m) sn <<= 1;
   for (int d = 0; d < 3; d++) {
-    for (int k = tid; k < sn; k += SV_THREADS) {
-      sm.hval[k] = INFINITY;
-      sm.hidx[k] = 0;
-    }
-    __syncthreads();
-    for (int k = tid; k < m; k += SV_THREADS) {
-      const int c = sm.clique[k];
-      const double rs = d == 0 ? sm.R2[0] * sm.S[c][0] + sm.R2[1] * sm.S[c][1] : (d == 1 ? sm.R2[2] * sm.S[c][0] + sm.R2[3] * sm.S[c][1] : sm.S[c][2]);
-      const double x = sm.D[c][d] - rs;
-      sm.res[k] = x;
-      sm.hval[2 * k] = x - range; sm.hidx[2 * k] = k + 1;
-      sm.hval[2 * k + 1] = x + range; sm.hidx[2 * k + 1] = -k - 1;
-    }
-    __syncthreads();
-    // bitonic sort by (value, original slot) == std::stable_sort by value
-    for (int k = 2; k <= sn; k <<= 1)
-      for (int j = k >> 1; j > 0; j >>= 1) {
-        for (int i = tid; i < sn; i += SV_THREADS) {
-          const int l = i ^ j;
-          if (l > i) {
-            const double a = sm.hval[i], b = sm.hval[l];
-            const int ia = sm.hidx[i], ib = sm.hidx[l];
-            // slot order of the unsorted array: 2k for +, 2k+1 for -
-            const int sa = ia > 0 ? 2 * (ia - 1) : 2 * (-ia - 1) + 1, sb = ib > 0 ? 2 * (ib - 1) : 2 * (-ib - 1) + 1;
-            const bool gt = a > b || (a == b && (ia == 0 ? 1 << 30 : sa) > (ib == 0 ? 1 << 30 : sb));
-            const bool up = (i & k) == 0;
-            if (gt == up) {
-              sm.hval[i] = b; sm.hval[l] = a;
-              sm.hidx[i] = ib; sm.hidx[l] = ia;
-            }
-          }
-        }
-        __syncthreads();
-      }
+    tls_sorted_intervals<SV_THREADS>(&sm.S[0][0], &sm.D[0][0], sm.clique, m, sm.gnc.R2, d, range, sn, sm.res, sm.hval, sm.hidx);
     if (tid == 0) {
-      const double w = 1.0 / (range * range);
-      double ris = range * m, dxw = 0, dwc = 0, sxi = 0, sxq = 0, best_cost = INFINITY, best = 0;
-      int card = 0;
-      for (int i = 0; i < 2 * m; i++) {
-        const int idx = abs(sm.hidx[i]) - 1;
-        const int eps = sm.hidx[i] > 0 ? 1 : -1;
-        const double X = sm.res[idx];
-        card += eps;
-        dwc += eps * w;
-        dxw += eps * w * X;
-        ris -= eps * range;
-        sxi += eps * X;
-        sxq += eps * X * X;
-        const double xh = dxw / dwc;
-        const double cost = (card * xh * xh + sxq - 2 * sxi * xh) + ris;
-        if (cost < best_cost) {
-          best_cost = cost;
-          best = xh;
-        }
-      }
-      sm.t[d] = best;
+      TlsSweep sweep(range, m);
+      for (int i = 0; i < 2 * m; i++) sweep.add(sm.hidx[i] > 0 ? 1 : -1, sm.res[abs(sm.hidx[i]) - 1]);
+      sm.t[d] = sweep.best;
     }
     __syncthreads();
   }
-  if (tid == 0) {
-    P.T[0] = sm.R2[0]; P.T[1] = sm.R2[1]; P.T[2] = 0; P.T[3] = sm.t[0];
-    P.T[4] = sm.R2[2]; P.T[5] = sm.R2[3]; P.T[6] = 0; P.T[7] = sm.t[1];
-    P.T[8] = 0; P.T[9] = 0; P.T[10] = 1; P.T[11] = sm.t[2];
-    P.T[12] = 0; P.T[13] = 0; P.T[14] = 0; P.T[15] = 1;
-    P.counters[3] = 1;
-    P.counters[5] = iters;
-  }
+  if (tid == 0) write_result(P, sm.gnc.R2, sm.t, iters);
 }
 
 // ------------------------------------------------------------------------------------------------
-// Matcher::advancedMatching tail + the TEASER++ solve for correspondence sets beyond MAXC: the same algorithm as
-// k_teaser_solve, restated as a short chain of kernels over a global-memory workspace (BigSolveWs) so that a set of
-// several thousand correspondences (8 MB of adjacency bits) is spread over the whole GPU.
+// Matcher::advancedMatching tail + the TEASER++ solve for correspondence sets beyond MAXC: the stages of
+// k_teaser_solve (the helpers above) run as a short chain of kernels over a global-memory workspace (BigSolveWs) so that
+// a set of several thousand correspondences (8 MB of adjacency bits) is spread over the whole GPU.  The chain peels
+// cores level by level and grows its greedy cliques one warp per start.
 // ------------------------------------------------------------------------------------------------
 // every member of a passing triplet survives (matcher.cc:314-320); (src, dst) ordering, sort, unique (:338-355).
 // The cross-checked pairs are unique already, so "unique" is a no-op; the sort is a bitonic sort of packed keys.
@@ -1286,20 +1329,7 @@ __global__ void __launch_bounds__(1024) k_adv_select(const MatchDev* pairs, Quat
   while (n2 < total) n2 <<= 1;
   for (int i = total + threadIdx.x; i < n2; i += 1024) akeys[i] = 0xFFFFFFFFFFFFFFFFull;
   __syncthreads();
-  for (int k = 2; k <= n2; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = threadIdx.x; i < n2; i += 1024) {
-        const int l = i ^ j;
-        if (l > i) {
-          const unsigned long long a = akeys[i], b = akeys[l];
-          if ((a > b) == ((i & k) == 0)) {
-            akeys[i] = b;
-            akeys[l] = a;
-          }
-        }
-      }
-      __syncthreads();
-    }
+  block_bitonic<1024>(n2, KeyCmpSwap{akeys});
   for (int i = threadIdx.x; i < total; i += 1024) {
     P.out_corr[2 * i] = (int)(akeys[i] >> 32);
     P.out_corr[2 * i + 1] = (int)(akeys[i] & 0xFFFFFFFFull);
@@ -1379,12 +1409,7 @@ __global__ void __launch_bounds__(256) k_big_gather(const MatchDev* pairs) {
   const BigSolveWs& W = *P.big;
   const int n = P.counters[2];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < 16) P.T[i] = (i % 5 == 0) ? 1.0 : 0.0;
-  if (i == 0) {
-    P.counters[3] = 0;
-    P.counters[4] = 0;
-    P.counters[5] = 0;
-  }
+  reset_result(P, i);
   if (i >= n) return;
   const CloudDev& src = P.swapped ? P.fj : P.fi;
   const CloudDev& dst = P.swapped ? P.fi : P.fj;
@@ -1404,35 +1429,18 @@ __global__ void __launch_bounds__(256) k_big_tim(const MatchDev* pairs, QuatroPa
   const double beta = 2.0 * prm.noise_bound;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < (long long)n * wn; idx += (long long)gridDim.x * blockDim.x) {
     const int i = (int)(idx / wn), w = (int)(idx % wn);
-    const double sx = W.S[3 * i], sy = W.S[3 * i + 1], sz = W.S[3 * i + 2];
-    const double dx = W.D[3 * i], dy = W.D[3 * i + 1], dz = W.D[3 * i + 2];
+    const double si[3] = {W.S[3 * i], W.S[3 * i + 1], W.S[3 * i + 2]};
+    const double di[3] = {W.D[3 * i], W.D[3 * i + 1], W.D[3 * i + 2]};
     unsigned bits = 0;
     const int jend = min(32, n - w * 32);
     for (int b = 0; b < jend; b++) {
       const int j = w * 32 + b;
       if (j == i) continue;
-      double a = 0, c = 0, t;
-      t = W.S[3 * j] - sx; a += t * t;
-      t = W.S[3 * j + 1] - sy; a += t * t;
-      t = W.S[3 * j + 2] - sz; a += t * t;
-      t = W.D[3 * j] - dx; c += t * t;
-      t = W.D[3 * j + 1] - dy; c += t * t;
-      t = W.D[3 * j + 2] - dz; c += t * t;
-      if (fabs(sqrt(a) - sqrt(c)) <= beta) bits |= 1u << b;
+      if (tim_edge(si, di, W.S + 3 * j, W.D + 3 * j, beta)) bits |= 1u << b;
     }
     W.adj[(size_t)i * W.words + w] = bits;
     if (bits) atomicAdd(&W.deg[i], __popc(bits));
   }
-}
-
-__device__ __forceinline__ int block_min_i(int v, int* red) {
-  for (int o = 16; o > 0; o >>= 1) v = min(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();  // red may still be read from the previous call
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  int r = red[threadIdx.x & 31];
-  for (int o = 16; o > 0; o >>= 1) r = min(r, __shfl_xor_sync(0xffffffffu, r, o));
-  return r;
 }
 
 // core numbers by level-synchronous peeling (every vertex whose remaining degree is <= the current level leaves in
@@ -1457,7 +1465,7 @@ __global__ void __launch_bounds__(1024) k_big_core(const MatchDev* pairs) {
     int mn = 0x7FFFFFFF;
     for (int v = tid; v < n; v += 1024)
       if (W.alive[v]) mn = min(mn, W.pdeg[v]);
-    mn = block_min_i(mn, red);
+    mn = block_reduce<1024>(mn, red, [](int a, int b) { return min(a, b); }, 0x7FFFFFFF);
     k = max(k, mn);
     if (tid == 0) nf = 0;
     __syncthreads();
@@ -1489,20 +1497,7 @@ __global__ void __launch_bounds__(1024) k_big_core(const MatchDev* pairs) {
                       : 0xFFFFFFFFFFFFFFFFull;
   if (tid == 0) *W.best = 0;
   __syncthreads();
-  for (int kk = 2; kk <= n2; kk <<= 1)
-    for (int j = kk >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < n2; i += 1024) {
-        const int l = i ^ j;
-        if (l > i) {
-          const unsigned long long a = W.skey[i], b = W.skey[l];
-          if ((a > b) == ((i & kk) == 0)) {
-            W.skey[i] = b;
-            W.skey[l] = a;
-          }
-        }
-      }
-      __syncthreads();
-    }
+  block_bitonic<1024>(n2, KeyCmpSwap{W.skey});
   for (int r = tid; r < n; r += 1024) {
     const int v = (int)(W.skey[r] & 0xFFFFF);
     W.order[r] = v;
@@ -1633,25 +1628,6 @@ __global__ void __launch_bounds__(256) k_big_greedy_wide(const MatchDev* pairs) 
   }
 }
 
-__device__ __forceinline__ double block_sum_d(double v, double* red) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double r = red[threadIdx.x & 31];
-  for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
-  return r;
-}
-__device__ __forceinline__ double block_max_d(double v, double* red) {
-  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double r = red[threadIdx.x & 31];
-  for (int o = 16; o > 0; o >>= 1) r = fmax(r, __shfl_xor_sync(0xffffffffu, r, o));
-  return r;
-}
-
 // pick the largest clique (lowest rank on ties), list it, GNC-TLS yaw rotation, TLS translation.  One block per pair.
 __global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, QuatroParamsDev prm, int wide) {
   const MatchDev& P = pairs[blockIdx.x];
@@ -1662,19 +1638,15 @@ __global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, Quat
   const int tid = threadIdx.x;
   __shared__ double red[32];
   __shared__ unsigned long long kred[32];
-  __shared__ int stop;
-  __shared__ double s_mu, s_prev, s_R2[4], s_t[3];
+  __shared__ GncState gnc;
+  __shared__ double s_t[3];
   constexpr int SWEEP = 2048;
   __shared__ double cX[SWEEP];
   __shared__ int cE[SWEEP];
   {
     unsigned long long key = 0;
     for (int r = tid; r < n; r += 1024) key = max(key, clique_key(W.csize[r], r));
-    for (int o = 16; o > 0; o >>= 1) key = max(key, __shfl_xor_sync(0xffffffffu, key, o));
-    if ((tid & 31) == 0) kred[tid >> 5] = key;
-    __syncthreads();
-    key = kred[tid & 31];
-    for (int o = 16; o > 0; o >>= 1) key = max(key, __shfl_xor_sync(0xffffffffu, key, o));
+    key = block_reduce<1024>(key, kred, [](unsigned long long a, unsigned long long b) { return max(a, b); }, 0ull);
     const int br = (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull));
     for (int v = tid; v < n; v += 1024) W.alive[v] = 0;  // member flags
     __syncthreads();
@@ -1689,109 +1661,14 @@ __global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, Quat
       n, [&](int v) { return W.alive[v] != 0; }, [&](int pos, int v) { W.clique[pos] = v; });
   if (tid == 0) P.counters[4] = m;
   if (m <= 1) return;  // solution_.valid stays false
-  const int nt = m - 1;
-  double nb2 = prm.noise_bound * prm.noise_bound;
-  if (nb2 < 1e-16) nb2 = 1e-2;
-  for (int k = tid; k < nt; k += 1024) W.w[k] = 1.0;
-  if (tid == 0) {
-    s_mu = 1.0;
-    s_prev = INFINITY;
-    stop = 0;
-    s_R2[0] = 1; s_R2[1] = 0; s_R2[2] = 0; s_R2[3] = 1;
-  }
-  __syncthreads();
-  int iters = 0;
-  for (int it = 0; it < prm.max_iter; it++) {
-    iters = it + 1;
-    double h0 = 0, h1 = 0, h2 = 0, h3 = 0;
-    for (int k = tid; k < nt; k += 1024) {
-      const int c0 = W.clique[k], c1 = W.clique[k + 1];
-      const double ax = W.S[3 * c1] - W.S[3 * c0], ay = W.S[3 * c1 + 1] - W.S[3 * c0 + 1];
-      const double bx = W.D[3 * c1] - W.D[3 * c0], by = W.D[3 * c1 + 1] - W.D[3 * c0 + 1];
-      const double w = W.w[k];
-      h0 += ax * w * bx; h1 += ax * w * by; h2 += ay * w * bx; h3 += ay * w * by;
-    }
-    h0 = block_sum_d(h0, red); h1 = block_sum_d(h1, red); h2 = block_sum_d(h2, red); h3 = block_sum_d(h3, red);
-    const double th = atan2(h1 - h2, h0 + h3);
-    const double cs = cos(th), sn = sin(th);
-    double mx = 0;
-    for (int k = tid; k < nt; k += 1024) {
-      const int c0 = W.clique[k], c1 = W.clique[k + 1];
-      const double ax = W.S[3 * c1] - W.S[3 * c0], ay = W.S[3 * c1 + 1] - W.S[3 * c0 + 1], az = W.S[3 * c1 + 2] - W.S[3 * c0 + 2];
-      const double bx = W.D[3 * c1] - W.D[3 * c0], by = W.D[3 * c1 + 1] - W.D[3 * c0 + 1], bz = W.D[3 * c1 + 2] - W.D[3 * c0 + 2];
-      const double rx = bx - (cs * ax - sn * ay), ry = by - (sn * ax + cs * ay), rz = bz - az;
-      const double r = rx * rx + ry * ry + rz * rz;
-      W.res[k] = r;
-      mx = fmax(mx, r);
-    }
-    mx = block_max_d(mx, red);
-    if (tid == 0) {
-      s_R2[0] = cs; s_R2[1] = -sn; s_R2[2] = sn; s_R2[3] = cs;
-      if (it == 0) {
-        s_mu = 1.0 / (2.0 * mx / nb2 - 1.0);
-        if (s_mu <= 0) stop = 1;
-      }
-    }
-    __syncthreads();
-    if (stop) break;
-    const double mu = s_mu;
-    const double th1 = (mu + 1) / mu * nb2, th2 = mu / (mu + 1) * nb2;
-    double cost = 0;
-    for (int k = tid; k < nt; k += 1024) {
-      const double r = W.res[k];
-      cost += W.w[k] * r;
-      W.w[k] = r >= th1 ? 0.0 : (r <= th2 ? 1.0 : sqrt(nb2 * mu * (mu + 1) / r) - mu);
-    }
-    cost = block_sum_d(cost, red);
-    if (tid == 0) {
-      const double diff = fabs(cost - s_prev);
-      s_mu = mu * prm.gnc_factor;
-      s_prev = cost;
-      if (diff < prm.cost_thr) stop = 1;
-    }
-    __syncthreads();
-    if (stop) break;
-  }
-  __syncthreads();
+  const int iters = gnc_tls_yaw<1024>(W.S, W.D, W.clique, m, W.w, W.res, red, gnc, prm);
   const double range = prm.noise_bound;
   int n2 = 2;
   while (n2 < 2 * m) n2 <<= 1;
   for (int d = 0; d < 3; d++) {
-    for (int k = tid; k < n2; k += 1024) {
-      W.hval[k] = INFINITY;
-      W.hidx[k] = 0;
-    }
-    __syncthreads();
-    for (int k = tid; k < m; k += 1024) {
-      const int c = W.clique[k];
-      const double rs = d == 0 ? s_R2[0] * W.S[3 * c] + s_R2[1] * W.S[3 * c + 1] : (d == 1 ? s_R2[2] * W.S[3 * c] + s_R2[3] * W.S[3 * c + 1] : W.S[3 * c + 2]);
-      const double x = W.D[3 * c + d] - rs;
-      W.res[k] = x;
-      W.hval[2 * k] = x - range; W.hidx[2 * k] = k + 1;
-      W.hval[2 * k + 1] = x + range; W.hidx[2 * k + 1] = -k - 1;
-    }
-    __syncthreads();
-    for (int k = 2; k <= n2; k <<= 1)
-      for (int j = k >> 1; j > 0; j >>= 1) {
-        for (int i = tid; i < n2; i += 1024) {
-          const int l = i ^ j;
-          if (l > i) {
-            const double a = W.hval[i], b = W.hval[l];
-            const int ia = W.hidx[i], ib = W.hidx[l];
-            const int sa = ia > 0 ? 2 * (ia - 1) : 2 * (-ia - 1) + 1, sb = ib > 0 ? 2 * (ib - 1) : 2 * (-ib - 1) + 1;
-            const bool gt = a > b || (a == b && (ia == 0 ? 1 << 30 : sa) > (ib == 0 ? 1 << 30 : sb));
-            if (gt == ((i & k) == 0)) {
-              W.hval[i] = b; W.hval[l] = a;
-              W.hidx[i] = ib; W.hidx[l] = ia;
-            }
-          }
-        }
-        __syncthreads();
-      }
+    tls_sorted_intervals<1024>(W.S, W.D, W.clique, m, gnc.R2, d, range, n2, W.res, W.hval, W.hidx);
     // serial consensus sweep by one thread, fed from shared memory in chunks
-    const double w = 1.0 / (range * range);
-    double ris = range * m, dxw = 0, dwc = 0, sxi = 0, sxq = 0, best_cost = INFINITY, best = 0;
-    int card = 0;
+    TlsSweep sweep(range, m);
     for (int base = 0; base < 2 * m; base += SWEEP) {
       const int cnt = min(SWEEP, 2 * m - base);
       for (int i = tid; i < cnt; i += 1024) {
@@ -1801,35 +1678,13 @@ __global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, Quat
       }
       __syncthreads();
       if (tid == 0)
-        for (int i = 0; i < cnt; i++) {
-          const int eps = cE[i];
-          const double X = cX[i];
-          card += eps;
-          dwc += eps * w;
-          dxw += eps * w * X;
-          ris -= eps * range;
-          sxi += eps * X;
-          sxq += eps * X * X;
-          const double xh = dxw / dwc;
-          const double cost = (card * xh * xh + sxq - 2 * sxi * xh) + ris;
-          if (cost < best_cost) {
-            best_cost = cost;
-            best = xh;
-          }
-        }
+        for (int i = 0; i < cnt; i++) sweep.add(cE[i], cX[i]);
       __syncthreads();
     }
-    if (tid == 0) s_t[d] = best;
+    if (tid == 0) s_t[d] = sweep.best;
     __syncthreads();
   }
-  if (tid == 0) {
-    P.T[0] = s_R2[0]; P.T[1] = s_R2[1]; P.T[2] = 0; P.T[3] = s_t[0];
-    P.T[4] = s_R2[2]; P.T[5] = s_R2[3]; P.T[6] = 0; P.T[7] = s_t[1];
-    P.T[8] = 0; P.T[9] = 0; P.T[10] = 1; P.T[11] = s_t[2];
-    P.T[12] = 0; P.T[13] = 0; P.T[14] = 0; P.T[15] = 1;
-    P.counters[3] = 1;
-    P.counters[5] = iters;
-  }
+  if (tid == 0) write_result(P, gnc.R2, s_t, iters);
 }
 
 // coarse_aligned_ = transformPcd(src, T_quatro): double math, cast to float (utilities.hpp:164-175), ORIGINAL order,
