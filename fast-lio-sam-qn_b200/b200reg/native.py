@@ -97,6 +97,7 @@ EXPORTS = [
     "b200reg_comm_unique_id", "b200reg_comm_init", "b200reg_comm_destroy", "b200reg_comm_rank", "b200reg_comm_world",
     "b200reg_allgather_results", "b200reg_radius_search", "b200reg_quatro_align_ex", "b200reg_quatro_solve_tap",
     "b200reg_ctx_set_lm_trace", "b200reg_lm_trace", "b200reg_ctx_set_loop_clouds", "b200reg_loop_clouds",
+    "b200reg_match_tap",
 ]
 ESTATE = -4  # B200REG_ESTATE
 # B200REG_CLOUD_*: the loop clouds (Context.set_loop_clouds / Context.loop_clouds)
@@ -490,6 +491,26 @@ class Context:
                                               code, C.byref(prm), C.byref(info), clique.ctypes.data_as(C.c_void_p)))
         out = info.as_dict()
         out["clique"] = clique[:out["clique_size"]].copy()
+        return out
+
+    def match_tap(self, pairs, distance_threshold=35.0, advanced=False):
+        """The feature matcher alone on caller descriptors.  pairs: list of (fi (ni, 33), fj (nj, 33)) with nj <= ni, fi the
+        base of the forward search -> one dict per pair: nn (nj,) int32, dis (nj,) float32, rnn (ni,) int32 (-1 where no
+        reverse search ran), mutual (m, 2) int32 (i, j) pairs in ascending j (include/b200reg.h)."""
+        fs = [(np.ascontiguousarray(a, np.float32), np.ascontiguousarray(b, np.float32)) for a, b in pairs]
+        assert all(a.ndim == 2 and a.shape[1] == 33 and b.ndim == 2 and b.shape[1] == 33 for a, b in fs)
+        cnt = len(fs)
+        out = [dict(nn=np.empty(len(b), np.int32), dis=np.empty(len(b), np.float32), rnn=np.empty(len(a), np.int32),
+                    mutual=np.empty((len(b), 2), np.int32)) for a, b in fs]
+        ptrs = lambda arrs: (C.c_void_p * cnt)(*[x.ctypes.data for x in arrs])
+        nm = np.empty(cnt, np.int32)
+        _check(lib().b200reg_match_tap(self.h, cnt, ptrs([a for a, _ in fs]), (C.c_int32 * cnt)(*[len(a) for a, _ in fs]),
+                                       ptrs([b for _, b in fs]), (C.c_int32 * cnt)(*[len(b) for _, b in fs]),
+                                       C.c_double(distance_threshold), int(bool(advanced)), ptrs([o["nn"] for o in out]),
+                                       ptrs([o["dis"] for o in out]), ptrs([o["rnn"] for o in out]),
+                                       ptrs([o["mutual"] for o in out]), nm.ctypes.data_as(C.c_void_p)))
+        for o, m in zip(out, nm):
+            o["mutual"] = o["mutual"][:m].copy()
         return out
 
     def get_covariances(self, cloud):

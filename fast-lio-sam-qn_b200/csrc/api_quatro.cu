@@ -1,6 +1,7 @@
 // api_quatro.cu -- the C ABI of the Quatro path: FPFH descriptors, b200reg_quatro_align, coarse-to-fine and
 // b200reg_loop_closure.
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 
@@ -141,12 +142,20 @@ struct BigWsLayout {
   }
 };
 
+// squared feature distance gate of the matcher (dis > thr2 is dropped, matcher.cc:422,444).  advancedMatching searches
+// without a gate: FLT_MAX makes every finite distance qualify.  A square that overflows, or a NaN threshold, drops nothing
+// in the reference either: +inf.
+static float match_thr2(double distance_threshold, bool advanced) {
+  if (advanced) return 3.402823466e38f;
+  const float t2 = (float)distance_threshold * (float)distance_threshold;
+  return t2 <= 3.402823466e38f ? t2 : INFINITY;
+}
+
 static QuatroParamsDev quatro_params_dev(const b200reg_quatro_params* prm, bool advanced) {
   QuatroParamsDev q;
   q.normal_r2 = (float)(prm->fpfh_normal_radius * prm->fpfh_normal_radius);
   q.fpfh_r2 = (float)(prm->fpfh_radius * prm->fpfh_radius);
-  // advancedMatching searches without a distance gate: FLT_MAX makes every finite distance qualify
-  q.thr2 = advanced ? 3.402823466e38f : (float)prm->distance_threshold * (float)prm->distance_threshold;
+  q.thr2 = match_thr2(prm->distance_threshold, advanced);
   q.advanced = advanced ? 1 : 0;
   q.tuple_scale = (float)prm->tuple_scale;
   q.max_corres = prm->max_corres;
@@ -596,6 +605,107 @@ int b200reg_quatro_solve_tap(b200reg_ctx* c, int n, const float* src_xyz, const 
   info->clique_size = got[4];
   info->gnc_iterations = got[5];
   info->reserved = 0;
+  return B200REG_OK;
+}
+
+int b200reg_match_tap(b200reg_ctx* c, int count, const float* const* fi, const int32_t* ni, const float* const* fj, const int32_t* nj,
+                      double distance_threshold, int advanced, int32_t* const* nn_out, float* const* dis_out, int32_t* const* rnn_out,
+                      int32_t* const* mutual_out, int32_t* n_mutual_out) {
+  if (!c || count <= 0 || !fi || !ni || !fj || !nj || !nn_out || !dis_out || !rnn_out || !mutual_out || !n_mutual_out)
+    return fail(B200REG_EINVAL, "bad argument");
+  for (int k = 0; k < count; k++) {
+    if (!fi[k] || !fj[k] || !nn_out[k] || !dis_out[k] || !rnn_out[k] || !mutual_out[k] || ni[k] < 1 || nj[k] < 1)
+      return fail(B200REG_EINVAL, "bad argument");
+    if (nj[k] > ni[k]) return fail(B200REG_EINVAL, "nj > ni: fi is the base of the forward search and must be the larger set");
+  }
+  CU(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  Scratch scratch(c);
+  // cloud 2k = fi of pair k, 2k + 1 = its fj: the record tables b200reg_clouds_fpfh keeps, and the sort's temporaries
+  std::vector<CloudDev> cl(2 * (size_t)count);
+  std::vector<MatchDev> pairs(count);
+  Layout l;
+  std::vector<size_t> o_c(2 * (size_t)count), o_p(count);
+  auto cloud_bytes = [](size_t n) {
+    Layout x;
+    for (size_t b : {n * FPAD * 4, n * 16, n * FPAD * 4, n * 16, 2 * ((n + 63) / 64) * 16, n * 4, n * 4, n * 4, n * 4, n * 4})
+      x.take(b);
+    x.take(radix_sort_ws_bytes((int)n, 32));
+    return x.size;
+  };
+  int max_n = 0, max_ni = 0, max_nj = 0;
+  for (int k = 0; k < count; k++) {
+    o_c[2 * k] = l.take(cloud_bytes(ni[k]));
+    o_c[2 * k + 1] = l.take(cloud_bytes(nj[k]));
+    o_p[k] = l.take(((size_t)nj[k] * 5 + (size_t)ni[k] * 2) * 4 + 32 + 64 + 256);
+    max_ni = std::max(max_ni, (int)ni[k]);
+    max_nj = std::max(max_nj, (int)nj[k]);
+  }
+  max_n = max_ni;
+  char* slab = nullptr;
+  CU(scratch.alloc((void**)&slab, l.size));
+  for (int q = 0; q < 2 * count; q++) {
+    const size_t n = q & 1 ? nj[q / 2] : ni[q / 2];
+    CloudDev& d = cl[q];
+    char* b = slab + o_c[q];
+    Layout x;
+    d.n = (int)n;
+    d.fpfh = (float*)(b + x.take(n * FPAD * 4));
+    d.fproj = (float4*)(b + x.take(n * 16));
+    d.fpfh_s = (float*)(b + x.take(n * FPAD * 4));
+    d.fproj_s = (float4*)(b + x.take(n * 16));
+    d.ftile = (float4*)(b + x.take(2 * ((n + 63) / 64) * 16));
+    d.fcode_s = (uint32_t*)(b + x.take(n * 4));
+    d.keys[0] = (uint32_t*)(b + x.take(n * 4));
+    d.keys[1] = (uint32_t*)(b + x.take(n * 4));
+    d.vals[0] = (uint32_t*)(b + x.take(n * 4));
+    d.vals[1] = (uint32_t*)(b + x.take(n * 4));
+    const size_t ws = radix_sort_ws_bytes((int)n, 32);
+    d.hist = (uint32_t*)(b + x.take(ws));
+    CU(cudaMemsetAsync(d.hist, 0, ws, s));
+    // the caller's rows into slots 0..32 of the record table; k_load_records completes the records in place
+    CU(cudaMemcpy2DAsync(d.fpfh, FPAD * 4, q & 1 ? fj[q / 2] : fi[q / 2], FDIM * 4, FDIM * 4, n, cudaMemcpyHostToDevice, s));
+  }
+  for (int k = 0; k < count; k++) {
+    MatchDev& m = pairs[k];
+    m.fi = cl[2 * k];
+    m.fj = cl[2 * k + 1];
+    const size_t a = ni[k], b = nj[k];
+    char* p = slab + o_p[k];
+    m.nn = (int*)p;
+    m.dis = (float*)(p + b * 4);
+    m.corres = (int*)(p + b * 8);
+    m.tkey = (unsigned*)(p + b * 16);
+    m.first_j = (int*)(p + b * 20);
+    m.rnn = (int*)(p + b * 20 + a * 4);
+    m.counters = (int*)(p + b * 20 + a * 8);
+    m.stats = (double*)(p + (b * 20 + a * 8 + 32 + 63) / 64 * 64);
+  }
+  CloudDev* d_cl = nullptr;
+  MatchDev* d_pairs = nullptr;
+  CU(scratch.upload(&d_cl, cl.data(), sizeof(CloudDev) * cl.size()));
+  CU(scratch.upload(&d_pairs, pairs.data(), sizeof(MatchDev) * count));
+  {
+    ProfScope ps(c, CLS_MATCH);
+    c->launches += launch_load_records(d_cl, 2 * count, max_n, s);
+    c->launches += launch_feature_order(d_cl, 2 * count, max_n, s);
+    c->launches += launch_feature_match(d_pairs, count, max_ni, max_nj, match_thr2(distance_threshold, !!advanced), advanced ? 1 : 0, s);
+  }
+  CU(cudaGetLastError());
+  std::vector<int> counters(8 * (size_t)count);
+  for (int k = 0; k < count; k++) {
+    CU(cudaMemcpyAsync(nn_out[k], pairs[k].nn, (size_t)nj[k] * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(dis_out[k], pairs[k].dis, (size_t)nj[k] * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(rnn_out[k], pairs[k].rnn, (size_t)ni[k] * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&counters[8 * k], pairs[k].counters, 32, cudaMemcpyDeviceToHost, s));
+  }
+  CU(cudaStreamSynchronize(s));
+  for (int k = 0; k < count; k++) {
+    n_mutual_out[k] = counters[8 * k + 1];
+    if (n_mutual_out[k] > 0)
+      CU(cudaMemcpyAsync(mutual_out[k], pairs[k].corres, (size_t)n_mutual_out[k] * 8, cudaMemcpyDeviceToHost, s));
+  }
+  CU(cudaStreamSynchronize(s));
   return B200REG_OK;
 }
 

@@ -30,6 +30,13 @@ void launch_transform_out(const CloudDev& c, const float* d_Tf, float* d_out3, c
 // quatro.cu
 cudaError_t quatro_init_device();
 int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2, float fpfh_r2, cudaStream_t s);
+// the stages of launch_fpfh and launch_quatro_match_solve that b200reg_match_tap runs on caller descriptors:
+//   launch_load_records   rows of 33 bins in c.fpfh (stride FPAD) -> records, original index = row (the k_fpfh tail)
+//   launch_feature_order  k_fcode, radix sort, k_fgather (keys / vals / hist as for launch_radix_sort)
+//   launch_feature_match  k_match_init, k_feat_nn both ways, k_first_hit, k_mutual
+int launch_load_records(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s);
+int launch_feature_order(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s);
+int launch_feature_match(const MatchDev* d_pairs, int count, int max_ni, int max_nj, float thr2, int advanced, cudaStream_t s);
 // optimizedMatching: k_teaser_solve solves the sets of at most MAXC and leaves larger ones (counters[2] > MAXC) to
 // launch_big_solve
 int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, int max_nj, const QuatroParamsDev& prm, cudaStream_t s);

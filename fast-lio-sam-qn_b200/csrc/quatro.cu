@@ -144,6 +144,41 @@ __global__ void __launch_bounds__(STEP_THREADS) k_spfh(const CloudDev* clouds, f
   out[33] = 0.f; out[34] = 0.f; out[35] = 0.f;
 }
 
+// The one writer of a descriptor record (k_fpfh, and k_load_records for the matcher tap): bins in slots 0..32, original
+// index (int bits) in slot 33, usable flag in slot 34 (some bin != 0), hash of the bins' bits in slot 35; plus the
+// matcher's filter coordinates (fpfh_basis.cuh): projections on three fixed orthonormal directions and the norm of the
+// residual, computed from the residual VECTOR (no cancellation of large sums)
+__device__ __forceinline__ void write_record(float* out, float4* fproj, const float (&v)[FDIM], float orig_bits) {
+  bool any = false;
+#pragma unroll
+  for (int k = 0; k < FDIM; k++) {
+    out[k] = v[k];
+    any |= (v[k] != 0.f);
+  }
+  out[33] = orig_bits;
+  out[34] = any ? 1.f : 0.f;
+  float x[FDIM];
+  float c0 = 0.f, c1 = 0.f, c2 = 0.f;
+  uint32_t hsh = 0x811C9DC5u;
+#pragma unroll
+  for (int k = 0; k < FDIM; k++) {
+    hsh = (hsh ^ __float_as_uint(v[k])) * 0x01000193u;
+    hsh ^= hsh >> 15;
+    x[k] = v[k] - FB_MU[k];
+    c0 += x[k] * FB_U[0][k];
+    c1 += x[k] * FB_U[1][k];
+    c2 += x[k] * FB_U[2][k];
+  }
+  float rr = 0.f;
+#pragma unroll
+  for (int k = 0; k < FDIM; k++) {
+    const float e = x[k] - ((c0 * FB_U[0][k] + c1 * FB_U[1][k]) + c2 * FB_U[2][k]);
+    rr += e * e;
+  }
+  out[35] = __uint_as_float(hsh);
+  *fproj = make_float4(c0, c1, c2, sqrtf(rr));
+}
+
 // ------------------------------------------------------------------------------------------------
 // Q3 FPFH: sum SPFH(q)/d2 over the neighbours, each 11-bin block rescaled to 100
 // ------------------------------------------------------------------------------------------------
@@ -182,39 +217,22 @@ __global__ void __launch_bounds__(STEP_THREADS) k_fpfh(const CloudDev* clouds, f
     s2 += h[22 + k];
   }
   const float sc0 = s0 != 0.f ? 100.0f / s0 : 0.f, sc1 = s1 != 0.f ? 100.0f / s1 : 0.f, sc2 = s2 != 0.f ? 100.0f / s2 : 0.f;
-  float* out = c.fpfh + (size_t)i * FPAD;
-  bool any = false;
+  float v[FDIM];
 #pragma unroll
-  for (int k = 0; k < FDIM; k++) {
-    const float v = h[k] * (k < 11 ? sc0 : (k < 22 ? sc1 : sc2));
-    out[k] = v;
-    any |= (v != 0.f);
-  }
-  out[33] = p.w;  // original index (int bits)
-  out[34] = any ? 1.f : 0.f;
-  // the matcher's filter coordinates (fpfh_basis.cuh): projections on three fixed orthonormal directions and the norm of
-  // the residual, computed from the residual VECTOR (no cancellation of large sums); plus a hash of the record's bits
-  float x[FDIM];
-  float c0 = 0.f, c1 = 0.f, c2 = 0.f;
-  uint32_t hsh = 0x811C9DC5u;
+  for (int k = 0; k < FDIM; k++) v[k] = h[k] * (k < 11 ? sc0 : (k < 22 ? sc1 : sc2));
+  write_record(c.fpfh + (size_t)i * FPAD, &c.fproj[i], v, p.w);  // p.w: original index (int bits)
+}
+
+// caller descriptors (b200reg_match_tap): row i of c.fpfh holds 33 bins (stride FPAD) and becomes record i, original index i
+__global__ void __launch_bounds__(256) k_load_records(const CloudDev* clouds) {
+  const CloudDev& c = clouds[blockIdx.y];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c.n) return;
+  float* row = c.fpfh + (size_t)i * FPAD;
+  float v[FDIM];
 #pragma unroll
-  for (int k = 0; k < FDIM; k++) {
-    const float v = h[k] * (k < 11 ? sc0 : (k < 22 ? sc1 : sc2));
-    hsh = (hsh ^ __float_as_uint(v)) * 0x01000193u;
-    hsh ^= hsh >> 15;
-    x[k] = v - FB_MU[k];
-    c0 += x[k] * FB_U[0][k];
-    c1 += x[k] * FB_U[1][k];
-    c2 += x[k] * FB_U[2][k];
-  }
-  float rr = 0.f;
-#pragma unroll
-  for (int k = 0; k < FDIM; k++) {
-    const float e = x[k] - ((c0 * FB_U[0][k] + c1 * FB_U[1][k]) + c2 * FB_U[2][k]);
-    rr += e * e;
-  }
-  out[35] = __uint_as_float(hsh);
-  c.fproj[i] = make_float4(c0, c1, c2, sqrtf(rr));
+  for (int k = 0; k < FDIM; k++) v[k] = row[k];
+  write_record(row, &c.fproj[i], v, __int_as_float(i));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -371,11 +389,19 @@ __device__ __forceinline__ float tile_lb(const float4& q, const float4& lo, cons
   return __fmaf_rn(e3, e3, __fmaf_rn(e2, e2, __fmaf_rn(e1, e1, e0 * e0)));
 }
 // acceptance threshold of the filter for a query whose best squared distance so far is `best`.  The filter value is a
-// true lower bound of the distance up to fp32 rounding of the coordinates (worst case 2.4e-3 in distance for |a - mu| <=
-// 173, measured 7e-5: profiles/emulate_projected_bound_margin.py) and of the refine's sum (4e-6 relative).
+// true lower bound of the distance up to fp32 rounding of the coordinates and of the refine's sum (4e-6 relative).  Over
+// the whole descriptor domain (three blocks >= 0 summing to 100) |a - mu| <= 220.5 (one-hot blocks where mu is least),
+// and with r taken from the residual vector as write_record does, the derived worst case of that rounding is 2.9e-3 in
+// distance (tests/match_ref.py: derived_excess), inside the 4e-3.  On crafted pairs where the bound is tight (parallel
+// residuals, one-hot anchors at 220.5) sqrt(filt_lb) comes within 6e-6 of the fp32 distance, never above it.
 __device__ __forceinline__ float filt_bound(float best) {
   const float sb = sqrtf(best) * 1.00001f + 4e-3f;
   return sb * sb;
+}
+// the search keeps d2 < gate_lim(thr2), i.e. d2 <= thr2 (matcher.cc:422,444 drop dis > thr2).  thr2 = +inf (a threshold
+// whose square overflows) keeps every pair, as the reference does; nextafter of +inf would be a NaN that keeps none.
+__device__ __forceinline__ float gate_lim(float thr2) {
+  return thr2 < INFINITY ? __int_as_float(__float_as_int(thr2) + 1) : INFINITY;  // nextafter(thr2, +inf)
 }
 
 // Exact 33-D 1-NN by filter-and-refine over filter-ordered tiles.
@@ -411,7 +437,7 @@ __global__ void __launch_bounds__(NN_THREADS) k_feat_nn(const MatchDev* pairs, i
   __shared__ unsigned s_need[3];  // block-level need masks of the current / next chunks of tile visits
   __shared__ int s_t0;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const float lim = __int_as_float(__float_as_int(thr2) + 1);  // nextafter(thr2, +inf): d2 == thr2 still qualifies
+  const float lim = gate_lim(thr2);
   // stage this thread's query (row `lane` of its warp)
   const int qi = q0 + threadIdx.x;
   int qorig = -1;
@@ -1706,11 +1732,20 @@ int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2,
   k_normals<<<grid, STEP_THREADS, 0, s>>>(d_clouds, normal_r2);
   k_spfh<<<grid, STEP_THREADS, 0, s>>>(d_clouds, fpfh_r2);
   k_fpfh<<<grid, STEP_THREADS, 0, s>>>(d_clouds, fpfh_r2);
-  // the matcher's view: records in the order of their filter-space Morton code, duplicates collapsed, boxed per tile
+  return 3 + launch_feature_order(d_clouds, count, max_n, s);
+}
+
+// the matcher's view: records in the order of their filter-space Morton code, duplicates collapsed, boxed per tile
+int launch_feature_order(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s) {
   k_fcode<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_clouds);
   const int ls = launch_radix_sort(d_clouds, count, max_n, 32, s);  // 32-bit keys, 3 passes of 11 bits: result in keys[1] / vals[1]
   k_fgather<<<dim3((max_n + NN_TILE - 1) / NN_TILE, count), NN_TILE, 0, s>>>(d_clouds);
-  return 5 + ls;
+  return 2 + ls;
+}
+
+int launch_load_records(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s) {
+  k_load_records<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_clouds);
+  return 1;
 }
 
 size_t solve_smem_bytes() { return sizeof(SolveSmem); }
@@ -1734,15 +1769,22 @@ int launch_teaser_solve(const MatchDev* d_pairs, int count, const QuatroParamsDe
   return 1;
 }
 
-int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, int max_nj, const QuatroParamsDev& prm, cudaStream_t s) {
+// the feature matcher up to the mutual list (nn, dis, first_j, rnn, corres, counters[1]); also zeroes counters and stats
+int launch_feature_match(const MatchDev* d_pairs, int count, int max_ni, int max_nj, float thr2, int advanced, cudaStream_t s) {
   int l = 0;
   k_match_init<<<dim3((max_ni + 255) / 256, count), 256, 0, s>>>(d_pairs); l++;
+  k_feat_nn<<<dim3((max_nj + NN_THREADS - 1) / NN_THREADS, count), NN_THREADS, 0, s>>>(d_pairs, 0, thr2); l++;
+  k_first_hit<<<dim3((max_nj + 255) / 256, count), 256, 0, s>>>(d_pairs, thr2); l++;
+  k_feat_nn<<<dim3((max_ni + NN_THREADS - 1) / NN_THREADS, count), NN_THREADS, 0, s>>>(d_pairs, 1, thr2); l++;
+  k_mutual<<<count, 1024, 0, s>>>(d_pairs, thr2, advanced); l++;
+  return l;
+}
+
+int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, int max_nj, const QuatroParamsDev& prm, cudaStream_t s) {
+  int l = launch_feature_match(d_pairs, count, max_ni, max_nj, prm.thr2, prm.advanced, s);
+  // normalizePoints: reads the points only and writes stats[0..6], which no kernel of the matcher reads
   k_cloud_sum<<<dim3(1, count, 2), 1024, 0, s>>>(d_pairs); l++;
   k_cloud_scale<<<dim3(64, count, 2), 256, 0, s>>>(d_pairs); l++;
-  k_feat_nn<<<dim3((max_nj + NN_THREADS - 1) / NN_THREADS, count), NN_THREADS, 0, s>>>(d_pairs, 0, prm.thr2); l++;
-  k_first_hit<<<dim3((max_nj + 255) / 256, count), 256, 0, s>>>(d_pairs, prm.thr2); l++;
-  k_feat_nn<<<dim3((max_ni + NN_THREADS - 1) / NN_THREADS, count), NN_THREADS, 0, s>>>(d_pairs, 1, prm.thr2); l++;
-  k_mutual<<<count, 1024, 0, s>>>(d_pairs, prm.thr2, prm.advanced); l++;
   k_tuple_trials<<<dim3(128, count), 256, 0, s>>>(d_pairs, prm); l++;
   if (!prm.advanced) {
     k_tuple_select<<<count, 1024, (size_t)tuple_sort_len(prm.max_corres) * 8, s>>>(d_pairs, prm); l++;

@@ -460,6 +460,21 @@ int b200reg_radius_search(b200reg_ctx* ctx, const b200reg_cloud* cloud, const fl
  * indices, ascending.                                                                                           */
 int b200reg_quatro_solve_tap(b200reg_ctx* ctx, int n, const float* src_xyz, const float* dst_xyz, int wide,
                              const b200reg_quatro_params* params, b200reg_quatro_info* info, int32_t* clique_out);
+/* The feature matcher of b200reg_quatro_align alone, on caller descriptors: for each of `count` pairs, fi[k] (ni[k] x 33
+ * host floats) and fj[k] (nj[k] x 33), in the matcher's roles (fi the base of the forward search: 1 <= nj[k] <= ni[k],
+ * otherwise B200REG_EINVAL; b200reg_quatro_align swaps its clouds to get there).  An all-zero row is unusable: never a
+ * neighbour, never matched.  Distances are fp32 ((e0*e0 + e1*e1) + ...) + e32*e32 without FMA, ties go to the lower row.
+ *   nn_out[k]      nj[k]: row of fi nearest to row j of fj, -1 when it is unusable or no usable row lies within the gate
+ *                  d2 <= fp32(distance_threshold)^2 (no gate when advanced != 0, or when that square overflows or is NaN)
+ *   dis_out[k]     nj[k]: its squared distance (meaningful where nn >= 0)
+ *   rnn_out[k]     ni[k]: row of fj nearest to row i of fi where the reverse search ran (optimizedMatching: i is the nn of
+ *                  some j within the gate; advancedMatching: of any j), -1 elsewhere
+ *   mutual_out[k]  up to nj[k] (i, j) pairs, ascending j: optimizedMatching keeps (i, j) when j is the lowest j whose nn
+ *                  is i and rnn(i) == j; advancedMatching when nn(j) = i and rnn(i) == j
+ *   n_mutual_out   count: the length of each mutual list (b200reg_quatro_info::n_mutual)                       */
+int b200reg_match_tap(b200reg_ctx* ctx, int count, const float* const* fi, const int32_t* ni, const float* const* fj,
+                      const int32_t* nj, double distance_threshold, int advanced, int32_t* const* nn_out,
+                      float* const* dis_out, int32_t* const* rnn_out, int32_t* const* mutual_out, int32_t* n_mutual_out);
 /* normals (n x 3, NaN where fewer than 3 neighbours) and FPFH (n x 33), original point order.            */
 int b200reg_get_fpfh(b200reg_ctx* ctx, const b200reg_cloud* cloud, float* normals_out, float* fpfh_out);
 /* n x 9 doubles (row-major 3x3 block of the reference's Matrix4d), original point order.          */
