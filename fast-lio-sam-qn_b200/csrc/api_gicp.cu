@@ -120,7 +120,7 @@ static int lm_arena_ensure(b200reg_ctx* c, int count) {
   }
   if (!a.graph.exec) {
     const int blocks = c->sm_count * LM_BLOCKS_PER_SM;
-    const cudaError_t e = lm_graph_build(&a.graph, a.d_pairs, a.d_states, a.d_guess, a.d_call, a.d_sched, blocks, blocks);
+    const cudaError_t e = lm_graph_build(&a.graph, a.d_pairs, a.d_states, a.d_guess, a.d_call, a.d_sched, blocks, blocks, lm_slot_cache(a.cap));
     if (e != cudaSuccess) return fail(B200REG_ECUDA, std::string("building the LM graph: ") + cudaGetErrorString(e));
   }
   return B200REG_OK;
@@ -133,12 +133,12 @@ static void lm_step(b200reg_ctx* c) {
   const int blocks = c->sm_count * LM_BLOCKS_PER_SM;
   {
     ProfScope ps(c, CLS_SEARCH);
-    launch_gicp_search(A.d_pairs, A.d_states, blocks, A.d_call, A.d_sched, c->stream);
+    launch_gicp_search(A.d_pairs, A.d_states, blocks, A.d_call, A.d_sched, lm_slot_cache(A.cap), c->stream);
     c->launches++;
   }
   {
     ProfScope ps(c, CLS_ACCUM);
-    launch_gicp_accum(A.d_pairs, A.d_states, blocks, A.d_sched, c->stream);
+    launch_gicp_accum(A.d_pairs, A.d_states, blocks, A.d_sched, lm_slot_cache(A.cap), c->stream);
     c->launches++;
   }
   {

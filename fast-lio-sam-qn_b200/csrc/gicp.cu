@@ -321,8 +321,13 @@ __device__ __forceinline__ void cov_knn(const CloudDev& c, int i, float4 q, Heap
     }
   }
   res.heapify();
-  knn_walk<Heap>(c, q.x, q.y, q.z, res, lo, hi);
+  knn_walk(c, q.x, q.y, q.z, res, nullptr, lo, hi);  // stack in local memory: on chip it ran slower on H100 (DESIGN.md §3)
 }
+
+// On-chip traversal stack depth of k_gicp_search (knn_walk, knn.cuh).  From profiles/emulate_stack_depth.py on the bench's
+// first pair (DESIGN.md §3): the seeded 1-NN walks stay within 6 entries for 99.8 % of their pushes (the one unseeded pass
+// per pair goes 18 deep and spills the rest to local memory).
+constexpr int SEARCH_STACK = 6;
 
 // K is the CAPACITY of the result set; k <= K neighbours enter the covariance (the k nearest of the K nearest are the
 // k nearest), so every k in 1..32 is served by the next instantiated capacity.  k > 32 runs k_covariance_large
@@ -393,30 +398,35 @@ __global__ void __launch_bounds__(STEP_THREADS, (K <= 16 ? 10 : 4)) k_covariance
 //                  App. A.6) and runs the LM controller; the last block of the STEP rebuilds the schedule from the pairs'
 //                  new phases -- no host round trip per iteration, finished pairs cost nothing from the next step on.
 // ---------------------------------------------------------------------------------------
-// The step's slot list in shared memory (first LM_SMEM_SLOTS entries; beyond that straight from global memory).
+// The step's slot list in shared memory: the first n_cached entries (dynamic shared memory of lm_slot_cache(arena
+// capacity) entries, sized where the kernels are launched), beyond that straight from global memory.  A context that runs
+// 16-pair jobs (arena of 24 pairs) caches 384 B instead of reserving LM_SMEM_SLOTS (8 KB) per block: the rest of the
+// SM's L1 / shared memory stays L1.
 struct SlotView {
   const LmSlot* g;
   const LmSlot* sh;
-  __device__ __forceinline__ LmSlot get(int k) const { return k < LM_SMEM_SLOTS ? sh[k] : g[k]; }
+  int n_cached;
+  __device__ __forceinline__ LmSlot get(int k) const { return k < n_cached ? sh[k] : g[k]; }
 };
-__device__ __forceinline__ void load_slots(const LmSched* sched, int n_active, LmSlot* sh) {
+__device__ __forceinline__ void load_slots(const LmSched* sched, int n_active, int n_cached, LmSlot* sh) {
   const int4* src = reinterpret_cast<const int4*>(sched->slots);
   int4* dst = reinterpret_cast<int4*>(sh);
-  for (int k = threadIdx.x; k < min(n_active, LM_SMEM_SLOTS); k += blockDim.x) dst[k] = __ldcg(&src[k]);
+  for (int k = threadIdx.x; k < min(n_active, n_cached); k += blockDim.x) dst[k] = __ldcg(&src[k]);
   __syncthreads();
 }
 
 __global__ void __launch_bounds__(STEP_THREADS, 16) k_gicp_search(const PairDev* pairs, const PairState* states, const LmCall* call,
-                                                                const LmSched* sched) {
+                                                                const LmSched* sched, int n_cached) {
   __shared__ float s_Tf[12];
-  __shared__ __align__(16) LmSlot s_slots[LM_SMEM_SLOTS];
+  __shared__ int2 s_stack[SEARCH_STACK][STEP_THREADS];
+  extern __shared__ __align__(16) LmSlot s_slots[];  // [n_cached]
   const double max_corr_dist2 = call->prm.max_corr_dist2;
   const int total_items = sched->total_items;
   const int n_active = sched->n_active;
   const int stride = sched->stride;
   if ((int)blockIdx.x >= total_items) return;
-  load_slots(sched, n_active, s_slots);
-  const SlotView slots{sched->slots, s_slots};
+  load_slots(sched, n_active, n_cached, s_slots);
+  const SlotView slots{sched->slots, s_slots, n_cached};
   for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
     const int slot = item / stride, blk = item - slot * stride;
     const LmSlot sl = slots.get(slot);
@@ -455,7 +465,7 @@ __global__ void __launch_bounds__(STEP_THREADS, 16) k_gicp_search(const PairDev*
         res.p[0] = pp;
       }
     }
-    knn_walk(P.tgt, qx, qy, qz, res);
+    knn_walk<SEARCH_STACK, STEP_THREADS>(P.tgt, qx, qy, qz, res, &s_stack[0][threadIdx.x]);
     P.sqd[i] = res.d[0];
     if (phase == PH_LINEARIZE) P.corr[i] = ((double)res.d[0] < max_corr_dist2) ? res.p[0] : -1;
   }
@@ -466,14 +476,18 @@ __global__ void __launch_bounds__(STEP_THREADS, 16) k_gicp_search(const PairDev*
 // kernel sums the rows in a fixed order.  (Round 1 and the first version of this round reduced per block and let the
 // last-arriving block of a pair run the controller: four __syncthreads, a __threadfence and an atomic round trip per item
 // made the streaming phases barrier- and latency-bound, ncu: barrier 7.9 / long-scoreboard 17 stalled warps per issue.)
-__global__ void __launch_bounds__(STEP_THREADS, 8) k_gicp_accum(const PairDev* pairs, const PairState* states, const LmSched* sched) {
-  __shared__ __align__(16) LmSlot s_slots[LM_SMEM_SLOTS];
+// 4 blocks per SM (up to 128 registers): the linearize pass holds the 28 fp64 values plus the inputs of M, J and e and
+// needs 116 registers.  Under the 64-register cap of 8 blocks per SM it spilled 324 B per thread, more than the pass's
+// own loads, and ran 1.7x longer (DESIGN.md §3); 6 blocks (80 registers) still spill 84 B.
+__global__ void __launch_bounds__(STEP_THREADS, 4) k_gicp_accum(const PairDev* pairs, const PairState* states, const LmSched* sched,
+                                                               int n_cached) {
+  extern __shared__ __align__(16) LmSlot s_slots[];  // [n_cached]
   const int total_items = sched->total_items;
   const int n_active = sched->n_active;
   const int stride = sched->stride;
   if ((int)blockIdx.x >= total_items) return;
-  load_slots(sched, n_active, s_slots);
-  const SlotView slots{sched->slots, s_slots};
+  load_slots(sched, n_active, n_cached, s_slots);
+  const SlotView slots{sched->slots, s_slots, n_cached};
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
     const int slot = item / stride, blk = item - slot * stride;
@@ -653,7 +667,7 @@ __global__ void __launch_bounds__(STEP_THREADS) k_knn_queries(CloudDev c, const 
   const float* qq = q + (size_t)i * qstride;
   KnnSet<K> res;
   res.init();
-  knn_walk(c, qq[0], qq[1], qq[2], res);
+  knn_walk(c, qq[0], qq[1], qq[2], res);  // a debug tap: the stack stays in local memory
 #pragma unroll
   for (int j = 0; j < K; j++) {
     if (j < kout) {
@@ -769,11 +783,12 @@ void launch_gicp_init(const PairDev* pairs, PairState* states, const double* d_g
 // One LM step over every still-active pair = search + accumulate + controller.  blocks_*: persistent grid sizes (work
 // items are strided over them); the kernels are correct for any value >= 1.
 constexpr int CTRL_BLOCKS = 64;
-void launch_gicp_search(const PairDev* pairs, const PairState* states, int blocks, const LmCall* call, const LmSched* sched, cudaStream_t s) {
-  k_gicp_search<<<blocks, STEP_THREADS, 0, s>>>(pairs, states, call, sched);
+void launch_gicp_search(const PairDev* pairs, const PairState* states, int blocks, const LmCall* call, const LmSched* sched, int n_cached,
+                        cudaStream_t s) {
+  k_gicp_search<<<blocks, STEP_THREADS, sizeof(LmSlot) * n_cached, s>>>(pairs, states, call, sched, n_cached);
 }
-void launch_gicp_accum(const PairDev* pairs, const PairState* states, int blocks, const LmSched* sched, cudaStream_t s) {
-  k_gicp_accum<<<blocks, STEP_THREADS, 0, s>>>(pairs, states, sched);
+void launch_gicp_accum(const PairDev* pairs, const PairState* states, int blocks, const LmSched* sched, int n_cached, cudaStream_t s) {
+  k_gicp_accum<<<blocks, STEP_THREADS, sizeof(LmSlot) * n_cached, s>>>(pairs, states, sched, n_cached);
 }
 void launch_gicp_control(const PairDev* pairs, PairState* states, LmCall* call, LmSched* sched, cudaStream_t s) {
   k_gicp_control<<<CTRL_BLOCKS, CTRL_THREADS, 0, s>>>(pairs, states, call, sched);
@@ -785,7 +800,7 @@ void launch_gicp_control(const PairDev* pairs, PairState* states, LmCall* call, 
 // All kernel arguments are pointers into the context's persistent LM arena, so the executable graph is reused by every call
 // until the arena grows.
 cudaError_t lm_graph_build(LmGraph* g, const PairDev* pairs, PairState* states, const double* guess, LmCall* call, LmSched* sched,
-                           int blocks_search, int blocks_accum) {
+                           int blocks_search, int blocks_accum, int n_cached) {
   cudaError_t e;
   if ((e = cudaGraphCreate(&g->graph, 0)) != cudaSuccess) return e;
   cudaGraphNode_t n_init, n_while, n_search, n_accum, n_ctrl;
@@ -812,20 +827,22 @@ cudaError_t lm_graph_build(LmGraph* g, const PairDev* pairs, PairState* states, 
   const LmCall* ccall = call;
   const LmSched* csched = sched;
   {
-    void* args[] = {(void*)&pairs, (void*)&cstates, (void*)&ccall, (void*)&csched};
+    void* args[] = {(void*)&pairs, (void*)&cstates, (void*)&ccall, (void*)&csched, (void*)&n_cached};
     cudaKernelNodeParams kp = {};
     kp.func = (void*)k_gicp_search;
     kp.gridDim = dim3(blocks_search);
     kp.blockDim = dim3(STEP_THREADS);
+    kp.sharedMemBytes = sizeof(LmSlot) * n_cached;
     kp.kernelParams = args;
     if ((e = cudaGraphAddKernelNode(&n_search, body, nullptr, 0, &kp)) != cudaSuccess) return e;
   }
   {
-    void* args[] = {(void*)&pairs, (void*)&cstates, (void*)&csched};
+    void* args[] = {(void*)&pairs, (void*)&cstates, (void*)&csched, (void*)&n_cached};
     cudaKernelNodeParams kp = {};
     kp.func = (void*)k_gicp_accum;
     kp.gridDim = dim3(blocks_accum);
     kp.blockDim = dim3(STEP_THREADS);
+    kp.sharedMemBytes = sizeof(LmSlot) * n_cached;
     kp.kernelParams = args;
     if ((e = cudaGraphAddKernelNode(&n_accum, body, &n_search, 1, &kp)) != cudaSuccess) return e;
   }

@@ -131,7 +131,9 @@ struct LmSlot {
   int phase;   // the pair's phase during this step
   int seeded;  // n_lin > 0: corr[] holds the previous linearization's correspondences
 };
-constexpr int LM_SMEM_SLOTS = 512;  // slot entries cached per block (8 KB); larger batches read the rest from global memory
+constexpr int LM_SMEM_SLOTS = 512;  // most slot entries cached per block (8 KB); larger batches read the rest from global memory
+// slot entries the step kernels cache (dynamic shared memory) for an arena of `cap` pairs: every slot of a batch that fits
+__host__ __device__ inline int lm_slot_cache(int cap) { return cap < LM_SMEM_SLOTS ? cap : LM_SMEM_SLOTS; }
 
 struct LmSched {
   int n_pairs;

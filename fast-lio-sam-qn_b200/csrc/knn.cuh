@@ -253,12 +253,18 @@ __device__ __forceinline__ bool near_far_step(const NodeRec& n, float qx, float 
 
 // Exact K-NN of (qx,qy,qz) in cloud c.  One thread per query; Morton-sorted queries keep
 // neighbouring lanes on neighbouring paths (coherent loads, low divergence).
-template <typename Res>
-__device__ __forceinline__ void knn_walk(const CloudDev& c, float qx, float qy, float qz, Res& res, int skip_lo = 1, int skip_hi = 0) {
+// The traversal stack holds (ref, bound) entries.  The first S live (8 B each) in a shared-memory column of the calling
+// thread, sh = &column[0][threadIdx.x] of a __shared__ int2[S][stride] ([slot][thread]: the bank is the thread, as in
+// KnnHeap, so the divergent pushes and pops of a warp are conflict free); entries S.. go to local-memory arrays that a walk
+// only touches when it goes deeper than S (profiles/emulate_stack_depth.py: how deep the walks of each kernel go).
+// S = 0 (sh unused): the whole stack in local memory, where every push and pop is an STL/LDL through L1.
+template <int S = 0, int stride = 1, typename Res>
+__device__ __forceinline__ void knn_walk(const CloudDev& c, float qx, float qy, float qz, Res& res, int2* sh = nullptr, int skip_lo = 1,
+                                         int skip_hi = 0) {
   const float4* __restrict__ pts = c.pts;
   const float4* __restrict__ tn = c.tnodes;  // read once: c may be a reference into global memory (clouds[blockIdx.y])
-  int stack_ref[MAX_STACK];
-  float stack_d[MAX_STACK];
+  int stack_ref[MAX_STACK - S];
+  float stack_d[MAX_STACK - S];
   int sp = 0;
   int ref = c.root_ref;
   float dnode = 0.f;
@@ -266,8 +272,12 @@ __device__ __forceinline__ void knn_walk(const CloudDev& c, float qx, float qy, 
     bool alive = !(dnode > res.worst());
     while (alive && ref >= 0)  // internal node: both children's boxes live in one 64-B record
       alive = near_far_step(load_node(tn, ref), qx, qy, qz, res.worst(), ref, dnode, [&](int r, float d) {
-        stack_ref[sp] = r;
-        stack_d[sp] = d;
+        if (sp < S) {
+          sh[sp * stride] = make_int2(r, __float_as_int(d));
+        } else {
+          stack_ref[sp - S] = r;
+          stack_d[sp - S] = d;
+        }
         sp++;
       });
     if (alive) {  // leaf: up to LEAF consecutive points
@@ -293,9 +303,10 @@ __device__ __forceinline__ void knn_walk(const CloudDev& c, float qx, float qy, 
     bool found = false;
     while (sp > 0) {
       sp--;
-      if (!(stack_d[sp] > res.worst())) {
-        ref = stack_ref[sp];
-        dnode = stack_d[sp];
+      const float d = sp < S ? __int_as_float(sh[sp * stride].y) : stack_d[sp - S];
+      if (!(d > res.worst())) {
+        ref = sp < S ? sh[sp * stride].x : stack_ref[sp - S];
+        dnode = d;
         found = true;
         break;
       }

@@ -17,11 +17,13 @@ int launch_index_build(const CloudDev* d_clouds, int count, int max_n, cudaStrea
 // covariance_large_slab_bytes(count, max_n, k) of device scratch in slab (nullptr when that is 0)
 int launch_covariances(const CloudDev* d_clouds, int count, int max_n, int k, int method, unsigned long long* slab, cudaStream_t s);
 void launch_gicp_init(const PairDev* pairs, PairState* states, const double* d_guess, LmCall* call, LmSched* sched, cudaStream_t s);
-void launch_gicp_search(const PairDev* pairs, const PairState* states, int blocks, const LmCall* call, const LmSched* sched, cudaStream_t s);
-void launch_gicp_accum(const PairDev* pairs, const PairState* states, int blocks, const LmSched* sched, cudaStream_t s);
+// n_cached: slot entries the step kernels cache in shared memory, lm_slot_cache(capacity of the LM arena)
+void launch_gicp_search(const PairDev* pairs, const PairState* states, int blocks, const LmCall* call, const LmSched* sched, int n_cached,
+                        cudaStream_t s);
+void launch_gicp_accum(const PairDev* pairs, const PairState* states, int blocks, const LmSched* sched, int n_cached, cudaStream_t s);
 void launch_gicp_control(const PairDev* pairs, PairState* states, LmCall* call, LmSched* sched, cudaStream_t s);
 cudaError_t lm_graph_build(LmGraph* g, const PairDev* pairs, PairState* states, const double* guess, LmCall* call, LmSched* sched,
-                           int blocks_search, int blocks_accum);
+                           int blocks_search, int blocks_accum, int n_cached);
 void lm_graph_destroy(LmGraph* g);
 int launch_knn_queries(const CloudDev& c, const float* d_q, int nq, int qstride, int k, int* idx, float* d2, cudaStream_t s, int brute);
 void launch_set_covariances(const CloudDev& c, const double* d_cov9, cudaStream_t s);
