@@ -48,6 +48,24 @@ LM_TRIAL_DTYPE = np.dtype([("outer", "<i4"), ("trial", "<i4"), ("decision", "<i4
                            ("T", "<f8", (3, 4))])
 
 
+class LmCase(C.Structure):
+    """b200reg_lm_case: one state of the LM controller (Context.lm_step_tap)."""
+    _fields_ = [("R", C.c_double * 9), ("t", C.c_double * 3), ("H", C.c_double * 36), ("b", C.c_double * 6), ("y0", C.c_double),
+                ("yi", C.c_double), ("lambda", C.c_double), ("nu", C.c_double), ("params", GicpParams), ("outer_it", C.c_int32),
+                ("inner_it", C.c_int32), ("mode", C.c_int32), ("reserved", C.c_int32)]
+
+
+class LmStep(C.Structure):
+    """b200reg_lm_step: what the LM controller made of one LmCase."""
+    _fields_ = [("d", C.c_double * 6), ("dR", C.c_double * 9), ("dt", C.c_double * 3), ("Rt", C.c_double * 9), ("tt", C.c_double * 3),
+                ("R", C.c_double * 9), ("t", C.c_double * 3), ("lambda", C.c_double), ("nu", C.c_double), ("record", LmTrial),
+                ("phase", C.c_int32), ("converged", C.c_int32), ("lm_failed", C.c_int32), ("has_trial", C.c_int32),
+                ("outer_it", C.c_int32), ("inner_it", C.c_int32)]
+
+
+LM_TAP_MODES = {"linearize": 0, "trial": 1}
+
+
 class QuatroParams(C.Structure):
     _fields_ = [("fpfh_normal_radius", C.c_double), ("fpfh_radius", C.c_double), ("noise_bound", C.c_double),
                 ("rot_gnc_factor", C.c_double), ("rot_cost_thr", C.c_double), ("rot_max_iter", C.c_int32),
@@ -97,7 +115,7 @@ EXPORTS = [
     "b200reg_comm_unique_id", "b200reg_comm_init", "b200reg_comm_destroy", "b200reg_comm_rank", "b200reg_comm_world",
     "b200reg_allgather_results", "b200reg_radius_search", "b200reg_quatro_align_ex", "b200reg_quatro_solve_tap",
     "b200reg_ctx_set_lm_trace", "b200reg_lm_trace", "b200reg_ctx_set_loop_clouds", "b200reg_loop_clouds",
-    "b200reg_match_tap",
+    "b200reg_match_tap", "b200reg_lm_step_tap",
 ]
 ESTATE = -4  # B200REG_ESTATE
 # B200REG_CLOUD_*: the loop clouds (Context.set_loop_clouds / Context.loop_clouds)
@@ -538,6 +556,36 @@ class Context:
         _check(lib().b200reg_compute_error(self.h, src.h, tgt.h, Tl.ctypes.data_as(C.c_void_p), Tt.ctypes.data_as(C.c_void_p),
                                            C.c_double(max_corr_dist), C.byref(err)))
         return err.value
+
+    def lm_step_tap(self, cases):
+        """The solve's LM controller on caller states.  cases: dicts with mode ("linearize" or "trial"), H (6, 6), b (6,),
+        y0, lambda (< 0: the init rule), and optionally R (3, 3) / t (3,) (x0, default identity), nu (2), yi (0), outer_it,
+        inner_it (0) and params (GicpParams, default_params()) -> one dict per case: d, dR (3, 3), dt, Rt (3, 3), tt, R, t,
+        lambda, nu (after the decision), record (mode "trial": the trial's trace record, LM_TRIAL_DTYPE), phase, converged,
+        lm_failed, has_trial, outer_it, inner_it."""
+        n = len(cases)
+        arr = (LmCase * n)()
+        for c, k in zip(arr, cases):
+            c.R[:] = [float(x) for x in np.asarray(k.get("R", np.eye(3)), np.float64).reshape(9)]
+            c.t[:] = [float(x) for x in np.asarray(k.get("t", np.zeros(3)), np.float64).reshape(3)]
+            c.H[:] = [float(x) for x in np.asarray(k["H"], np.float64).reshape(36)]
+            c.b[:] = [float(x) for x in np.asarray(k["b"], np.float64).reshape(6)]
+            c.y0, c.yi = float(k["y0"]), float(k.get("yi", 0.0))
+            setattr(c, "lambda", float(k["lambda"]))
+            c.nu = float(k.get("nu", 2.0))
+            c.params = k.get("params") or default_params()
+            c.outer_it, c.inner_it = int(k.get("outer_it", 0)), int(k.get("inner_it", 0))
+            c.mode = LM_TAP_MODES[k["mode"]]
+        out = (LmStep * n)()
+        _check(lib().b200reg_lm_step_tap(self.h, n, arr, out))
+        res = []
+        for o in out:
+            rec = np.frombuffer(bytes(o.record), LM_TRIAL_DTYPE)[0]
+            res.append(dict(d=np.array(o.d), dR=np.array(o.dR).reshape(3, 3), dt=np.array(o.dt), Rt=np.array(o.Rt).reshape(3, 3),
+                            tt=np.array(o.tt), R=np.array(o.R).reshape(3, 3), t=np.array(o.t), nu=o.nu, record=rec,
+                            phase=o.phase, converged=o.converged, lm_failed=o.lm_failed, has_trial=o.has_trial,
+                            outer_it=o.outer_it, inner_it=o.inner_it, **{"lambda": getattr(o, "lambda")}))
+        return res
 
 
 def comm_unique_id():

@@ -109,6 +109,8 @@ size_t b200reg_struct_size(int which) {
     case 4: return sizeof(b200reg_loop_config);
     case 5: return sizeof(b200reg_loop_factor);
     case 6: return sizeof(b200reg_lm_trial);
+    case 7: return sizeof(b200reg_lm_case);
+    case 8: return sizeof(b200reg_lm_step);
     default: return 0;
   }
 }

@@ -1,5 +1,5 @@
 // api_gicp.cu -- the C ABI of the Nano-GICP path: the context's LM arena, b200reg_gicp_align, b200reg_icp_alignment and the
-// linearize / compute_error taps.
+// linearize / compute_error / LM controller taps.
 #include <algorithm>
 #include <cstddef>
 #include <cstdlib>
@@ -236,7 +236,7 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
   auto& tr = c->lm_trace;
   tr.valid = false;
   if (tr.enabled) {
-    // every outer iteration makes at most max(lm_max_iterations, 1) trials: the buffer holds any solve's records
+    // every outer iteration makes at most lm_max_iterations trials (none when that is <= 0): the buffer holds any solve's records
     hc.trace_stride = (long long)std::max(params->max_iterations, 0) * std::max(params->lm_max_iterations, 1);
     const size_t bytes = sizeof(b200reg_lm_trial) * (size_t)hc.trace_stride * count;
     if (bytes) {
@@ -475,6 +475,23 @@ int b200reg_compute_error(b200reg_ctx* c, const b200reg_cloud* src, const b200re
   CU(cudaMemcpyAsync(&st, d_st, sizeof(PairState), cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
   *err = st.y_trial;
+  return B200REG_OK;
+}
+
+int b200reg_lm_step_tap(b200reg_ctx* c, int n, const b200reg_lm_case* cases, b200reg_lm_step* out) {
+  if (!c || n <= 0 || !cases || !out) return fail(B200REG_EINVAL, "bad argument");
+  CU(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  Scratch scratch(c);
+  b200reg_lm_case* d_cases = nullptr;
+  b200reg_lm_step* d_out = nullptr;
+  CU(scratch.alloc((void**)&d_cases, sizeof(b200reg_lm_case) * (size_t)n));
+  CU(scratch.alloc((void**)&d_out, sizeof(b200reg_lm_step) * (size_t)n));
+  CU(cudaMemcpyAsync(d_cases, cases, sizeof(b200reg_lm_case) * (size_t)n, cudaMemcpyHostToDevice, s));
+  c->launches += launch_lm_step_tap(d_cases, n, d_out, s);
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(out, d_out, sizeof(b200reg_lm_step) * (size_t)n, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
   return B200REG_OK;
 }
 

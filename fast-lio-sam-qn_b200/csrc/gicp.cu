@@ -86,11 +86,24 @@ __device__ void so3_exp_matrix(const double w[3], double R[9]) {
   R[6] = txz - twy;       R[7] = tyz + twx;       R[8] = 1 - (txx + tyy);
 }
 
+// is_converged (lsq_registration_impl.hpp:117-127): max of (1.0 / eps) * |x| < 1, the reciprocal first as the reference
+// writes it (|x| / eps rounds differently at |x| = eps for some eps, e.g. 1e-5).  A NaN anywhere in the step is not
+// converged: the reference's maxCoeff of an all-NaN block is NaN and NaN < 1 is false (fmax would drop it).  DESIGN §4.
 __device__ bool delta_converged(const PairState* st, const GicpParamsDev& prm) {
-  double mr = 0, mt = 0;
-  for (int i = 0; i < 9; i++) mr = fmax(mr, fabs(st->dR[i] - ((i % 4) == 0 ? 1.0 : 0.0)) / prm.rotation_eps);
-  for (int i = 0; i < 3; i++) mt = fmax(mt, fabs(st->dt[i]) / prm.transformation_eps);
-  return fmax(mr, mt) < 1.0;
+  const double ir = 1.0 / prm.rotation_eps, it = 1.0 / prm.transformation_eps;
+  double m = 0;
+  bool nan = false;
+  for (int i = 0; i < 9; i++) {
+    const double v = ir * fabs(st->dR[i] - ((i % 4) == 0 ? 1.0 : 0.0));
+    nan |= isnan(v);
+    m = fmax(m, v);
+  }
+  for (int i = 0; i < 3; i++) {
+    const double v = it * fabs(st->dt[i]);
+    nan |= isnan(v);
+    m = fmax(m, v);
+  }
+  return !nan && m < 1.0;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -151,13 +164,22 @@ __device__ void lm_update(PairState* st, const double* sums, const GicpParamsDev
     st->y0 = sums[27];
     st->n_lin++;
     st->nr_iterations = st->outer_it;
-    if (st->lambda < 0.0) {
+    if (st->lambda < 0.0) {  // maxCoeff of |diag H|: a NaN on the diagonal makes lambda NaN, as in the reference
       double mx = 0;
-      for (int i = 0; i < 6; i++) mx = fmax(mx, fabs(st->H[7 * i]));
-      st->lambda = prm.lm_init_lambda_factor * mx;
+      bool nan = false;
+      for (int i = 0; i < 6; i++) {
+        nan |= isnan(st->H[7 * i]);
+        mx = fmax(mx, fabs(st->H[7 * i]));
+      }
+      st->lambda = prm.lm_init_lambda_factor * (nan ? (double)NAN : mx);
     }
     st->nu = 2.0;
     st->inner_it = 0;
+    if (prm.lm_max_iterations <= 0) {  // step_lm's trial loop runs no trial and returns false: "lm not converged!!"
+      st->lm_failed = 1;
+      lm_finish(st, 0);
+      return;
+    }
     lm_prepare_trial(st);
   } else if (phase == PH_TRIAL) {
     const double yi = sums[0];
@@ -739,6 +761,80 @@ __global__ void __launch_bounds__(STEP_THREADS) k_knn_brute(CloudDev c, const fl
       }
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------
+// debug tap: the LM controller (lm_prepare_trial / lm_update, the functions the solve runs) on caller-supplied states,
+// one thread per case (b200reg_lm_step_tap)
+// ---------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) k_lm_step_tap(const b200reg_lm_case* cases, int n, b200reg_lm_step* out) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const b200reg_lm_case& c = cases[k];
+  GicpParamsDev prm;  // the fields lm_update reads
+  prm.max_iterations = c.params.max_iterations;
+  prm.lm_max_iterations = c.params.lm_max_iterations;
+  prm.max_corr_dist2 = 0.0;
+  prm.transformation_eps = c.params.transformation_eps;
+  prm.rotation_eps = c.params.rotation_eps;
+  prm.lm_init_lambda_factor = c.params.lm_init_lambda_factor;
+  prm.icp_score_thr = 0.0;
+  PairState st;
+  memset(&st, 0, sizeof(st));
+  for (int i = 0; i < 9; i++) st.R[i] = c.R[i];
+  for (int i = 0; i < 3; i++) st.t[i] = c.t[i];
+  st.lambda = c.lambda;
+  st.nu = c.nu;
+  st.outer_it = c.outer_it;
+  st.inner_it = c.inner_it;
+  st.nr_iterations = c.outer_it;
+  st.phase = PH_LINEARIZE;
+  double sums[NRED];
+  int q = 0;
+  for (int i = 0; i < 6; i++)
+    for (int j = i; j < 6; j++) sums[q++] = c.H[6 * i + j];  // the upper triangle, as k_gicp_control hands it over
+  for (int i = 0; i < 6; i++) sums[21 + i] = c.b[i];
+  sums[27] = c.y0;
+  b200reg_lm_step& o = out[k];
+  memset(&o, 0, sizeof(o));
+  if (c.mode == 0) {
+    lm_update(&st, sums, prm, PH_LINEARIZE, 0, nullptr, nullptr);
+  } else {
+    for (int i = 0; i < 36; i++) st.H[i] = c.H[i];
+    for (int i = 0; i < 6; i++) st.b[i] = c.b[i];
+    st.y0 = c.y0;
+    lm_prepare_trial(&st);
+  }
+  // the trial this call prepared (a rejection prepares the next one: these are the values before the decision)
+  for (int i = 0; i < 6; i++) o.d[i] = st.d[i];
+  for (int i = 0; i < 9; i++) {
+    o.dR[i] = st.dR[i];
+    o.Rt[i] = st.Rt[i];
+  }
+  for (int i = 0; i < 3; i++) {
+    o.dt[i] = st.dt[i];
+    o.tt[i] = st.tt[i];
+  }
+  o.has_trial = st.phase == PH_TRIAL;
+  if (c.mode != 0 && o.has_trial) {
+    const double yi[1] = {c.yi};
+    lm_update(&st, yi, prm, PH_TRIAL, 0, nullptr, &o.record);
+  }
+  o.lambda = st.lambda;
+  o.nu = st.nu;
+  o.phase = st.phase;
+  o.converged = st.converged;
+  o.lm_failed = st.lm_failed;
+  o.outer_it = st.outer_it;
+  o.inner_it = st.inner_it;
+  for (int i = 0; i < 9; i++) o.R[i] = st.R[i];
+  for (int i = 0; i < 3; i++) o.t[i] = st.t[i];
+}
+
+int launch_lm_step_tap(const b200reg_lm_case* d_cases, int n, b200reg_lm_step* d_out, cudaStream_t s) {
+  if (n <= 0) return 0;
+  k_lm_step_tap<<<(n + 127) / 128, 128, 0, s>>>(d_cases, n, d_out);
+  return 1;
 }
 
 // setSourceCovariances / setTargetCovariances: caller's 3x3 blocks (original order) -> packed symmetric, sorted order

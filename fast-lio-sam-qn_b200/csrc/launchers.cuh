@@ -27,6 +27,7 @@ cudaError_t lm_graph_build(LmGraph* g, const PairDev* pairs, PairState* states, 
 void lm_graph_destroy(LmGraph* g);
 int launch_knn_queries(const CloudDev& c, const float* d_q, int nq, int qstride, int k, int* idx, float* d2, cudaStream_t s, int brute);
 void launch_set_covariances(const CloudDev& c, const double* d_cov9, cudaStream_t s);
+int launch_lm_step_tap(const b200reg_lm_case* d_cases, int n, b200reg_lm_step* d_out, cudaStream_t s);
 void launch_transform_out(const CloudDev& c, const float* d_Tf, float* d_out3, cudaStream_t s);
 
 // quatro.cu

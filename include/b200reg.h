@@ -136,9 +136,43 @@ typedef struct b200reg_lm_trial {
   double T[12];        /* x0 after the decision, row-major 3 x 4                                                     */
 } b200reg_lm_trial;
 
+/* One input of b200reg_lm_step_tap: the LM controller's state at one point of step_lm. */
+typedef struct b200reg_lm_case {
+  double R[9], t[3];   /* x0, row-major                                                                           */
+  double H[36];        /* symmetric 6 x 6, row-major (mode 0 reads the upper triangle, as linearize hands it over)  */
+  double b[6];
+  double y0;           /* error at x0                                                                              */
+  double yi;           /* mode 1: compute_error at the trial pose                                                  */
+  double lambda;       /* lm_lambda_ in force; < 0 = not yet set (mode 0 then applies the init rule)                */
+  double nu;           /* mode 1: the nu in force (mode 0 resets it to 2)                                           */
+  b200reg_gicp_params params;  /* the controller reads max_iterations, lm_max_iterations, transformation_eps,
+                                  rotation_eps and lm_init_lambda_factor                                            */
+  int32_t outer_it;    /* nr_iterations_                                                                           */
+  int32_t inner_it;    /* mode 1: step_lm's i of this trial                                                        */
+  int32_t mode;        /* 0: the start of step_lm after linearize (H, b, y0) and its first trial's step;
+                          1: one trial: the step from (H, b, lambda), then the decision on yi                        */
+  int32_t reserved;
+} b200reg_lm_case;
+
+/* One output of b200reg_lm_step_tap. */
+typedef struct b200reg_lm_step {
+  double d[6];         /* the trial's step (rotation, translation), from the device's solve of (H + lambda I) d = -b  */
+  double dR[9];        /* so3_exp(d[0..2]), row-major                                                              */
+  double dt[3];
+  double Rt[9], tt[3]; /* the trial pose delta * x0                                                                */
+  double R[9], t[3];   /* x0 after the decision                                                                    */
+  double lambda, nu;   /* after the decision                                                                       */
+  b200reg_lm_trial record;  /* mode 1: the trial's trace record (rho, decision, ...)                              */
+  int32_t phase;       /* 0 linearize next, 1 a trial is prepared, 2 the solve is finished                         */
+  int32_t converged;
+  int32_t lm_failed;
+  int32_t has_trial;   /* a trial was prepared (d .. tt hold it)                                                    */
+  int32_t outer_it, inner_it;  /* after the decision                                                               */
+} b200reg_lm_step;
+
 /* sizeof() of the ABI structs as compiled into the library, so that a binding (ctypes, cgo, JNI ...) can check its own
  * layout at load time: 0 gicp_params, 1 result, 2 quatro_params, 3 quatro_info, 4 loop_config, 5 loop_factor,
- * 6 lm_trial.  0 = unknown. */
+ * 6 lm_trial, 7 lm_case, 8 lm_step.  0 = unknown. */
 size_t b200reg_struct_size(int which);
 
 /* ---- context ---------------------------------------------------------------------- */
@@ -488,6 +522,11 @@ int b200reg_linearize(b200reg_ctx* ctx, const b200reg_cloud* src, const b200reg_
  * taken from ONE linearize at T_lin16 (they stay stale, as in step_lm), then sum e^T M e is evaluated at T_trial16.  */
 int b200reg_compute_error(b200reg_ctx* ctx, const b200reg_cloud* src, const b200reg_cloud* tgt, const double* T_lin16,
                           const double* T_trial16, double max_corr_dist, double* err);
+/* The LM controller of the solve (step_lm, lsq_registration_impl.hpp:160-208) on n caller-supplied states, one device
+ * thread per case, through the same device functions b200reg_gicp_align runs: mode 0 runs what follows a linearize
+ * (lambda init, nu = 2, the first trial's step, or lm_failed when lm_max_iterations <= 0); mode 1 prepares one trial from
+ * (H, b, lambda) and decides it on yi (accept / reject / converged / out of trials, the lambda and nu rules).       */
+int b200reg_lm_step_tap(b200reg_ctx* ctx, int n, const b200reg_lm_case* cases, b200reg_lm_step* out);
 
 #ifdef __cplusplus
 }

@@ -17,11 +17,11 @@ class GicpParams(C.Structure):
     # effective defaults of the reference deployment (SURVEY.md App. A.1)
     _fields_ = [("k_correspondences", C.c_int), ("max_iterations", C.c_int), ("max_corr_dist", C.c_double),
                 ("transformation_eps", C.c_double), ("rotation_eps", C.c_double), ("lm_max_iterations", C.c_int),
-                ("lm_init_lambda_factor", C.c_double)]
+                ("lm_init_lambda_factor", C.c_double), ("regularization", C.c_int)]
 
     @staticmethod
     def default():
-        return GicpParams(15, 32, 52.5, 0.01, 2e-3, 10, 1e-9)
+        return GicpParams(15, 32, 52.5, 0.01, 2e-3, 10, 1e-9, 3)
 
 
 class GicpResult(C.Structure):

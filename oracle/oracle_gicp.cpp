@@ -395,14 +395,22 @@ static double compute_error(const GicpProblem& P, const Iso& x) {
   return sum_errors;
 }
 
-// LsqRegistration::is_converged, NG/impl/lsq_registration_impl.hpp:117-127
+// LsqRegistration::is_converged, NG/impl/lsq_registration_impl.hpp:117-127: (1.0 / eps) * |x| as written there (:123-124),
+// and a NaN anywhere in delta is not converged (the maxCoeff of an all-NaN block is NaN, and NaN < 1 is false)
 static bool is_converged(const Iso& delta, double rot_eps, double trans_eps) {
-  double mr = 0, mt = 0;
+  double m = 0;
+  bool nan = false;
   for (int i = 0; i < 3; i++) {
-    for (int j = 0; j < 3; j++) mr = std::max(mr, std::fabs(delta.R(i, j) - (i == j ? 1.0 : 0.0)) / rot_eps);
-    mt = std::max(mt, std::fabs(delta.t[i]) / trans_eps);
+    for (int j = 0; j < 3; j++) {
+      const double v = 1.0 / rot_eps * std::fabs(delta.R(i, j) - (i == j ? 1.0 : 0.0));
+      nan = nan || std::isnan(v);
+      m = std::max(m, v);
+    }
+    const double v = 1.0 / trans_eps * std::fabs(delta.t[i]);
+    nan = nan || std::isnan(v);
+    m = std::max(m, v);
   }
-  return std::max(mr, mt) < 1;
+  return !nan && m < 1;
 }
 
 }  // namespace orc
@@ -419,6 +427,7 @@ struct orc_gicp_params {
   double rotation_eps;         // lsq_registration_impl.hpp:53 -> 2e-3
   int lm_max_iterations;       // lsq_registration_impl.hpp:58 -> 10
   double lm_init_lambda_factor;  // lsq_registration_impl.hpp:59 -> 1e-9
+  int regularization;          // RegularizationMethod of both clouds' covariances: 0 NONE .. 4 FROBENIUS (3 PLANE)
 };
 
 struct orc_gicp_result {
@@ -534,11 +543,11 @@ int orc_gicp_align(const float* src, int N, int sstride, const float* tgt, int M
   sidx.build(src, N, sstride);  // setInputSource -> buildIndex (nano_gicp_impl.hpp:120-129)
   double t1 = now_ms();
   std::vector<double> cov_src((size_t)N * 9), cov_tgt((size_t)M * 9);
-  covariances(src, N, sstride, sidx, prm->k_correspondences, cov_src.data(), nullptr);
+  covariances(src, N, sstride, sidx, prm->k_correspondences, cov_src.data(), nullptr, prm->regularization);
   double t2 = now_ms();
   tidx.build(tgt, M, tstride);
   double t3 = now_ms();
-  covariances(tgt, M, tstride, tidx, prm->k_correspondences, cov_tgt.data(), nullptr);
+  covariances(tgt, M, tstride, tidx, prm->k_correspondences, cov_tgt.data(), nullptr, prm->regularization);
   double t4 = now_ms();
   // pcl::Registration::align builds PCL's own FLANN tree on the target as well
   // (SURVEY §3.4 "hidden 3rd tree build"); charged to the CPU baseline as one more build.
@@ -560,10 +569,14 @@ int orc_gicp_align(const float* src, int N, int sstride, const float* tgt, int M
     Iso xlin = x0;
     double y0 = linearize(P, x0, H, b);
     n_lin++;
-    if (lm_lambda < 0.0) {
+    if (lm_lambda < 0.0) {  // maxCoeff of |diag H|; a NaN there makes lambda NaN
       double mx = 0;
-      for (int d = 0; d < 6; d++) mx = std::max(mx, std::fabs(H[7 * d]));
-      lm_lambda = prm->lm_init_lambda_factor * mx;
+      bool nan = false;
+      for (int d = 0; d < 6; d++) {
+        nan = nan || std::isnan(H[7 * d]);
+        mx = std::max(mx, std::fabs(H[7 * d]));
+      }
+      lm_lambda = prm->lm_init_lambda_factor * (nan ? std::nan("") : mx);
     }
     double nu = 2.0;
     Iso delta = iso_identity();

@@ -32,10 +32,13 @@ def so3_exp(w):
 
 
 def is_converged(delta, rotation_eps, transformation_eps):
-    """LsqRegistration::is_converged (lsq_registration_impl.hpp:117-127)."""
-    r = np.abs(delta[:3, :3] - np.eye(3)).max() / rotation_eps
-    t = np.abs(delta[:3, 3]).max() / transformation_eps
-    return max(r, t) < 1
+    """LsqRegistration::is_converged (lsq_registration_impl.hpp:117-127): (1.0 / eps) * |x| as the reference writes it; a
+    NaN anywhere in delta is not converged."""
+    r = 1.0 / rotation_eps * np.abs(delta[:3, :3] - np.eye(3))
+    t = 1.0 / transformation_eps * np.abs(delta[:3, 3])
+    if np.isnan(r).any() or np.isnan(t).any():
+        return False
+    return max(r.max(), t.max()) < 1
 
 
 def replay(oracle, src, tgt, params=None, guess=None):
@@ -53,6 +56,9 @@ def replay(oracle, src, tgt, params=None, guess=None):
         if lam is None:  # lm_lambda_ < 0 at the first step_lm of the solve (:165-167)
             lam = prm.lm_init_lambda_factor * np.abs(np.diag(H)).max()
         nu = 2.0
+        if prm.lm_max_iterations <= 0:  # step_lm runs no trial and returns false: "lm not converged!!"
+            assert (n_trials, outcome) == (0, 0) and it == len(o["trace"]) - 1, ("no trial", it, n_trials, outcome)
+            break
         for i in range(prm.lm_max_iterations):
             d = np.linalg.solve(H + lam * np.eye(6), -b)
             delta = np.eye(4)

@@ -45,8 +45,11 @@ def test_struct_layouts_match_header():
     lib = native.lib()
     lib.b200reg_struct_size.restype = ctypes.c_size_t
     for which, st in enumerate((native.GicpParams, native.Result, native.QuatroParams, native.QuatroInfo, native.LoopConfig,
-                                native.LoopFactor)):
+                                native.LoopFactor, native.LmTrial, native.LmCase, native.LmStep)):
         assert lib.b200reg_struct_size(which) == ctypes.sizeof(st), st.__name__
+    assert lib.b200reg_struct_size(9) == 0
+    assert ctypes.sizeof(native.LmCase) == 58 * 8 + 56 + 4 * 4 and native.LmCase.params.offset == 58 * 8
+    assert ctypes.sizeof(native.LmStep) == 44 * 8 + 200 + 6 * 4 and native.LmStep.record.offset == 44 * 8
     assert native.Result.pose_between.offset == 192
     p = native.default_params()
     assert (p.k_correspondences, p.max_iterations, p.lm_max_iterations) == (15, 32, 10)
