@@ -115,7 +115,7 @@ EXPORTS = [
     "b200reg_comm_unique_id", "b200reg_comm_init", "b200reg_comm_destroy", "b200reg_comm_rank", "b200reg_comm_world",
     "b200reg_allgather_results", "b200reg_radius_search", "b200reg_quatro_align_ex", "b200reg_quatro_solve_tap",
     "b200reg_ctx_set_lm_trace", "b200reg_lm_trace", "b200reg_ctx_set_loop_clouds", "b200reg_loop_clouds",
-    "b200reg_match_tap", "b200reg_lm_step_tap",
+    "b200reg_match_tap", "b200reg_lm_step_tap", "b200reg_index_tap", "b200reg_sort_tap",
 ]
 ESTATE = -4  # B200REG_ESTATE
 # B200REG_CLOUD_*: the loop clouds (Context.set_loop_clouds / Context.loop_clouds)
@@ -530,6 +530,46 @@ class Context:
         for o, m in zip(out, nm):
             o["mutual"] = o["mutual"][:m].copy()
         return out
+
+    def index_tap(self, arrays, device=False):
+        """The spatial index of each cloud as b200reg_clouds_create builds it, in one batched build.  arrays: host float32
+        (n, >= 3) arrays of one width (the record stride), or with device=True contiguous float32 CUDA tensors (anything with
+        data_ptr()) of one width -> one dict per cloud: keys (n,) uint32 sorted Morton keys, pts (n, 4) float32 sorted points
+        (w = original index bits), orig (n,) int32 (those bits), rank (n,) int32, tnodes (n - 1, 4, 4) float32 records,
+        root_ref (int)."""
+        if device:
+            ptrs, ns, width = [a.data_ptr() for a in arrays], [int(a.shape[0]) for a in arrays], int(arrays[0].shape[1])
+        else:
+            arrs = [_pts(a) for a in arrays]
+            ptrs, ns, width = [a.ctypes.data for a in arrs], [len(a) for a in arrs], arrs[0].shape[1]
+        assert all(int(a.shape[1]) == width for a in arrays)
+        cnt = len(ns)
+        out = [dict(keys=np.empty(n, np.uint32), pts=np.empty((n, 4), np.float32), rank=np.empty(n, np.int32),
+                    tnodes=np.empty((max(n - 1, 1), 4, 4), np.float32)) for n in ns]
+        vp = lambda key: (C.c_void_p * cnt)(*[o[key].ctypes.data for o in out])
+        roots = np.empty(cnt, np.int32)
+        _check(lib().b200reg_index_tap(self.h, cnt, (C.c_void_p * cnt)(*ptrs), (C.c_size_t * cnt)(*ns), C.c_size_t(width * 4),
+                                       int(bool(device)), vp("keys"), vp("pts"), vp("rank"), vp("tnodes"),
+                                       roots.ctypes.data_as(C.c_void_p)))
+        for o, n, r in zip(out, ns, roots):
+            o["tnodes"] = o["tnodes"][:n - 1]
+            o["orig"] = o["pts"][:, 3].view(np.int32).copy()
+            o["root_ref"] = int(r)
+        return out
+
+    def sort_tap(self, keys, vals=None, key_bits=32):
+        """The shared stable radix sort on host arrays, one batched call.  keys: list of uint32 arrays; vals: list of uint32
+        arrays (default: 0..n-1) -> list of (sorted keys, values carried along); key_bits 30 or 32 (include/b200reg.h)."""
+        ks = [np.ascontiguousarray(k, np.uint32) for k in keys]
+        vs = [np.arange(len(k), dtype=np.uint32) for k in ks] if vals is None else [np.ascontiguousarray(v, np.uint32) for v in vals]
+        assert all(len(k) == len(v) for k, v in zip(ks, vs))
+        cnt = len(ks)
+        ko = [np.empty_like(k) for k in ks]
+        vo = [np.empty_like(v) for v in vs]
+        vp = lambda arrs: (C.c_void_p * cnt)(*[a.ctypes.data for a in arrs])
+        _check(lib().b200reg_sort_tap(self.h, cnt, vp(ks), vp(vs), (C.c_int32 * cnt)(*[len(k) for k in ks]), int(key_bits),
+                                      vp(ko), vp(vo)))
+        return list(zip(ko, vo))
 
     def get_covariances(self, cloud):
         out = np.empty((cloud.n, 3, 3), np.float64)

@@ -217,7 +217,7 @@ int b200reg_clouds_create(b200reg_ctx* c, int count, const float* const* xyz, co
 }  // extern "C"
 
 int b200::clouds_create(b200reg_ctx* c, int count, const float* const* xyz, const size_t* n, size_t stride_bytes, int on_device,
-                        bool keep_intensity, b200reg_cloud** out) {
+                        bool keep_intensity, b200reg_cloud** out, uint32_t* const* keys_out) {
   if (!c || count <= 0 || !xyz || !n || !out) return fail(B200REG_EINVAL, "bad argument");
   if (stride_bytes < 12 || stride_bytes % 4) return fail(B200REG_EINVAL, "stride_bytes must be a multiple of 4, >= 12");
   for (int i = 0; i < count; i++)
@@ -303,6 +303,9 @@ int b200::clouds_create(b200reg_ctx* c, int count, const float* const* xyz, cons
     for (int i = 0; i < count; i++) c->prof_bytes[CLS_BUILD] += 36.0 * descs[i].n;  // SURVEY §8(d) K1
   }
   CU(cudaGetLastError());
+  if (keys_out)  // the sorted Morton keys, before the temporaries go (b200reg_index_tap)
+    for (int i = 0; i < count; i++)
+      CU(cudaMemcpyAsync(keys_out[i], descs[i].keys[radix_sort_result_buf(30)], (size_t)descs[i].n * 4, cudaMemcpyDeviceToHost, s));
   if (keep_intensity) {  // from the raw records, while they are still there
     std::vector<float*> inten(count);
     for (int i = 0; i < count; i++) inten[i] = bag.cl[i]->inten;
@@ -320,7 +323,7 @@ int b200::clouds_create(b200reg_ctx* c, int count, const float* const* xyz, cons
     d.parent_node = d.parent_leaf = nullptr;
     d.bbox = nullptr;
   }
-  if (!on_device) CU(cudaStreamSynchronize(s));  // host buffers have been consumed when the call returns (pinned or not)
+  if (!on_device || keys_out) CU(cudaStreamSynchronize(s));  // host buffers have been consumed (or filled) when the call returns
   std::copy(bag.cl.begin(), bag.cl.end(), out);  // the caller owns the clouds from here on
   bag.cl.clear();
   return B200REG_OK;
@@ -665,6 +668,73 @@ int b200reg_cloud_points(b200reg_ctx* c, const b200reg_cloud* cl, float* xyz_out
     xyz_out[3 * (size_t)orig[p] + 1] = pts[p].y;
     xyz_out[3 * (size_t)orig[p] + 2] = pts[p].z;
   }
+  return B200REG_OK;
+}
+
+int b200reg_index_tap(b200reg_ctx* c, int count, const float* const* xyz, const size_t* n, size_t stride_bytes, int on_device,
+                      uint32_t* const* keys_out, float* const* pts_out, int32_t* const* rank_out, float* const* tnodes_out,
+                      int32_t* root_ref_out) {
+  if (!c || count <= 0 || !keys_out || !pts_out || !rank_out || !tnodes_out || !root_ref_out) return fail(B200REG_EINVAL, "bad argument");
+  for (int i = 0; i < count; i++)
+    if (!keys_out[i] || !pts_out[i] || !rank_out[i] || (!tnodes_out[i] && n && n[i] > 1)) return fail(B200REG_EINVAL, "bad argument");
+  CloudBag bag(c);
+  bag.cl.assign(count, nullptr);
+  if (const int rc = clouds_create(c, count, xyz, n, stride_bytes, on_device, false, bag.cl.data(), keys_out)) return rc;
+  cudaStream_t s = c->stream;
+  for (int i = 0; i < count; i++) {
+    const CloudDev& d = bag.cl[i]->dev;
+    CU(cudaMemcpyAsync(pts_out[i], d.pts, (size_t)d.n * 16, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(rank_out[i], d.rank, (size_t)d.n * 4, cudaMemcpyDeviceToHost, s));
+    if (d.n > 1) CU(cudaMemcpyAsync(tnodes_out[i], d.tnodes, (size_t)(d.n - 1) * 64, cudaMemcpyDeviceToHost, s));
+    root_ref_out[i] = d.root_ref;
+  }
+  CU(cudaStreamSynchronize(s));
+  return B200REG_OK;
+}
+
+int b200reg_sort_tap(b200reg_ctx* c, int count, const uint32_t* const* keys, const uint32_t* const* vals, const int32_t* n,
+                     int key_bits, uint32_t* const* keys_out, uint32_t* const* vals_out) {
+  if (!c || count <= 0 || !keys || !vals || !n || !keys_out || !vals_out) return fail(B200REG_EINVAL, "bad argument");
+  if (key_bits != 30 && key_bits != 32) return fail(B200REG_EINVAL, "key_bits must be 30 or 32");
+  for (int i = 0; i < count; i++) {
+    if (!keys[i] || !vals[i] || !keys_out[i] || !vals_out[i]) return fail(B200REG_EINVAL, "bad argument");
+    // the look-back publishes (flag << 30) | count: a digit count must fit 30 bits
+    if (n[i] < 1 || n[i] >= (1 << 30)) return fail(B200REG_EINVAL, "sizes must be 1..2^30-1");
+  }
+  CU(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  Scratch scratch(c);
+  std::vector<CloudDev> descs(count);
+  std::vector<size_t> o_ws(count);
+  Layout zl;
+  for (int i = 0; i < count; i++) o_ws[i] = zl.take(radix_sort_ws_bytes(n[i], key_bits));
+  char* zeroed = nullptr;
+  CU(scratch.alloc((void**)&zeroed, zl.size));
+  CU(cudaMemsetAsync(zeroed, 0, zl.size, s));
+  int max_n = 0;
+  for (int i = 0; i < count; i++) {
+    CloudDev d = {};
+    d.n = n[i];
+    for (int b = 0; b < 2; b++) {
+      CU(scratch.alloc((void**)&d.keys[b], (size_t)n[i] * 4));
+      CU(scratch.alloc((void**)&d.vals[b], (size_t)n[i] * 4));
+    }
+    CU(cudaMemcpyAsync(d.keys[0], keys[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(d.vals[0], vals[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, s));
+    d.hist = (uint32_t*)(zeroed + o_ws[i]);
+    descs[i] = d;
+    max_n = std::max(max_n, d.n);
+  }
+  CloudDev* d_descs = nullptr;
+  CU(scratch.upload(&d_descs, descs.data(), sizeof(CloudDev) * count));
+  c->launches += launch_radix_sort(d_descs, count, max_n, key_bits, s);
+  CU(cudaGetLastError());
+  const int r = radix_sort_result_buf(key_bits);
+  for (int i = 0; i < count; i++) {
+    CU(cudaMemcpyAsync(keys_out[i], descs[i].keys[r], (size_t)n[i] * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(vals_out[i], descs[i].vals[r], (size_t)n[i] * 4, cudaMemcpyDeviceToHost, s));
+  }
+  CU(cudaStreamSynchronize(s));
   return B200REG_OK;
 }
 

@@ -166,9 +166,10 @@ struct Layout {
 // RegistrationOutput's defaults (loop_closure.h:64-70): identity transforms, score_ = DBL_MAX, not valid
 b200reg_result default_result();
 
-// b200reg_clouds_create; keep_intensity: each cloud also keeps the intensities of its records (b200reg_cloud::inten)
+// b200reg_clouds_create; keep_intensity: each cloud also keeps the intensities of its records (b200reg_cloud::inten);
+// keys_out (b200reg_index_tap): n[i] host words per cloud receive its sorted Morton keys before the build's temporaries go
 int clouds_create(b200reg_ctx* c, int count, const float* const* xyz, const size_t* n, size_t stride_bytes, int on_device,
-                  bool keep_intensity, b200reg_cloud** out);
+                  bool keep_intensity, b200reg_cloud** out, uint32_t* const* keys_out = nullptr);
 
 // The clouds of `count` pairs, built in one batch: the source clouds come first, then the targets.  They go to src_out /
 // tgt_out and are owned by `bag`.

@@ -329,18 +329,25 @@ __global__ void __launch_bounds__(256) k_gicp_init(const PairDev* pairs, PairSta
 // ---------------------------------------------------------------------------------------
 // Seed the heap with the K points around position i in Morton order (cheap, coalesced, usually most of the true
 // neighbours: the traversal then starts with a tight bound and only ever inserts improvements) and walk the tree.
+// A seed enters on the walk's own rule, d2 <= FLT_MAX: the NaN points (all at key 0, so often among the first points'
+// seeds) and points at infinity leave an empty slot, as they are never candidates of the walk.
 template <typename Heap, int K>
 __device__ __forceinline__ void cov_knn(const CloudDev& c, int i, float4 q, Heap& res) {
   int lo = max(0, i - K / 2), hi = min(c.n - 1, lo + K - 1);
   lo = max(0, hi - (K - 1));
 #pragma unroll
   for (int j = 0; j < K; j++) {
+    float d = 3.402823466e+38f;
+    int pos = -1;
     if (lo + j <= hi) {
       const float4 p = __ldg(&c.pts[lo + j]);
-      res.set(j, dist2_rn(q.x, q.y, q.z, p.x, p.y, p.z), lo + j);
-    } else {
-      res.set(j, 3.402823466e+38f, -1);
+      const float dj = dist2_rn(q.x, q.y, q.z, p.x, p.y, p.z);
+      if (dj <= d) {
+        d = dj;
+        pos = lo + j;
+      }
     }
+    res.set(j, d, pos);
   }
   res.heapify();
   knn_walk(c, q.x, q.y, q.z, res, nullptr, lo, hi);  // stack in local memory: on chip it ran slower on H100 (DESIGN.md §3)

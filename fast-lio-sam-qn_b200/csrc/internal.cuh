@@ -29,7 +29,10 @@ constexpr int STEP_THREADS = 128;  // threads per block of the per-point kernels
 constexpr int NRED = 28;           // 21 (H upper) + 6 (b) + 1 (err)
 constexpr int FDIM = 33;           // FPFHSignature33
 constexpr int FPAD = 36;           // descriptor record padded to 144 B (9 x float4, TMA-bulk friendly)
-constexpr int MAX_STACK = 64;      // >= LBVH depth: 30 key bits + index tie-break bits
+// >= LBVH depth.  Karras' delta strictly increases along a root-to-leaf path; distinct 30-bit keys give delta in [2, 31],
+// equal keys 32 + clz(i ^ j) with 8 <= i ^ j < 2^26 over a record's >= LEAF + 1 points (n <= 2^26), i.e. [38, 60]: at
+// most 30 + 23 = 53 records on a path (tests/index_ref.py: depth_bound; a comb of key bits plus a run reaches it).
+constexpr int MAX_STACK = 64;
 
 // The tnodes record format above, in one place: leaf_ref encodes a leaf, leaf_span decodes it, load_node reads a record.
 __host__ __device__ __forceinline__ int leaf_ref(int start, int count) { return -1 - ((start << 4) | count); }

@@ -290,14 +290,16 @@ __device__ __forceinline__ void knn_walk(const CloudDev& c, float qx, float qy, 
       for (int j = 0; j < LEAF; j++) {
         const float4 p = __ldg(&pts[base + (j < cnt ? j : 0)]);
         dl[j] = dist2_rn(qx, qy, qz, p.x, p.y, p.z);
-        if (j < cnt && !(dl[j] > w0) && !(base + j >= skip_lo && base + j <= skip_hi)) mask |= 1u << j;
+        // d <= w, not !(d > w): a point with a NaN coordinate (NaN d2) is never a candidate (KnnHeap::offer would evict
+        // its root for one)
+        if (j < cnt && dl[j] <= w0 && !(base + j >= skip_lo && base + j <= skip_hi)) mask |= 1u << j;
       }
       // ONE insertion site per leaf: candidates are fed in slot order through a select chain
       while (mask) {
         const int j = __ffs(mask) - 1;
         mask &= mask - 1;
         const float dj = res.leaf_distance(dl, j, pts, base + j, qx, qy, qz);
-        if (!(dj > res.worst())) res.offer(dj, base + j, pts);
+        if (dj <= res.worst()) res.offer(dj, base + j, pts);
       }
     }
     bool found = false;

@@ -527,6 +527,24 @@ int b200reg_compute_error(b200reg_ctx* ctx, const b200reg_cloud* src, const b200
  * (lambda init, nu = 2, the first trial's step, or lm_failed when lm_max_iterations <= 0); mode 1 prepares one trial from
  * (H, b, lambda) and decides it on yi (accept / reject / converged / out of trials, the lambda and nu rules).       */
 int b200reg_lm_step_tap(b200reg_ctx* ctx, int n, const b200reg_lm_case* cases, b200reg_lm_step* out);
+/* The spatial index of `count` clouds, built exactly as b200reg_clouds_create builds them (same arguments, same batched
+ * launches), read back and released.  Per cloud i of n[i] points:
+ *   keys_out[i]    n[i] words: the 30-bit Morton keys in sorted order
+ *   pts_out[i]     n[i] x 4 floats: the sorted points, w = the int bits of the original index
+ *   rank_out[i]    n[i]: original index -> sorted position
+ *   tnodes_out[i]  (n[i] - 1) x 16 floats (may be NULL when n[i] == 1): record r holds both children of internal node r,
+ *                  (lo0.xyz, ref0) (hi0.xyz, -) (lo1.xyz, ref1) (hi1.xyz, -), a ref >= 0 naming an internal node and a ref
+ *                  < 0 the leaf -1 - ((start << 4) | count); records inside a collapsed leaf are never written
+ *   root_ref_out   count: 0 (an internal root) or the leaf reference of a cloud of at most 8 points                    */
+int b200reg_index_tap(b200reg_ctx* ctx, int count, const float* const* xyz, const size_t* n, size_t stride_bytes, int on_device,
+                      uint32_t* const* keys_out, float* const* pts_out, int32_t* const* rank_out, float* const* tnodes_out,
+                      int32_t* root_ref_out);
+/* The stable LSD radix sort the index build, the voxel grid, the matcher and the radius search share, on `count` caller
+ * arrays of host (key, value) words in one batched call: keys_out[i] / vals_out[i] receive the n[i] pairs ordered by key,
+ * equal keys in input order.  key_bits 30 (three 10-bit passes: the order of the low 30 bits, the bits above ride
+ * along) or 32 (three 11-bit passes).  1 <= n[i] < 2^30, the most the sort's 30-bit tile counts hold.              */
+int b200reg_sort_tap(b200reg_ctx* ctx, int count, const uint32_t* const* keys, const uint32_t* const* vals, const int32_t* n,
+                     int key_bits, uint32_t* const* keys_out, uint32_t* const* vals_out);
 
 #ifdef __cplusplus
 }

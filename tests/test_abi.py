@@ -22,6 +22,8 @@ def test_header_symbols_are_exported():
         assert hasattr(lib, n), "include/b200reg.h declares %s but libb200reg.so does not export it" % n
     from b200reg.native import EXPORTS
     assert set(EXPORTS) <= set(names)
+    # the read-only taps of the parity tests are bound as well (index build, shared radix sort, matcher, LM controller)
+    assert {"b200reg_index_tap", "b200reg_sort_tap", "b200reg_match_tap", "b200reg_lm_step_tap"} <= set(EXPORTS)
 
 
 def test_no_gpu_means_loud_failure_not_fallback():
