@@ -116,6 +116,7 @@ EXPORTS = [
     "b200reg_allgather_results", "b200reg_radius_search", "b200reg_quatro_align_ex", "b200reg_quatro_solve_tap",
     "b200reg_ctx_set_lm_trace", "b200reg_lm_trace", "b200reg_ctx_set_loop_clouds", "b200reg_loop_clouds",
     "b200reg_match_tap", "b200reg_lm_step_tap", "b200reg_index_tap", "b200reg_sort_tap",
+    "b200reg_batch_submit_perform_loop_closure",
 ]
 ESTATE = -4  # B200REG_ESTATE
 # B200REG_CLOUD_*: the loop clouds (Context.set_loop_clouds / Context.loop_clouds)
@@ -150,6 +151,7 @@ def lib():
         _lib.b200reg_keyframes_cloud_size.restype = C.c_size_t
         _lib.b200reg_batch_submit_icp.restype = C.c_int64
         _lib.b200reg_batch_submit_loop_closure.restype = C.c_int64
+        _lib.b200reg_batch_submit_perform_loop_closure.restype = C.c_int64
         _lib.b200reg_batch_launch_count.restype = C.c_int64
     return _lib
 
@@ -692,6 +694,31 @@ class Batch:
         self._keep[t] = (res, qi)
         return t
 
+    def submit_perform_loop_closure(self, kf, query, closest=None, cfg=None):
+        """LoopClosure::performLoopClosure over the device keyframe store `kf` (Keyframes) for the query keyframes, as a job
+        that sees the store as it is now (keyframe count, corrected poses, clouds).  closest None: the job runs
+        fetchClosestKeyframeIdx itself with cfg's radius and time difference.  Returns a ticket; wait(t, want_quatro=True)
+        gives the Result and QuatroInfo arrays, byte for byte those of kf.perform_loop_closure(..., raw=True)."""
+        cfg = cfg or default_loop_config()
+        q = np.ascontiguousarray(query, np.int32)
+        cnt = len(q)
+        cl = None if closest is None else np.ascontiguousarray(closest, np.int32)
+        assert cl is None or len(cl) == cnt
+        res = (Result * cnt)()
+        qi = (QuatroInfo * cnt)()
+        t = lib().b200reg_batch_submit_perform_loop_closure(self.h, kf.h, cnt, q.ctypes.data_as(C.c_void_p),
+                                                            None if cl is None else cl.ctypes.data_as(C.c_void_p), C.byref(cfg), res, qi)
+        if t < 0:
+            _check(int(t))
+        self._keep[t] = (res, qi)
+        return t
+
+    def wait_all(self):
+        """Waits for every job in flight; their results are dropped (wait() per ticket keeps them)."""
+        rc = lib().b200reg_batch_wait_all(self.h)
+        self._keep.clear()
+        _check(rc)
+
     def wait(self, ticket, want_latency=False, want_quatro=False):
         lat = C.c_double()
         rc = lib().b200reg_batch_wait(self.h, C.c_int64(ticket), C.byref(lat))
@@ -710,8 +737,11 @@ class Keyframes:
         _check(lib().b200reg_keyframes_create(ctx.h, C.byref(self.h)))
 
     def destroy(self):
+        """Raises (and keeps the store) while batch-driver jobs that read it are in flight."""
         if self.h:
-            lib().b200reg_keyframes_destroy(self.ctx.h, self.h)
+            rc = lib().b200reg_keyframes_destroy(self.ctx.h, self.h)
+            if rc == ESTATE:
+                _check(rc)
             self.h = None
 
     def __len__(self):

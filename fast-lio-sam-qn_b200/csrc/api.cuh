@@ -8,6 +8,7 @@
 
 #include <cstddef>
 #include <cstdint>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -16,6 +17,8 @@
 #include "launchers.cuh"
 
 using namespace b200;
+
+struct KfJob;  // a batch-driver job over the keyframe store (api_keyframes.cu)
 
 namespace b200 {
 int fail(int code, const std::string& msg);  // sets b200reg_last_error() and returns code
@@ -182,6 +185,15 @@ int create_pair_clouds(b200reg_ctx* c, int count, const float* const* src_xyz, c
 int sorted_to_original(b200reg_ctx* c, const CloudDev& d, std::vector<int>& orig, std::vector<float4>* pts_out = nullptr);
 
 void lm_arena_free(b200reg_ctx* c);  // api_gicp.cu
+
+// b200reg_perform_loop_closure as a job of the batch driver (api_keyframes.cu; batch.cu runs it).  kf_job_create, on the
+// submitting thread, refuses what the synchronous call refuses, then copies the arguments, the store's state (keyframe
+// count, corrected poses, cloud pointers and sizes) and its latest ingest mark; the store counts the job as in flight
+// until the job object is released.  kf_job_run, on a worker, waits on its stream for that mark and runs the same
+// attempt as the synchronous call on the worker's context.
+int kf_job_create(b200reg_keyframes* kf, int device, int count, const int32_t* query_idx, const int32_t* closest_idx,
+                  const b200reg_loop_config* cfg, std::shared_ptr<KfJob>* out);
+int kf_job_run(b200reg_ctx* c, KfJob* j, b200reg_result* out, b200reg_quatro_info* quatro_out);
 
 // The stored LM trace belongs to the pairs of the last b200reg_gicp_align.  A caller that ran that solve on a subset of its
 // `count` pairs (solve pair k = its pair where[k]; `where` empty when no solve ran) renumbers it to its own pairs; the

@@ -1,8 +1,10 @@
 // api_keyframes.cu -- the C ABI around registration: the keyframe store, candidate search, sub-map assembly,
 // b200reg_perform_loop_closure and the loop factors.
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstring>
+#include <memory>
 
 #include "api.cuh"
 
@@ -14,12 +16,30 @@ struct KfSlab {
   float4* base = nullptr;
   size_t cap = 0, used = 0;  // points
 };
-struct b200reg_keyframes {
+// What a loop-closure attempt reads of the store.  The store keeps the live state; a job of the batch driver
+// (b200reg_batch_submit_perform_loop_closure) keeps a copy taken at submit.  Both read keyframes through this one shape.
+struct KfState {
   std::vector<float4*> pts;
   std::vector<int> n;
   std::vector<double> poses;   // 16 per keyframe, row-major
   std::vector<double> stamps;
+  int size() const { return (int)pts.size(); }
+};
+// The stream-ordered mark of the latest ingest: recorded on the ingesting context's stream after every add; a job's stream
+// waits for it before the job reads a keyframe.  A mark that a job still holds is never recorded again: the next add makes
+// a new one.
+struct IngestMark {
+  cudaEvent_t ev = nullptr;
+  ~IngestMark() {
+    if (ev) cudaEventDestroy(ev);
+  }
+};
+struct b200reg_keyframes {
+  KfState st;
   std::vector<KfSlab> slabs;
+  int device = 0;
+  std::shared_ptr<IngestMark> ingest;
+  std::atomic<int> jobs{0};  // batch-driver jobs that hold a copy of `st` and have not finished
 };
 constexpr size_t KF_SLAB_POINTS = (size_t)8 << 20;  // 8 Mi points = 128 MB per slab unless reserved otherwise
 
@@ -37,9 +57,32 @@ static int kf_alloc(b200reg_keyframes* kf, size_t n, size_t min_slab, float4** o
   return B200REG_OK;
 }
 
-static int assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
+// after the uploads of an add are queued on c's stream: mark them for the jobs that will read the new keyframe
+static int mark_ingest(b200reg_ctx* c, b200reg_keyframes* kf) {
+  // only this thread hands out marks, so a use count of 1 cannot grow under us: no job holds this mark
+  if (!kf->ingest || kf->ingest.use_count() > 1) {
+    std::shared_ptr<IngestMark> m(new IngestMark);
+    CU(cudaEventCreateWithFlags(&m->ev, cudaEventDisableTiming));
+    kf->ingest = m;
+  }
+  CU(cudaEventRecord(kf->ingest->ev, c->stream));
+  return B200REG_OK;
+}
+
+static int assemble_clouds(b200reg_ctx* c, const KfState& kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
                            const b200reg_loop_config* cfg, const int32_t* n_keyframes, bool keep_intensity, b200reg_cloud** src_out,
                            b200reg_cloud** dst_out);
+static int fetch_closest(b200reg_ctx* c, const KfState& kf, int count, const int32_t* query_idx, double radius, double tdiff,
+                         int32_t* closest_out);
+static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
+                                const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out);
+
+// the configuration ranges sub-map assembly refuses (nullptr: none), for the call itself and for a job's submit
+static const char* assembly_config_error(const b200reg_loop_config* cfg) {
+  if (2 * cfg->num_submap_keyframes + 1 > MAXSEG) return "num_submap_keyframes too large";
+  if (!(cfg->voxel_res > 0)) return "voxel_res must be positive";
+  return nullptr;
+}
 
 extern "C" {
 
@@ -59,12 +102,15 @@ void b200reg_default_loop_config(b200reg_loop_config* cfg) {
 int b200reg_keyframes_create(b200reg_ctx* c, b200reg_keyframes** out) {
   if (!c || !out) return fail(B200REG_EINVAL, "bad argument");
   *out = new b200reg_keyframes;
+  (*out)->device = c->device;
   return B200REG_OK;
 }
 
 int b200reg_keyframes_destroy(b200reg_ctx* c, b200reg_keyframes* kf) {
   if (!kf) return B200REG_OK;
   if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
+  if (kf->jobs.load() > 0)
+    return fail(B200REG_ESTATE, "batch-driver jobs that read this keyframe store are in flight; wait for them first");
   CU(cudaSetDevice(c->device));
   CU(cudaStreamSynchronize(c->stream));  // nothing in flight may still read a keyframe
   for (KfSlab& sl : kf->slabs) CU(cudaFree(sl.base));
@@ -84,7 +130,7 @@ int b200reg_keyframes_reserve(b200reg_ctx* c, b200reg_keyframes* kf, size_t n_po
   return B200REG_OK;
 }
 
-int b200reg_keyframes_size(const b200reg_keyframes* kf) { return kf ? (int)kf->pts.size() : 0; }
+int b200reg_keyframes_size(const b200reg_keyframes* kf) { return kf ? (int)kf->st.pts.size() : 0; }
 
 int b200reg_keyframes_add(b200reg_ctx* c, b200reg_keyframes* kf, const float* xyzi, size_t n, size_t stride_bytes, const double* pose16,
                           double timestamp) {
@@ -105,11 +151,15 @@ int b200reg_keyframes_add(b200reg_ctx* c, b200reg_keyframes* kf, const float* xy
     c->launches++;
     CU(cudaGetLastError());
   }
-  kf->pts.push_back(d);
-  kf->n.push_back((int)n);
-  kf->poses.insert(kf->poses.end(), pose16, pose16 + 16);
-  kf->stamps.push_back(timestamp);
-  return (int)kf->pts.size() - 1;
+  {
+    const int rc = mark_ingest(c, kf);
+    if (rc) return rc;
+  }
+  kf->st.pts.push_back(d);
+  kf->st.n.push_back((int)n);
+  kf->st.poses.insert(kf->st.poses.end(), pose16, pose16 + 16);
+  kf->st.stamps.push_back(timestamp);
+  return (int)kf->st.pts.size() - 1;
 }
 
 namespace {
@@ -168,33 +218,37 @@ int b200reg_keyframes_add_world(b200reg_ctx* c, b200reg_keyframes* kf, const flo
   launch_ingest_world(d_raw, (int)(stride_bytes / 4), (int)n, d_T, d_out, s);
   c->launches++;
   CU(cudaGetLastError());
+  {
+    const int rc = mark_ingest(c, kf);
+    if (rc) return rc;
+  }
   CU(cudaStreamSynchronize(s));  // Tinv lives on this stack frame; the caller's message buffer may go away
-  kf->pts.push_back(d_out);
-  kf->n.push_back((int)n);
-  kf->poses.insert(kf->poses.end(), P, P + 16);
-  kf->stamps.push_back(timestamp);
-  return (int)kf->pts.size() - 1;
+  kf->st.pts.push_back(d_out);
+  kf->st.n.push_back((int)n);
+  kf->st.poses.insert(kf->st.poses.end(), P, P + 16);
+  kf->st.stamps.push_back(timestamp);
+  return (int)kf->st.pts.size() - 1;
 }
 
 int b200reg_keyframes_get(b200reg_ctx* c, const b200reg_keyframes* kf, int idx, float* xyzi_out, double* pose16_out, double* ts_out) {
-  if (!c || !kf || idx < 0 || idx >= (int)kf->pts.size()) return fail(B200REG_EINVAL, "bad argument");
-  if (pose16_out) memcpy(pose16_out, &kf->poses[16 * (size_t)idx], 128);
-  if (ts_out) *ts_out = kf->stamps[idx];
+  if (!c || !kf || idx < 0 || idx >= (int)kf->st.pts.size()) return fail(B200REG_EINVAL, "bad argument");
+  if (pose16_out) memcpy(pose16_out, &kf->st.poses[16 * (size_t)idx], 128);
+  if (ts_out) *ts_out = kf->st.stamps[idx];
   if (xyzi_out) {
     CU(cudaSetDevice(c->device));
-    CU(cudaMemcpyAsync(xyzi_out, kf->pts[idx], (size_t)kf->n[idx] * 16, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(xyzi_out, kf->st.pts[idx], (size_t)kf->st.n[idx] * 16, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
   }
   return B200REG_OK;
 }
 
 size_t b200reg_keyframes_cloud_size(const b200reg_keyframes* kf, int idx) {
-  return (kf && idx >= 0 && idx < (int)kf->n.size()) ? (size_t)kf->n[idx] : 0;
+  return (kf && idx >= 0 && idx < (int)kf->st.n.size()) ? (size_t)kf->st.n[idx] : 0;
 }
 
 int b200reg_keyframes_set_pose(b200reg_ctx* c, b200reg_keyframes* kf, int idx, const double* pose16) {
-  if (!c || !kf || !pose16 || idx < 0 || idx >= (int)kf->pts.size()) return fail(B200REG_EINVAL, "bad argument");
-  memcpy(&kf->poses[16 * (size_t)idx], pose16, 128);
+  if (!c || !kf || !pose16 || idx < 0 || idx >= (int)kf->st.pts.size()) return fail(B200REG_EINVAL, "bad argument");
+  memcpy(&kf->st.poses[16 * (size_t)idx], pose16, 128);
   return B200REG_OK;
 }
 
@@ -262,7 +316,7 @@ int b200reg_loop_factor_from_poses(const double* Tb, const double* Pl, const dou
 int b200reg_loop_factors(b200reg_ctx* c, const b200reg_keyframes* kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
                          const b200reg_result* results, b200reg_loop_factor* out) {
   if (!c || !kf || count <= 0 || !query_idx || !closest_idx || !results || !out) return fail(B200REG_EINVAL, "bad argument");
-  const int nk = (int)kf->pts.size();
+  const int nk = (int)kf->st.pts.size();
   for (int i = 0; i < count; i++) {
     if (query_idx[i] < 0 || query_idx[i] >= nk || closest_idx[i] >= nk) return fail(B200REG_EINVAL, "keyframe index out of range");
     if (closest_idx[i] < 0) {  // no candidate: the reference returns before any registration (fast_lio_sam_qn.cpp:213-216)
@@ -271,7 +325,7 @@ int b200reg_loop_factors(b200reg_ctx* c, const b200reg_keyframes* kf, int count,
       out[i].to_idx = -1;
       continue;
     }
-    const int rc = b200reg_loop_factor_from_poses(results[i].pose_between, &kf->poses[16 * (size_t)query_idx[i]], &kf->poses[16 * (size_t)closest_idx[i]],
+    const int rc = b200reg_loop_factor_from_poses(results[i].pose_between, &kf->st.poses[16 * (size_t)query_idx[i]], &kf->st.poses[16 * (size_t)closest_idx[i]],
                                                   results[i].fitness, results[i].valid, query_idx[i], closest_idx[i], &out[i]);
     if (rc) return rc;
   }
@@ -281,7 +335,28 @@ int b200reg_loop_factors(b200reg_ctx* c, const b200reg_keyframes* kf, int count,
 int b200reg_fetch_closest_keyframes(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* query_idx, double radius,
                                     double tdiff, int32_t* closest_out) {
   if (!c || !kf || count <= 0 || !query_idx || !closest_out) return fail(B200REG_EINVAL, "bad argument");
-  const int nk = (int)kf->pts.size();
+  return fetch_closest(c, kf->st, count, query_idx, radius, tdiff, closest_out);
+}
+
+int b200reg_assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
+                            const b200reg_loop_config* cfg, int n_keyframes, b200reg_cloud** src_out, b200reg_cloud** dst_out) {
+  if (!kf || count <= 0) return fail(B200REG_EINVAL, "bad argument");
+  std::vector<int32_t> nks(count, n_keyframes > 0 ? n_keyframes : (int)kf->st.pts.size());
+  return b200reg_assemble_clouds_at(c, kf, count, src_idx, dst_idx, cfg, nks.data(), src_out, dst_out);
+}
+
+int b200reg_assemble_clouds_at(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
+                               const b200reg_loop_config* cfg, const int32_t* n_keyframes, b200reg_cloud** src_out,
+                               b200reg_cloud** dst_out) {
+  if (!kf) return fail(B200REG_EINVAL, "bad argument");
+  return assemble_clouds(c, kf->st, count, src_idx, dst_idx, cfg, n_keyframes, false, src_out, dst_out);
+}
+
+}  // extern "C"
+
+static int fetch_closest(b200reg_ctx* c, const KfState& kf, int count, const int32_t* query_idx, double radius, double tdiff,
+                         int32_t* closest_out) {
+  const int nk = kf.size();
   for (int i = 0; i < count; i++)
     if (query_idx[i] < 0 || query_idx[i] >= nk) return fail(B200REG_EINVAL, "query index out of range");
   CU(cudaSetDevice(c->device));
@@ -289,11 +364,11 @@ int b200reg_fetch_closest_keyframes(b200reg_ctx* c, b200reg_keyframes* kf, int c
   Scratch scratch(c);
   std::vector<double> pos(3 * (size_t)nk);
   for (int i = 0; i < nk; i++)
-    for (int d = 0; d < 3; d++) pos[3 * (size_t)i + d] = kf->poses[16 * (size_t)i + 4 * d + 3];
+    for (int d = 0; d < 3; d++) pos[3 * (size_t)i + d] = kf.poses[16 * (size_t)i + 4 * d + 3];
   double *d_pos = nullptr, *d_st = nullptr;
   int *d_q = nullptr, *d_o = nullptr;
   CU(scratch.upload(&d_pos, pos.data(), pos.size() * 8));
-  CU(scratch.upload(&d_st, kf->stamps.data(), (size_t)nk * 8));
+  CU(scratch.upload(&d_st, kf.stamps.data(), (size_t)nk * 8));
   CU(scratch.upload(&d_q, query_idx, (size_t)count * 4));
   CU(scratch.alloc((void**)&d_o, (size_t)count * 4));
   c->launches += launch_fetch_closest(d_pos, d_st, d_q, count, radius, tdiff, d_o, s);
@@ -302,32 +377,16 @@ int b200reg_fetch_closest_keyframes(b200reg_ctx* c, b200reg_keyframes* kf, int c
   return B200REG_OK;
 }
 
-int b200reg_assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
-                            const b200reg_loop_config* cfg, int n_keyframes, b200reg_cloud** src_out, b200reg_cloud** dst_out) {
-  if (!kf || count <= 0) return fail(B200REG_EINVAL, "bad argument");
-  std::vector<int32_t> nks(count, n_keyframes > 0 ? n_keyframes : (int)kf->pts.size());
-  return b200reg_assemble_clouds_at(c, kf, count, src_idx, dst_idx, cfg, nks.data(), src_out, dst_out);
-}
-
-int b200reg_assemble_clouds_at(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
-                               const b200reg_loop_config* cfg, const int32_t* n_keyframes, b200reg_cloud** src_out,
-                               b200reg_cloud** dst_out) {
-  return assemble_clouds(c, kf, count, src_idx, dst_idx, cfg, n_keyframes, false, src_out, dst_out);
-}
-
-}  // extern "C"
-
 // b200reg_assemble_clouds_at; keep_intensity: the clouds keep the voxel-mean intensities (b200reg_cloud::inten)
-static int assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
+static int assemble_clouds(b200reg_ctx* c, const KfState& kf, int count, const int32_t* src_idx, const int32_t* dst_idx,
                            const b200reg_loop_config* cfg, const int32_t* n_keyframes, bool keep_intensity, b200reg_cloud** src_out,
                            b200reg_cloud** dst_out) {
-  if (!c || !kf || count <= 0 || !src_idx || !dst_idx || !cfg || !n_keyframes || !src_out || !dst_out)
+  if (!c || count <= 0 || !src_idx || !dst_idx || !cfg || !n_keyframes || !src_out || !dst_out)
     return fail(B200REG_EINVAL, "bad argument");
   for (int i = 0; i < count; i++)
-    if (n_keyframes[i] <= 0 || n_keyframes[i] > (int)kf->pts.size()) return fail(B200REG_EINVAL, "n_keyframes out of range");
+    if (n_keyframes[i] <= 0 || n_keyframes[i] > kf.size()) return fail(B200REG_EINVAL, "n_keyframes out of range");
+  if (const char* e = assembly_config_error(cfg)) return fail(B200REG_EINVAL, e);
   const int range = cfg->num_submap_keyframes;
-  if (2 * range + 1 > MAXSEG) return fail(B200REG_EINVAL, "num_submap_keyframes too large");
-  if (!(cfg->voxel_res > 0)) return fail(B200REG_EINVAL, "voxel_res must be positive");
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Scratch scratch(c);
@@ -350,12 +409,12 @@ static int assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, con
       for (int i = centre - range; i < centre + range + 1; i++)
         if (i >= 0 && i < nk - 1) {  // the reference excludes the last keyframe (loop_closure.cpp:72,79,100)
           J.seg_kf[J.nseg] = i;
-          J.seg_off[J.nseg + 1] = J.seg_off[J.nseg] + kf->n[i];
+          J.seg_off[J.nseg + 1] = J.seg_off[J.nseg] + kf.n[i];
           J.nseg++;
         }
     } else {
       J.seg_kf[0] = centre;
-      J.seg_off[1] = kf->n[centre];
+      J.seg_off[1] = kf.n[centre];
       J.nseg = 1;
     }
     J.total = J.seg_off[J.nseg];
@@ -387,9 +446,9 @@ static int assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, con
     sd.hist = J.sort.hist;
     max_total = std::max(max_total, J.total);
   }
-  const int nkall = (int)kf->pts.size();
+  const int nkall = kf.size();
   std::vector<KeyframeDev> kd(nkall);
-  for (int i = 0; i < nkall; i++) kd[i] = KeyframeDev{kf->pts[i], kf->n[i], 0};
+  for (int i = 0; i < nkall; i++) kd[i] = KeyframeDev{kf.pts[i], kf.n[i], 0};
   AssembleJob* d_jobs = nullptr;
   CloudDev* d_sorts = nullptr;
   KeyframeDev* d_kf = nullptr;
@@ -397,7 +456,7 @@ static int assemble_clouds(b200reg_ctx* c, b200reg_keyframes* kf, int count, con
   CU(scratch.upload(&d_jobs, jobs.data(), sizeof(AssembleJob) * njobs));
   CU(scratch.upload(&d_sorts, sorts.data(), sizeof(CloudDev) * njobs));
   CU(scratch.upload(&d_kf, kd.data(), sizeof(KeyframeDev) * nkall));
-  CU(scratch.upload(&d_poses, kf->poses.data(), 128 * (size_t)nkall));
+  CU(scratch.upload(&d_poses, kf.poses.data(), 128 * (size_t)nkall));
   {
     ProfScope ps(c, CLS_MISC);
     const float inv_leaf = 1.0f / (float)cfg->voxel_res;
@@ -430,6 +489,14 @@ extern "C" {
 int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
                                  const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out) {
   if (!c || !kf || count <= 0 || !query_idx || !closest_idx || !cfg || !out) return fail(B200REG_EINVAL, "bad argument");
+  return perform_loop_closure(c, kf->st, count, query_idx, closest_idx, cfg, out, quatro_out);
+}
+
+}  // extern "C"
+
+// b200reg_perform_loop_closure on a view of the store: the live one, or a batch-driver job's copy
+static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
+                                const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out) {
   LoopCapture cap(c, count);
   std::vector<int32_t> qs, cs;
   std::vector<int> where;
@@ -476,4 +543,58 @@ int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int coun
   return rc;
 }
 
-}  // extern "C"
+// ---- b200reg_perform_loop_closure as a job of the batch driver (batch.cu) ------------------------------------------
+struct KfJob {
+  b200reg_keyframes* kf;
+  KfState st;                         // the store at submit
+  std::shared_ptr<IngestMark> ingest;  // the last add before submit (null: nothing was ever added)
+  std::vector<int32_t> query, closest;  // closest empty: the job runs fetchClosestKeyframeIdx first
+  b200reg_loop_config cfg;
+  explicit KfJob(b200reg_keyframes* k) : kf(k) { kf->jobs++; }
+  ~KfJob() { kf->jobs--; }
+};
+
+namespace b200 {
+
+int kf_job_create(b200reg_keyframes* kf, int device, int count, const int32_t* query_idx, const int32_t* closest_idx,
+                  const b200reg_loop_config* cfg, std::shared_ptr<KfJob>* out) {
+  if (!kf || count <= 0 || !query_idx || !cfg || !out) return fail(B200REG_EINVAL, "bad argument");
+  if (kf->device != device) return fail(B200REG_EINVAL, "the keyframe store lives on another device than the batch driver");
+  // what the synchronous call refuses: b200reg_fetch_closest_keyframes checks every query, assembly every pair with a
+  // candidate (the query's keyframe count q + 1 must exist and hold the candidate)
+  const int nk = kf->st.size();
+  for (int i = 0; i < count; i++) {
+    const int q = query_idx[i];
+    if (!closest_idx && (q < 0 || q >= nk)) return fail(B200REG_EINVAL, "query index out of range");
+    if (closest_idx && closest_idx[i] >= 0 && (q < 0 || q >= nk || closest_idx[i] > q))
+      return fail(B200REG_EINVAL, "keyframe index out of range");
+  }
+  if (const char* e = assembly_config_error(cfg)) return fail(B200REG_EINVAL, e);
+  std::shared_ptr<KfJob> j(new KfJob(kf));
+  j->st = kf->st;
+  j->ingest = kf->ingest;
+  j->query.assign(query_idx, query_idx + count);
+  if (closest_idx) j->closest.assign(closest_idx, closest_idx + count);
+  j->cfg = *cfg;
+  *out = std::move(j);
+  return B200REG_OK;
+}
+
+int kf_job_run(b200reg_ctx* c, KfJob* j, b200reg_result* out, b200reg_quatro_info* quatro_out) {
+  CU(cudaSetDevice(c->device));
+  if (j->ingest) CU(cudaStreamWaitEvent(c->stream, j->ingest->ev, 0));  // the adds' uploads land before any read
+  const int count = (int)j->query.size();
+  int rc = B200REG_OK;
+  if (j->closest.empty()) {
+    j->closest.resize(count);
+    rc = fetch_closest(c, j->st, count, j->query.data(), j->cfg.loop_detection_radius, j->cfg.loop_detection_timediff_threshold,
+                       j->closest.data());
+  }
+  if (!rc) rc = perform_loop_closure(c, j->st, count, j->query.data(), j->closest.data(), &j->cfg, out, quatro_out);
+  // a failed call may return with its kernels still queued: none may read a keyframe once the job counts as finished
+  const cudaError_t e = cudaStreamSynchronize(c->stream);
+  if (!rc && e != cudaSuccess) rc = fail(B200REG_ECUDA, std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e));
+  return rc;
+}
+
+}  // namespace b200

@@ -1,7 +1,8 @@
 // batch.cu -- the batch driver of the C ABI (include/b200reg.h, "b200reg_batch_*"): `depth` engine contexts, each on its
 // own host thread with its own CUDA streams and memory pool, take alternate jobs.  While one context waits for a PCIe
 // upload or polls its LM loop, the kernels of the others keep the SMs busy -- the batch-level concurrency SURVEY.md §8(d)
-// names as the lever for the HBM fraction.  Host code only; everything it calls is the public C ABI.
+// names as the lever for the HBM fraction.  Host code only; everything it calls is the public C ABI, except the jobs over
+// the keyframe store, which go through the job interface of api_keyframes.cu (api.cuh).
 //
 // Reference context: the reference registers ONE pair per 2 Hz timer tick, serially, on one thread
 // (fast_lio_sam_qn/src/fast_lio_sam_qn.cpp:203-219, LoopClosure is not re-entrant, :81).
@@ -16,12 +17,12 @@
 #include <thread>
 #include <vector>
 
-#include "../../include/b200reg.h"
+#include "api.cuh"
 
 namespace {
 
 struct Job {
-  int kind = 0;  // 0 icpAlignment, 1 coarseToFineAlignment
+  int kind = 0;  // 0 icpAlignment, 1 coarseToFineAlignment, 2 performLoopClosure over a keyframe store
   int count = 0;
   std::vector<const float*> src, tgt;
   std::vector<size_t> src_n, tgt_n;
@@ -29,6 +30,7 @@ struct Job {
   int on_device = 0;
   b200reg_gicp_params gp;
   b200reg_quatro_params qp;
+  std::shared_ptr<KfJob> kfjob;  // kind 2: its arguments and the store's state at submit
   b200reg_result* out = nullptr;
   b200reg_quatro_info* qout = nullptr;
   // completion
@@ -75,9 +77,12 @@ static void run_worker(b200reg_batch* b, Worker* w) {
     if (j->kind == 0)
       rc = b200reg_icp_alignment(w->ctx, j->count, j->src.data(), j->src_n.data(), j->tgt.data(), j->tgt_n.data(), j->stride, j->on_device,
                                  &j->gp, j->out);
-    else
+    else if (j->kind == 1)
       rc = b200reg_loop_closure(w->ctx, j->count, j->src.data(), j->src_n.data(), j->tgt.data(), j->tgt_n.data(), j->stride, j->on_device,
                                 &j->qp, &j->gp, j->out, j->qout);
+    else
+      rc = kf_job_run(w->ctx, j->kfjob.get(), j->out, j->qout);
+    j->kfjob.reset();  // the store no longer counts the job as in flight: a wait that returns sees it finished
     {
       std::lock_guard<std::mutex> lk(b->mu);
       j->status = rc;
@@ -178,6 +183,20 @@ int64_t b200reg_batch_submit_loop_closure(b200reg_batch* b, int count, const flo
   j->qp = *qparams;
   j->out = out;
   j->qout = quatro_out;
+  return submit(b, j);
+}
+
+int64_t b200reg_batch_submit_perform_loop_closure(b200reg_batch* b, b200reg_keyframes* kf, int count, const int32_t* query_idx,
+                                                  const int32_t* closest_idx, const b200reg_loop_config* cfg, b200reg_result* out,
+                                                  b200reg_quatro_info* quatro_out) {
+  if (!b || !out) return fail(B200REG_EINVAL, "bad argument");
+  std::shared_ptr<Job> j(new Job);
+  j->kind = 2;
+  j->count = count;
+  j->out = out;
+  j->qout = quatro_out;
+  const int rc = kf_job_create(kf, b->device, count, query_idx, closest_idx, cfg, &j->kfjob);
+  if (rc) return rc;
   return submit(b, j);
 }
 

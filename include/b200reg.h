@@ -426,6 +426,29 @@ int64_t b200reg_batch_submit_loop_closure(b200reg_batch* b, int count, const flo
                                           int on_device, const b200reg_quatro_params* qparams,
                                           const b200reg_gicp_params* gparams, b200reg_result* out,
                                           b200reg_quatro_info* quatro_out);
+/* LoopClosure::performLoopClosure for `count` query keyframes of the device keyframe store, as a job of the batch driver:
+ * loopTimerFunc off the caller's thread, its stages overlapping those of other jobs.  closest_idx NULL: the job runs
+ * fetchClosestKeyframeIdx itself first, with cfg's loop_detection_radius and loop_detection_timediff_threshold.
+ *   Same bytes: a job writes the same b200reg_result and b200reg_quatro_info records, byte for byte, as
+ *     b200reg_perform_loop_closure on the same store state, queries and config, at every driver depth; a NULL closest_idx
+ *     answers as b200reg_fetch_closest_keyframes followed by that call.
+ *   Snapshot at submit: the job sees the store as it is when it is submitted -- the keyframe count, the corrected poses,
+ *     the clouds.  Keyframes added and poses rewritten (b200reg_keyframes_set_pose) after the submit do not change its
+ *     answer.  The uploads of earlier adds are ordered before the job's reads on the device (an event per add, waited
+ *     for by the job's stream); the submitting thread does not block on them.
+ *   Lifetime: b200reg_keyframes_destroy on a store that jobs still read returns B200REG_ESTATE and frees nothing; after
+ *     their b200reg_batch_wait (or _wait_all) it behaves as before.
+ *   Errors: refused at submit with B200REG_EINVAL, as b200reg_perform_loop_closure refuses them: count <= 0 (count = 0
+ *     too), NULL query_idx / cfg / out, a query outside the store (every query when closest_idx is NULL, else every one
+ *     with a candidate), a candidate above its query, num_submap_keyframes or voxel_res out of range, and a store on
+ *     another device than the driver.  Everything else (Quatro and GICP parameter refusals, device failures) comes back
+ *     from b200reg_batch_wait with its message.
+ *   Threads: submits, keyframe adds and pose rewrites of a store that jobs read come from ONE host thread.  Loop-cloud
+ *     capture and LM tracing belong to a caller's context and are not available on driver jobs.                      */
+int64_t b200reg_batch_submit_perform_loop_closure(b200reg_batch* b, b200reg_keyframes* kf, int count,
+                                                  const int32_t* query_idx, const int32_t* closest_idx,
+                                                  const b200reg_loop_config* cfg, b200reg_result* out,
+                                                  b200reg_quatro_info* quatro_out);
 /* Blocks until the job is done; returns ITS status (the message is then in b200reg_last_error of the calling thread).
  * latency_ms (optional): submit -> completion on the host clock.  A ticket can be waited for once.               */
 int b200reg_batch_wait(b200reg_batch* b, int64_t ticket, double* latency_ms);
