@@ -225,15 +225,18 @@ int b200::clouds_create(b200reg_ctx* c, int count, const float* const* xyz, cons
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Scratch scratch(c);
-  std::vector<CloudDev> descs(count);
+  std::vector<BuildDev> builds(count);
   int max_n = 0;
   for (int i = 0; i < count; i++) out[i] = nullptr;
   CloudBag bag(c);  // a failure half way must not leak the clouds already created
-  // sort work memory and AABB arrival flags of the whole batch: ONE allocation, ONE memset
-  std::vector<size_t> z_ws(count), z_fl(count);
+  // per cloud a temporary slab (sort buffers, tree scratch, bbox partials, and the raw records when uploading); the sort
+  // work memory and AABB arrival flags of the whole batch: ONE allocation, ONE memset
+  std::vector<Layout> tl(count);
+  std::vector<SortLayout> sl;
+  std::vector<size_t> z_fl(count);
   Layout zl;
   for (int i = 0; i < count; i++) {
-    z_ws[i] = zl.take(radix_sort_ws_bytes((int)n[i], 30));
+    sl.emplace_back(tl[i], zl, (int)n[i], 30);
     z_fl[i] = zl.take((size_t)std::max((int)n[i] - 1, 1) * 4);
   }
   char* zeroed = nullptr;
@@ -243,9 +246,9 @@ int b200::clouds_create(b200reg_ctx* c, int count, const float* const* xyz, cons
     b200reg_cloud* cl = new b200reg_cloud;
     bag.cl.push_back(cl);
     CloudDev& d = cl->dev;
+    d = CloudDev{};
     d.n = (int)n[i];
     d.root_ref = d.n <= LEAF ? leaf_ref(0, d.n) : 0;
-    d.raw_stride = (int)(stride_bytes / 4);
     const size_t nn = (size_t)std::max(d.n - 1, 1);
     // persistent slab
     Layout pl;
@@ -260,68 +263,48 @@ int b200::clouds_create(b200reg_ctx* c, int count, const float* const* xyz, cons
     d.tnodes = (float4*)(slab + o_tn);
     d.cov = (double*)(slab + o_cov);
     d.rank = (int*)(slab + o_rank);
-    d.nrm = nullptr;
-    d.spfh = nullptr;
-    d.fpfh = nullptr;
-    d.fproj = nullptr;
-    d.fpfh_s = nullptr;
-    d.fproj_s = nullptr;
-    d.ftile = nullptr;
-    d.fcode_s = nullptr;
-    // temporary slab (sort buffers, tree scratch, bbox partials, and the raw records when uploading)
-    Layout tl;
-    const size_t t_k0 = tl.take((size_t)d.n * 4), t_k1 = tl.take((size_t)d.n * 4), t_v0 = tl.take((size_t)d.n * 4),
-                 t_v1 = tl.take((size_t)d.n * 4), t_i = tl.take(nn * sizeof(int4)), t_pn = tl.take(nn * 4),
-                 t_pl = tl.take((size_t)d.n * 4), t_b = tl.take(6 * BBOX_BLOCKS * sizeof(float)),
-                 t_raw = tl.take(on_device ? 0 : (size_t)d.n * stride_bytes);
+    const size_t t_i = tl[i].take(nn * sizeof(int4)), t_pn = tl[i].take(nn * 4), t_pl = tl[i].take((size_t)d.n * 4),
+                 t_b = tl[i].take(6 * BBOX_BLOCKS * sizeof(float)), t_raw = tl[i].take(on_device ? 0 : (size_t)d.n * stride_bytes);
     char* tmp = nullptr;
-    CU(scratch.alloc((void**)&tmp, tl.size));
-    d.keys[0] = (uint32_t*)(tmp + t_k0);
-    d.keys[1] = (uint32_t*)(tmp + t_k1);
-    d.vals[0] = (uint32_t*)(tmp + t_v0);
-    d.vals[1] = (uint32_t*)(tmp + t_v1);
-    d.hist = (uint32_t*)(zeroed + z_ws[i]);
-    d.flags = (uint32_t*)(zeroed + z_fl[i]);
-    d.info = (int4*)(tmp + t_i);
-    d.parent_node = (int*)(tmp + t_pn);
-    d.parent_leaf = (int*)(tmp + t_pl);
-    d.bbox = (float*)(tmp + t_b);
+    CU(scratch.alloc((void**)&tmp, tl[i].size));
+    BuildDev& b = builds[i];
+    b.sort = sl[i].bind(tmp, zeroed);
+    b.raw_stride = (int)(stride_bytes / 4);
+    b.flags = (uint32_t*)(zeroed + z_fl[i]);
+    b.info = (int4*)(tmp + t_i);
+    b.parent_node = (int*)(tmp + t_pn);
+    b.parent_leaf = (int*)(tmp + t_pl);
+    b.bbox = (float*)(tmp + t_b);
+    b.pts = d.pts;
+    b.tnodes = d.tnodes;
+    b.rank = d.rank;
     if (on_device) {
-      d.raw = xyz[i];
+      b.raw = xyz[i];
     } else {
       CU(cudaMemcpyAsync(tmp + t_raw, xyz[i], (size_t)d.n * stride_bytes, cudaMemcpyHostToDevice, s));
-      d.raw = (const float*)(tmp + t_raw);
+      b.raw = (const float*)(tmp + t_raw);
     }
-    descs[i] = d;
     max_n = std::max(max_n, d.n);
   }
-  CloudDev* d_descs = nullptr;
-  CU(scratch.upload(&d_descs, descs.data(), sizeof(CloudDev) * count));
+  BuildDev* d_builds = nullptr;
+  CU(scratch.upload(&d_builds, builds.data(), sizeof(BuildDev) * count));
   {
     ProfScope ps(c, CLS_BUILD);
-    c->launches += launch_index_build(d_descs, count, max_n, s);
-    for (int i = 0; i < count; i++) c->prof_bytes[CLS_BUILD] += 36.0 * descs[i].n;  // SURVEY §8(d) K1
+    c->launches += launch_index_build(d_builds, count, max_n, s);
+    for (int i = 0; i < count; i++) c->prof_bytes[CLS_BUILD] += 36.0 * n[i];  // SURVEY §8(d) K1
   }
   CU(cudaGetLastError());
   if (keys_out)  // the sorted Morton keys, before the temporaries go (b200reg_index_tap)
     for (int i = 0; i < count; i++)
-      CU(cudaMemcpyAsync(keys_out[i], descs[i].keys[radix_sort_result_buf(30)], (size_t)descs[i].n * 4, cudaMemcpyDeviceToHost, s));
+      CU(cudaMemcpyAsync(keys_out[i], builds[i].sort.sorted_keys(), n[i] * 4, cudaMemcpyDeviceToHost, s));
   if (keep_intensity) {  // from the raw records, while they are still there
     std::vector<float*> inten(count);
     for (int i = 0; i < count; i++) inten[i] = bag.cl[i]->inten;
     float** d_inten = nullptr;
     CU(scratch.upload(&d_inten, inten.data(), sizeof(float*) * count));
-    launch_gather_intensity(d_descs, count, max_n, d_inten, s);
+    launch_gather_intensity(d_builds, count, max_n, d_inten, s);
     c->launches++;
     CU(cudaGetLastError());
-  }
-  for (b200reg_cloud* cl : bag.cl) {  // the temporaries are gone once the build has run
-    CloudDev& d = cl->dev;
-    d.raw = nullptr;
-    d.keys[0] = d.keys[1] = d.vals[0] = d.vals[1] = d.hist = d.flags = nullptr;
-    d.info = nullptr;
-    d.parent_node = d.parent_leaf = nullptr;
-    d.bbox = nullptr;
   }
   if (!on_device || keys_out) CU(cudaStreamSynchronize(s));  // host buffers have been consumed (or filled) when the call returns
   std::copy(bag.cl.begin(), bag.cl.end(), out);  // the caller owns the clouds from here on
@@ -531,40 +514,39 @@ int b200reg_radius_search(b200reg_ctx* c, const b200reg_cloud* cl, const float* 
   Scratch scratch(c);
   ProfScope ps(c, CLS_MISC);
   float* d_q = nullptr;
-  uint32_t *qk[2], *qv[2];
   int* d_cnt = nullptr;
   int64_t* d_off = nullptr;
-  char* d_ws = nullptr;  // zeroed sort work memory: query order, then (several chunks) chunk grouping
+  char *qb = nullptr, *qz = nullptr;
   void* d_scan = nullptr;
-  const size_t sort_ws = radix_sort_ws_bytes(n, 30);
+  // the query order's sort buffers and zeroed work memory: the query order, then (several chunks) the chunk grouping
+  Layout ql, qzl;
+  const SortLayout qsl(ql, qzl, n, 30, 2);
   CU(scratch.upload(&d_q, queries, nq * qstride_bytes));
-  for (int b = 0; b < 2; b++) {
-    CU(scratch.alloc((void**)&qk[b], nq * 4));
-    CU(scratch.alloc((void**)&qv[b], nq * 4));
-  }
+  CU(scratch.alloc((void**)&qb, ql.size));
   CU(scratch.alloc((void**)&d_cnt, nq * 4));
   CU(scratch.alloc((void**)&d_off, (nq + 1) * 8));
   CU(scratch.alloc((void**)&d_scan, radius_scan_ws_bytes(n)));
-  CU(scratch.alloc((void**)&d_ws, 2 * sort_ws));
-  CU(cudaMemsetAsync(d_ws, 0, 2 * sort_ws, s));
-  // Stable sort of (k0, v0) with k1 / v1 as the ping-pong halves; *out = whichever value buffer holds the result.  The radix
-  // sort reads its arrays through a device-side descriptor (only n / keys / vals / hist are used).
-  auto sort = [&](int m, uint32_t* k0, uint32_t* k1, uint32_t* v0, uint32_t* v1, void* hist, int key_bits, uint32_t** out) -> int {
-    CloudDev d = {};
-    d.n = m;
-    d.keys[0] = k0; d.keys[1] = k1;
-    d.vals[0] = v0; d.vals[1] = v1;
-    d.hist = (uint32_t*)hist;
-    CloudDev* dd = nullptr;
+  CU(scratch.alloc((void**)&qz, qzl.size));
+  CU(cudaMemsetAsync(qz, 0, qzl.size, s));
+  // Stable sort of (keys[0], vals[0]) through a device copy of the descriptor; *out = the value array of the result
+  auto sort = [&](const SortDev& d, int key_bits, uint32_t** out) -> int {
+    SortDev* dd = nullptr;
     CU(scratch.upload(&dd, &d, sizeof(d)));
-    c->launches += launch_radix_sort(dd, 1, m, key_bits, s);
-    *out = radix_sort_result_buf(key_bits) ? v1 : v0;
+    c->launches += launch_radix_sort(dd, 1, d.n, key_bits, s);
+    *out = d.sorted_vals();
     return B200REG_OK;
   };
+  // d for m entries; vin (a later sort over the same four arrays): the value array that holds its input, the other is spare
+  auto resort = [](SortDev d, int m, const uint32_t* vin) {
+    d.n = m;
+    if (vin && d.vals[0] != vin) std::swap(d.vals[0], d.vals[1]);
+    return d;
+  };
   // 1. queries in the cloud's Morton order, 2. counts, 3. offsets
-  c->launches += launch_radius_query_keys(cl->dev, d_q, n, qs, qk[0], qv[0], s);
+  const SortDev qord = qsl.bind(qb, qz);
   uint32_t* order = nullptr;
-  if (const int rc = sort(n, qk[0], qk[1], qv[0], qv[1], d_ws, 30, &order)) return rc;
+  c->launches += launch_radius_query_keys(cl->dev, d_q, n, qs, qord.keys[0], qord.vals[0], s);
+  if (const int rc = sort(qord, 30, &order)) return rc;
   c->launches += launch_radius_count(cl->dev, d_q, qs, order, n, r2, d_cnt, s);
   c->launches += launch_radius_scan(d_cnt, n, d_off, d_scan, s);
   CU(cudaGetLastError());
@@ -591,25 +573,23 @@ int b200reg_radius_search(b200reg_ctx* c, const b200reg_cloud* cl, const float* 
   if (nchunks > 1) {  // group the Morton-ordered queries by chunk (stable: Morton order inside each chunk)
     int* d_starts = nullptr;
     CU(scratch.upload(&d_starts, starts.data(), starts.size() * 4));
-    uint32_t* other = order == qv[0] ? qv[1] : qv[0];
-    c->launches += launch_radius_chunk_keys(order, n, d_starts, nchunks, qk[0], other, s);
-    if (const int rc = sort(n, qk[0], qk[1], other, order, d_ws + sort_ws, 30, &order)) return rc;
+    const SortDev g = resort(qsl.bind(qb, qz, 1), n, order == qord.vals[0] ? qord.vals[1] : qord.vals[0]);
+    c->launches += launch_radius_chunk_keys(order, n, d_starts, nchunks, g.keys[0], g.vals[0], s);
+    if (const int rc = sort(g, 30, &order)) return rc;
   }
-  // per chunk: entries, three sort passes' key / value ping-pong, three zeroed sort work areas
+  // per chunk: entries, the key / value ping-pong of three sorts, three zeroed sort work areas
   const size_t m = (size_t)max_entries;
   int* e_idx = nullptr;
   float* e_d2 = nullptr;
-  uint32_t *e_seg = nullptr, *K[2], *V[2];
-  char* ews = nullptr;
-  const size_t ews1 = radix_sort_ws_bytes((int)m, 32);
+  uint32_t* e_seg = nullptr;
+  char *eb = nullptr, *ez = nullptr;
+  Layout el, ezl;
+  const SortLayout esl(el, ezl, (int)m, 32, 3);
   CU(scratch.alloc((void**)&e_idx, m * 4));
   CU(scratch.alloc((void**)&e_d2, m * 4));
   CU(scratch.alloc((void**)&e_seg, m * 4));
-  for (int b = 0; b < 2; b++) {
-    CU(scratch.alloc((void**)&K[b], m * 4));
-    CU(scratch.alloc((void**)&V[b], m * 4));
-  }
-  CU(scratch.alloc((void**)&ews, 3 * ews1));
+  CU(scratch.alloc((void**)&eb, el.size));
+  CU(scratch.alloc((void**)&ez, ezl.size));
   for (int ci = 0; ci < nchunks; ci++) {
     RadiusChunk ch;
     ch.q0 = ch.r0 = starts[ci];
@@ -617,22 +597,25 @@ int b200reg_radius_search(b200reg_ctx* c, const b200reg_cloud* cl, const float* 
     ch.base = offsets_out[ch.q0];
     const int me = (int)(offsets_out[starts[ci + 1]] - ch.base);
     if (me == 0) continue;
-    ch.e_idx = e_idx; ch.e_d2 = e_d2; ch.e_seg = e_seg; ch.keys = K[0]; ch.vals = V[0];
-    CU(cudaMemsetAsync(ews, 0, 3 * ews1, s));
+    const SortDev byi = resort(esl.bind(eb, ez, 0), me, nullptr);
+    ch.e_idx = e_idx; ch.e_d2 = e_d2; ch.e_seg = e_seg; ch.keys = byi.keys[0]; ch.vals = byi.vals[0];
+    CU(cudaMemsetAsync(ez, 0, ezl.size, s));
     c->launches += launch_radius_fill(cl->dev, d_q, qs, order, r2, d_off, ch, s);
     // stable LSD passes: original index, (sorted) d2, query -> per query ascending index or ascending (d2, index)
     uint32_t* cur = nullptr;
-    if (const int rc = sort(me, K[0], K[1], V[0], V[1], ews, 30, &cur)) return rc;
+    if (const int rc = sort(byi, 30, &cur)) return rc;
     if (sorted) {  // d2 >= 0 and never NaN here: its bit pattern orders like the value
-      c->launches += launch_radius_rekey(cur, me, (const uint32_t*)e_d2, K[0], s);
-      if (const int rc = sort(me, K[0], K[1], cur, cur == V[0] ? V[1] : V[0], ews + ews1, 32, &cur)) return rc;
+      const SortDev byd = resort(esl.bind(eb, ez, 1), me, cur);
+      c->launches += launch_radius_rekey(cur, me, (const uint32_t*)e_d2, byd.keys[0], s);
+      if (const int rc = sort(byd, 32, &cur)) return rc;
     }
-    c->launches += launch_radius_rekey(cur, me, e_seg, K[0], s);
-    if (const int rc = sort(me, K[0], K[1], cur, cur == V[0] ? V[1] : V[0], ews + 2 * ews1, 30, &cur)) return rc;
-    c->launches += launch_radius_gather(cur, me, e_idx, e_d2, (int*)K[0], (float*)K[1], s);
+    const SortDev byq = resort(esl.bind(eb, ez, 2), me, cur);
+    c->launches += launch_radius_rekey(cur, me, e_seg, byq.keys[0], s);
+    if (const int rc = sort(byq, 30, &cur)) return rc;
+    c->launches += launch_radius_gather(cur, me, e_idx, e_d2, (int*)byq.keys[0], (float*)byq.keys[1], s);
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(idx_out + ch.base, K[0], (size_t)me * 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(d2_out + ch.base, K[1], (size_t)me * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(idx_out + ch.base, byq.keys[0], (size_t)me * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(d2_out + ch.base, byq.keys[1], (size_t)me * 4, cudaMemcpyDeviceToHost, s));
   }
   CU(cudaStreamSynchronize(s));
   return B200REG_OK;
@@ -704,35 +687,31 @@ int b200reg_sort_tap(b200reg_ctx* c, int count, const uint32_t* const* keys, con
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Scratch scratch(c);
-  std::vector<CloudDev> descs(count);
-  std::vector<size_t> o_ws(count);
-  Layout zl;
-  for (int i = 0; i < count; i++) o_ws[i] = zl.take(radix_sort_ws_bytes(n[i], key_bits));
-  char* zeroed = nullptr;
-  CU(scratch.alloc((void**)&zeroed, zl.size));
-  CU(cudaMemsetAsync(zeroed, 0, zl.size, s));
+  // the buffers of all sorts in one allocation, their work memory in another, zeroed by one memset
+  std::vector<SortLayout> sl;
+  Layout bl, zl;
   int max_n = 0;
   for (int i = 0; i < count; i++) {
-    CloudDev d = {};
-    d.n = n[i];
-    for (int b = 0; b < 2; b++) {
-      CU(scratch.alloc((void**)&d.keys[b], (size_t)n[i] * 4));
-      CU(scratch.alloc((void**)&d.vals[b], (size_t)n[i] * 4));
-    }
-    CU(cudaMemcpyAsync(d.keys[0], keys[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(d.vals[0], vals[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, s));
-    d.hist = (uint32_t*)(zeroed + o_ws[i]);
-    descs[i] = d;
-    max_n = std::max(max_n, d.n);
+    sl.emplace_back(bl, zl, n[i], key_bits);
+    max_n = std::max(max_n, (int)n[i]);
   }
-  CloudDev* d_descs = nullptr;
-  CU(scratch.upload(&d_descs, descs.data(), sizeof(CloudDev) * count));
-  c->launches += launch_radix_sort(d_descs, count, max_n, key_bits, s);
-  CU(cudaGetLastError());
-  const int r = radix_sort_result_buf(key_bits);
+  char *bufs = nullptr, *zeroed = nullptr;
+  CU(scratch.alloc((void**)&bufs, bl.size));
+  CU(scratch.alloc((void**)&zeroed, zl.size));
+  CU(cudaMemsetAsync(zeroed, 0, zl.size, s));
+  std::vector<SortDev> sorts(count);
   for (int i = 0; i < count; i++) {
-    CU(cudaMemcpyAsync(keys_out[i], descs[i].keys[r], (size_t)n[i] * 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(vals_out[i], descs[i].vals[r], (size_t)n[i] * 4, cudaMemcpyDeviceToHost, s));
+    sorts[i] = sl[i].bind(bufs, zeroed);
+    CU(cudaMemcpyAsync(sorts[i].keys[0], keys[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(sorts[i].vals[0], vals[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, s));
+  }
+  SortDev* d_sorts = nullptr;
+  CU(scratch.upload(&d_sorts, sorts.data(), sizeof(SortDev) * count));
+  c->launches += launch_radix_sort(d_sorts, count, max_n, key_bits, s);
+  CU(cudaGetLastError());
+  for (int i = 0; i < count; i++) {
+    CU(cudaMemcpyAsync(keys_out[i], sorts[i].sorted_keys(), (size_t)n[i] * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(vals_out[i], sorts[i].sorted_vals(), (size_t)n[i] * 4, cudaMemcpyDeviceToHost, s));
   }
   CU(cudaStreamSynchronize(s));
   return B200REG_OK;

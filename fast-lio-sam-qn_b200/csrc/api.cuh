@@ -166,6 +166,30 @@ struct Layout {
   }
 };
 
+// The buffers of a radix sort (SortDev) of n keys: keys[2] / vals[2] from `bufs`, the work memory from `zeroed`, a Layout
+// whose allocation the caller zeroes (it may be `bufs` itself).  `sorts` > 1 reserves one work area per sort that runs
+// over the same buffers; bind(..., k) gives the descriptor with area k.  Offsets first, pointers at bind().
+struct SortLayout {
+  int n;
+  size_t ws;  // bytes of one work area
+  size_t o_keys[2], o_vals[2], o_hist;
+  SortLayout(Layout& bufs, Layout& zeroed, int n_, int key_bits, int sorts = 1) : n(n_), ws(radix_sort_ws_bytes(n_, key_bits)) {
+    for (int b = 0; b < 2; b++) o_keys[b] = bufs.take((size_t)n * 4);
+    for (int b = 0; b < 2; b++) o_vals[b] = bufs.take((size_t)n * 4);
+    o_hist = zeroed.take(sorts * ws);
+  }
+  SortDev bind(char* bufs, char* zeroed, int k = 0) const {
+    SortDev d;
+    d.n = n;
+    for (int b = 0; b < 2; b++) {
+      d.keys[b] = (uint32_t*)(bufs + o_keys[b]);
+      d.vals[b] = (uint32_t*)(bufs + o_vals[b]);
+    }
+    d.hist = (uint32_t*)(zeroed + o_hist + k * ws);
+    return d;
+  }
+};
+
 // RegistrationOutput's defaults (loop_closure.h:64-70): identity transforms, score_ = DBL_MAX, not valid
 b200reg_result default_result();
 

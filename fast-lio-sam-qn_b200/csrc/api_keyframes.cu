@@ -392,7 +392,7 @@ static int assemble_clouds(b200reg_ctx* c, const KfState& kf, int count, const i
   Scratch scratch(c);
   const int njobs = 2 * count;  // jobs [0,count) = src clouds, [count, 2 count) = dst clouds
   std::vector<AssembleJob> jobs(njobs);
-  std::vector<CloudDev> sorts(njobs);
+  std::vector<SortDev> sorts(njobs);
   int max_total = 0;
   for (int j = 0; j < njobs; j++) {
     const bool is_src = j < count;
@@ -422,7 +422,7 @@ static int assemble_clouds(b200reg_ctx* c, const KfState& kf, int count, const i
     const size_t n = J.total;
     Layout l;
     const size_t o_m = l.take(n * 16), o_o = l.take(n * 16), o_h = l.take(n * 4), o_b = l.take(32), o_c = l.take(16);
-    const size_t o_k0 = l.take(n * 4), o_k1 = l.take(n * 4), o_v0 = l.take(n * 4), o_v1 = l.take(n * 4), o_hist = l.take(radix_sort_ws_bytes(J.total, 32));
+    const SortLayout sl(l, l, J.total, 32);
     char* slab = nullptr;
     CU(scratch.alloc((void**)&slab, l.size));
     J.merged = (float4*)(slab + o_m);
@@ -430,31 +430,19 @@ static int assemble_clouds(b200reg_ctx* c, const KfState& kf, int count, const i
     J.heads = (int*)(slab + o_h);
     J.bbox = (int*)(slab + o_b);
     J.counters = (int*)(slab + o_c);
-    J.sort.keys[0] = (uint32_t*)(slab + o_k0);
-    J.sort.keys[1] = (uint32_t*)(slab + o_k1);
-    J.sort.vals[0] = (uint32_t*)(slab + o_v0);
-    J.sort.vals[1] = (uint32_t*)(slab + o_v1);
-    J.sort.hist = (uint32_t*)(slab + o_hist);
-    CU(cudaMemsetAsync(J.sort.hist, 0, radix_sort_ws_bytes(J.total, 32), s));
-    CloudDev& sd = sorts[j];
-    memset(&sd, 0, sizeof(sd));
-    sd.n = J.total;
-    sd.keys[0] = J.sort.keys[0];
-    sd.keys[1] = J.sort.keys[1];
-    sd.vals[0] = J.sort.vals[0];
-    sd.vals[1] = J.sort.vals[1];
-    sd.hist = J.sort.hist;
+    sorts[j] = sl.bind(slab, slab);
+    CU(cudaMemsetAsync(sorts[j].hist, 0, sl.ws, s));
     max_total = std::max(max_total, J.total);
   }
   const int nkall = kf.size();
   std::vector<KeyframeDev> kd(nkall);
   for (int i = 0; i < nkall; i++) kd[i] = KeyframeDev{kf.pts[i], kf.n[i], 0};
   AssembleJob* d_jobs = nullptr;
-  CloudDev* d_sorts = nullptr;
+  SortDev* d_sorts = nullptr;
   KeyframeDev* d_kf = nullptr;
   double* d_poses = nullptr;
   CU(scratch.upload(&d_jobs, jobs.data(), sizeof(AssembleJob) * njobs));
-  CU(scratch.upload(&d_sorts, sorts.data(), sizeof(CloudDev) * njobs));
+  CU(scratch.upload(&d_sorts, sorts.data(), sizeof(SortDev) * njobs));
   CU(scratch.upload(&d_kf, kd.data(), sizeof(KeyframeDev) * nkall));
   CU(scratch.upload(&d_poses, kf.poses.data(), 128 * (size_t)nkall));
   {

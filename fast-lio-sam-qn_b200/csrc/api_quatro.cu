@@ -441,32 +441,25 @@ int b200reg_clouds_fpfh(b200reg_ctx* c, int count, b200reg_cloud* const* clouds,
     max_n = std::max(max_n, cl->dev.n);
   }
   if (todo.empty()) return B200REG_OK;
-  {  // sort buffers of the filter-code ordering (scratch: only this call uses them); the work memory of all clouds is one
-     // region, zeroed by one memset
-    Layout l;
-    std::vector<size_t> o_ws, o_k;
-    for (auto& d : descs) o_ws.push_back(l.take(radix_sort_ws_bytes(d.n, 32)));
-    const size_t ws_total = l.size;
-    for (auto& d : descs)
-      for (int b = 0; b < 4; b++) o_k.push_back(l.take((size_t)d.n * 4));
-    char* sb = nullptr;
-    CU(scratch.alloc((void**)&sb, l.size));
-    CU(cudaMemsetAsync(sb, 0, ws_total, s));
-    for (size_t i = 0; i < descs.size(); i++) {
-      CloudDev& d = descs[i];
-      d.hist = (uint32_t*)(sb + o_ws[i]);
-      d.keys[0] = (uint32_t*)(sb + o_k[4 * i]);
-      d.keys[1] = (uint32_t*)(sb + o_k[4 * i + 1]);
-      d.vals[0] = (uint32_t*)(sb + o_k[4 * i + 2]);
-      d.vals[1] = (uint32_t*)(sb + o_k[4 * i + 3]);
-    }
-  }
+  // sort buffers of the filter-code ordering (scratch: only this call uses them); the work memory of all clouds is one
+  // region, zeroed by one memset
+  std::vector<SortLayout> sl;
+  Layout bl, zl;
+  for (auto& d : descs) sl.emplace_back(bl, zl, d.n, 32);
+  char *sb = nullptr, *sz = nullptr;
+  CU(scratch.alloc((void**)&sb, bl.size));
+  CU(scratch.alloc((void**)&sz, zl.size));
+  CU(cudaMemsetAsync(sz, 0, zl.size, s));
+  std::vector<SortDev> sorts;
+  for (auto& x : sl) sorts.push_back(x.bind(sb, sz));
   CloudDev* d_descs = nullptr;
+  SortDev* d_sorts = nullptr;
   CU(scratch.upload(&d_descs, descs.data(), sizeof(CloudDev) * descs.size()));
+  CU(scratch.upload(&d_sorts, sorts.data(), sizeof(SortDev) * sorts.size()));
   {
     ProfScope ps(c, CLS_FPFH);
     const float nr2 = (float)(normal_radius * normal_radius), fr2 = (float)(fpfh_radius * fpfh_radius);
-    c->launches += launch_fpfh(d_descs, (int)descs.size(), max_n, nr2, fr2, s);
+    c->launches += launch_fpfh(d_descs, d_sorts, (int)descs.size(), max_n, nr2, fr2, s);
     for (auto& d : descs) c->prof_bytes[CLS_FPFH] += (32.0 + 164.0 + 280.0) * d.n;  // SURVEY §8(d) Q1+Q2+Q3
   }
   CU(cudaGetLastError());
@@ -623,14 +616,14 @@ int b200reg_match_tap(b200reg_ctx* c, int count, const float* const* fi, const i
   Scratch scratch(c);
   // cloud 2k = fi of pair k, 2k + 1 = its fj: the record tables b200reg_clouds_fpfh keeps, and the sort's temporaries
   std::vector<CloudDev> cl(2 * (size_t)count);
+  std::vector<SortDev> sorts(2 * (size_t)count);
   std::vector<MatchDev> pairs(count);
   Layout l;
   std::vector<size_t> o_c(2 * (size_t)count), o_p(count);
   auto cloud_bytes = [](size_t n) {
     Layout x;
-    for (size_t b : {n * FPAD * 4, n * 16, n * FPAD * 4, n * 16, 2 * ((n + 63) / 64) * 16, n * 4, n * 4, n * 4, n * 4, n * 4})
-      x.take(b);
-    x.take(radix_sort_ws_bytes((int)n, 32));
+    for (size_t b : {n * FPAD * 4, n * 16, n * FPAD * 4, n * 16, 2 * ((n + 63) / 64) * 16, n * 4}) x.take(b);
+    SortLayout(x, x, (int)n, 32);
     return x.size;
   };
   int max_n = 0, max_ni = 0, max_nj = 0;
@@ -656,13 +649,9 @@ int b200reg_match_tap(b200reg_ctx* c, int count, const float* const* fi, const i
     d.fproj_s = (float4*)(b + x.take(n * 16));
     d.ftile = (float4*)(b + x.take(2 * ((n + 63) / 64) * 16));
     d.fcode_s = (uint32_t*)(b + x.take(n * 4));
-    d.keys[0] = (uint32_t*)(b + x.take(n * 4));
-    d.keys[1] = (uint32_t*)(b + x.take(n * 4));
-    d.vals[0] = (uint32_t*)(b + x.take(n * 4));
-    d.vals[1] = (uint32_t*)(b + x.take(n * 4));
-    const size_t ws = radix_sort_ws_bytes((int)n, 32);
-    d.hist = (uint32_t*)(b + x.take(ws));
-    CU(cudaMemsetAsync(d.hist, 0, ws, s));
+    const SortLayout sl(x, x, (int)n, 32);
+    sorts[q] = sl.bind(b, b);
+    CU(cudaMemsetAsync(sorts[q].hist, 0, sl.ws, s));
     // the caller's rows into slots 0..32 of the record table; k_load_records completes the records in place
     CU(cudaMemcpy2DAsync(d.fpfh, FPAD * 4, q & 1 ? fj[q / 2] : fi[q / 2], FDIM * 4, FDIM * 4, n, cudaMemcpyHostToDevice, s));
   }
@@ -682,13 +671,15 @@ int b200reg_match_tap(b200reg_ctx* c, int count, const float* const* fi, const i
     m.stats = (double*)(p + (b * 20 + a * 8 + 32 + 63) / 64 * 64);
   }
   CloudDev* d_cl = nullptr;
+  SortDev* d_sorts = nullptr;
   MatchDev* d_pairs = nullptr;
   CU(scratch.upload(&d_cl, cl.data(), sizeof(CloudDev) * cl.size()));
+  CU(scratch.upload(&d_sorts, sorts.data(), sizeof(SortDev) * sorts.size()));
   CU(scratch.upload(&d_pairs, pairs.data(), sizeof(MatchDev) * count));
   {
     ProfScope ps(c, CLS_MATCH);
     c->launches += launch_load_records(d_cl, 2 * count, max_n, s);
-    c->launches += launch_feature_order(d_cl, 2 * count, max_n, s);
+    c->launches += launch_feature_order(d_cl, d_sorts, 2 * count, max_n, s);
     c->launches += launch_feature_match(d_pairs, count, max_ni, max_nj, match_thr2(distance_threshold, !!advanced), advanced ? 1 : 0, s);
   }
   CU(cudaGetLastError());

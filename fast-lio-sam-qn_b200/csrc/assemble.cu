@@ -84,8 +84,9 @@ __global__ void __launch_bounds__(256) k_assemble(const AssembleJob* jobs, const
 }
 
 // pcl::VoxelGrid first pass: idx = ijk0 + ijk1*dx + ijk2*dx*dy with ijk = floor(p * (1/L)) - float(min_b)
-__global__ void __launch_bounds__(256) k_voxel_keys(const AssembleJob* jobs, float inv_leaf) {
+__global__ void __launch_bounds__(256) k_voxel_keys(const AssembleJob* jobs, const SortDev* sorts, float inv_leaf) {
   const AssembleJob& J = jobs[blockIdx.y];
+  const SortDev& S = sorts[blockIdx.y];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= J.total) return;
   int min_b[3], div_b[3];
@@ -99,8 +100,8 @@ __global__ void __launch_bounds__(256) k_voxel_keys(const AssembleJob* jobs, flo
   }
   if (cells > 2147483647LL) {  // PCL: "Leaf size is too small ... Integer indices would overflow" -> input returned as is
     if (i == 0) J.counters[1] = 1;
-    J.sort.keys[0][i] = (uint32_t)i;
-    J.sort.vals[0][i] = (uint32_t)i;
+    S.keys[0][i] = (uint32_t)i;
+    S.vals[0][i] = (uint32_t)i;
     return;
   }
   // PCL keeps the index as unsigned int; div_b can exceed the guard's per-axis count by one, so the index can pass 2^31
@@ -109,18 +110,18 @@ __global__ void __launch_bounds__(256) k_voxel_keys(const AssembleJob* jobs, flo
   const uint32_t i0 = (uint32_t)(int)(floorf(p.x * inv_leaf) - (float)min_b[0]);
   const uint32_t i1 = (uint32_t)(int)(floorf(p.y * inv_leaf) - (float)min_b[1]);
   const uint32_t i2 = (uint32_t)(int)(floorf(p.z * inv_leaf) - (float)min_b[2]);
-  J.sort.keys[0][i] = i0 + i1 * (uint32_t)div_b[0] + i2 * ((uint32_t)div_b[0] * (uint32_t)div_b[1]);
-  J.sort.vals[0][i] = (uint32_t)i;
+  S.keys[0][i] = i0 + i1 * (uint32_t)div_b[0] + i2 * ((uint32_t)div_b[0] * (uint32_t)div_b[1]);
+  S.vals[0][i] = (uint32_t)i;
 }
 
 // ordered compaction of the run heads (one block per job); heads[v] = first sorted slot of voxel v
-__global__ void __launch_bounds__(1024) k_voxel_heads(const AssembleJob* jobs, int kbuf) {
+__global__ void __launch_bounds__(1024) k_voxel_heads(const AssembleJob* jobs, const SortDev* sorts) {
   const AssembleJob& J = jobs[blockIdx.x];
   __shared__ int wsum[32];
   __shared__ int carry;
   if (threadIdx.x == 0) carry = 0;
   __syncthreads();
-  const uint32_t* keys = J.sort.keys[kbuf];
+  const uint32_t* keys = sorts[blockIdx.x].sorted_keys();
   for (int base = 0; base < J.total; base += 1024) {
     const int i = base + threadIdx.x;
     const int head = (i < J.total && (i == 0 || keys[i] != keys[i - 1])) ? 1 : 0;
@@ -153,13 +154,13 @@ __global__ void __launch_bounds__(1024) k_voxel_heads(const AssembleJob* jobs, i
 }
 
 // centroid of x, y, z, intensity per voxel: fp32 running sums in sorted (= ascending point index) order
-__global__ void __launch_bounds__(256) k_voxel_centroid(const AssembleJob* jobs, int kbuf) {
+__global__ void __launch_bounds__(256) k_voxel_centroid(const AssembleJob* jobs, const SortDev* sorts) {
   const AssembleJob& J = jobs[blockIdx.y];
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   const int nv = J.counters[0];
   if (v >= nv) return;
   const int a = J.heads[v], b = v + 1 < nv ? J.heads[v + 1] : J.total;
-  const uint32_t* vals = J.sort.vals[kbuf];
+  const uint32_t* vals = sorts[blockIdx.y].sorted_vals();
   float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
   for (int j = a; j < b; j++) {
     const float4 p = J.merged[vals[j]];
@@ -194,10 +195,10 @@ __global__ void __launch_bounds__(256) k_pack_xyzi(const float* raw, int stride,
 }
 // Intensities of the raw records a cloud was built from, ORIGINAL order (clouds created inside a call that captures its loop
 // clouds): k_pack_xyzi's rule -- float 3 for 4..7-float records, float 4 from pcl::PointXYZI's 8 on -- and 0 for bare xyz
-__global__ void __launch_bounds__(256) k_gather_intensity(const CloudDev* clouds, float* const* inten) {
-  const CloudDev& c = clouds[blockIdx.y];
+__global__ void __launch_bounds__(256) k_gather_intensity(const BuildDev* builds, float* const* inten) {
+  const BuildDev& c = builds[blockIdx.y];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= c.n) return;
+  if (i >= c.sort.n) return;
   const float* p = c.raw + (size_t)i * c.raw_stride;
   inten[blockIdx.y][i] = c.raw_stride >= 8 ? p[4] : c.raw_stride >= 4 ? p[3] : 0.f;
 }
@@ -218,8 +219,8 @@ __global__ void __launch_bounds__(256) k_capture_rows(const CaptureRow* rows, in
   }
 }
 
-void launch_gather_intensity(const CloudDev* d_clouds, int count, int max_n, float* const* d_inten, cudaStream_t s) {
-  k_gather_intensity<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_clouds, d_inten);
+void launch_gather_intensity(const BuildDev* d_builds, int count, int max_n, float* const* d_inten, cudaStream_t s) {
+  k_gather_intensity<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_builds, d_inten);
 }
 
 void launch_capture_rows(const CaptureRow* d_rows, int nrows, int max_n, cudaStream_t s) {
@@ -240,17 +241,15 @@ int launch_fetch_closest(const double* d_pos, const double* d_stamp, const int* 
   return 1;
 }
 
-// d_sort: CloudDev descriptors whose n/keys/vals/hist alias the jobs' sort fields
-int launch_assemble_voxelize(const AssembleJob* d_jobs, const CloudDev* d_sort, int count, int max_total, const KeyframeDev* d_kfs,
+int launch_assemble_voxelize(const AssembleJob* d_jobs, const SortDev* d_sorts, int count, int max_total, const KeyframeDev* d_kfs,
                              const double* d_poses, float inv_leaf, cudaStream_t s) {
   int l = 0;
   k_assemble_init<<<count, 32, 0, s>>>(d_jobs); l++;
   k_assemble<<<dim3(min((max_total + 255) / 256, 1184), count), 256, 0, s>>>(d_jobs, d_kfs, d_poses); l++;
-  k_voxel_keys<<<dim3((max_total + 255) / 256, count), 256, 0, s>>>(d_jobs, inv_leaf); l++;
-  l += launch_radix_sort(d_sort, count, max_total, 32, s);  // voxel indices use up to 31 bits: 3 passes of 11 bits
-  const int kbuf = radix_sort_result_buf(32);
-  k_voxel_heads<<<count, 1024, 0, s>>>(d_jobs, kbuf); l++;
-  k_voxel_centroid<<<dim3((max_total + 255) / 256, count), 256, 0, s>>>(d_jobs, kbuf); l++;
+  k_voxel_keys<<<dim3((max_total + 255) / 256, count), 256, 0, s>>>(d_jobs, d_sorts, inv_leaf); l++;
+  l += launch_radix_sort(d_sorts, count, max_total, 32, s);  // voxel indices use up to 31 bits: 3 passes of 11 bits
+  k_voxel_heads<<<count, 1024, 0, s>>>(d_jobs, d_sorts); l++;
+  k_voxel_centroid<<<dim3((max_total + 255) / 256, count), 256, 0, s>>>(d_jobs, d_sorts); l++;
   return l;
 }
 

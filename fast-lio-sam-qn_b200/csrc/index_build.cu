@@ -27,10 +27,10 @@ namespace b200 {
 // ------------------------------------------------------------------------------------
 // bounding box: per-block partials, reduced again by every block of the next kernel
 // ------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_bbox(const CloudDev* clouds) {
-  const CloudDev& c = clouds[blockIdx.y];
+__global__ void __launch_bounds__(256) k_bbox(const BuildDev* builds) {
+  const BuildDev& c = builds[blockIdx.y];
   float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < c.n; i += gridDim.x * blockDim.x) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < c.sort.n; i += gridDim.x * blockDim.x) {
     const float* p = c.raw + (size_t)i * c.raw_stride;
 #pragma unroll
     for (int d = 0; d < 3; d++) {
@@ -65,11 +65,10 @@ __global__ void __launch_bounds__(256) k_bbox(const CloudDev* clouds) {
 // ------------------------------------------------------------------------------------
 // stable LSD radix sort with one kernel per pass
 // ------------------------------------------------------------------------------------
-// Work memory of one sort (CloudDev::hist, ZERO-INITIALISED by the caller), in 32-bit words:
+// Work memory of one sort (SortDev::hist, ZERO-INITIALISED by the caller), in 32-bit words:
 //   [0, P*R)                  global digit histograms of the P passes (R = 2^BITS bins)
 //   [P*R, P*R + 32)           tile tickets, one per pass
 //   [P*R + 32 + p*T*R ...)    look-back words of pass p: T tiles x R digits, (flag << 30) | count
-constexpr int SORT_PASSES = 3;
 constexpr uint32_t LB_AGG = 1u << 30, LB_INC = 2u << 30, LB_MASK = (1u << 30) - 1u;
 
 __host__ __device__ inline int sort_tiles(int n) { return (n + SORT_TILE - 1) / SORT_TILE; }
@@ -78,7 +77,6 @@ __host__ __device__ inline size_t sort_ws_words(int n) {
   return (size_t)SORT_PASSES * (1 << BITS) + 32 + (size_t)SORT_PASSES * sort_tiles(n) * (1 << BITS);
 }
 size_t radix_sort_ws_bytes(int n, int key_bits) { return 4 * (key_bits <= 30 ? sort_ws_words<10>(n) : sort_ws_words<11>(n)); }
-int radix_sort_result_buf(int) { return SORT_PASSES & 1; }
 
 // block-wide accumulation of the digit histograms of all passes (shared by the fused Morton kernel and k_sort_ghist)
 template <int BITS>
@@ -101,10 +99,10 @@ struct GHist {
 };
 
 // bbox partials -> Morton keys (cubic cells) + sort histograms.  Grid: (tiles of SORT_TILE points, cloud).
-__global__ void __launch_bounds__(SORT_THREADS) k_morton_ghist(const CloudDev* clouds, int bbox_blocks) {
-  const CloudDev& c = clouds[blockIdx.y];
+__global__ void __launch_bounds__(SORT_THREADS) k_morton_ghist(const BuildDev* builds, int bbox_blocks) {
+  const BuildDev& c = builds[blockIdx.y];
   const int base = blockIdx.x * SORT_TILE;
-  if (base >= c.n) return;
+  if (base >= c.sort.n) return;
   __shared__ uint32_t sh[SORT_PASSES * 1024];
   __shared__ float s_box[6];
   GHist<10> gh{sh};
@@ -133,25 +131,25 @@ __global__ void __launch_bounds__(SORT_THREADS) k_morton_ghist(const CloudDev* c
 #pragma unroll
   for (int j = 0; j < SORT_ITEMS; j++) {
     const int i = base + j * SORT_THREADS + threadIdx.x;
-    if (i < c.n) {
+    if (i < c.sort.n) {
       const float* p = c.raw + (size_t)i * c.raw_stride;
       const uint32_t q0 = (uint32_t)min(max((int)((p[0] - lo0) * scale), 0), 1023);
       const uint32_t q1 = (uint32_t)min(max((int)((p[1] - lo1) * scale), 0), 1023);
       const uint32_t q2 = (uint32_t)min(max((int)((p[2] - lo2) * scale), 0), 1023);
       const uint32_t key = (expand10(q2) << 2) | (expand10(q1) << 1) | expand10(q0);
-      c.keys[0][i] = key;
-      c.vals[0][i] = (uint32_t)i;
+      c.sort.keys[0][i] = key;
+      c.sort.vals[0][i] = (uint32_t)i;
       gh.add(key);
     }
   }
   __syncthreads();
-  gh.flush(c.hist);
+  gh.flush(c.sort.hist);
 }
 
 // digit histograms of keys that some other kernel produced (voxel grid, descriptor norm codes)
 template <int BITS>
-__global__ void __launch_bounds__(SORT_THREADS) k_sort_ghist(const CloudDev* clouds) {
-  const CloudDev& c = clouds[blockIdx.y];
+__global__ void __launch_bounds__(SORT_THREADS) k_sort_ghist(const SortDev* sorts) {
+  const SortDev& c = sorts[blockIdx.y];
   const int base = blockIdx.x * SORT_TILE;
   if (base >= c.n) return;
   extern __shared__ uint32_t sh_dyn[];
@@ -167,12 +165,17 @@ __global__ void __launch_bounds__(SORT_THREADS) k_sort_ghist(const CloudDev* clo
   gh.flush(c.hist);
 }
 
-// One pass: reads keys/vals[pass & 1], writes [(pass + 1) & 1].  GATHER (last pass of the index build): instead of the
-// value array the kernel writes the sorted points (w = original index) and the inverse permutation.
-template <int BITS, bool GATHER>
-__global__ void __launch_bounds__(SORT_THREADS) k_sort_pass(const CloudDev* clouds, int pass) {
+__device__ __forceinline__ const SortDev& sort_of(const SortDev& d) { return d; }
+__device__ __forceinline__ const SortDev& sort_of(const BuildDev& d) { return d.sort; }
+
+// One pass over the SortDev of each descriptor D (a SortDev, or the index build's BuildDev): reads keys/vals[pass & 1],
+// writes [(pass + 1) & 1].  GATHER (last pass of the index build): instead of the value array the kernel writes the
+// cloud's sorted points (w = original index) and the inverse permutation.
+template <int BITS, bool GATHER, class D>
+__global__ void __launch_bounds__(SORT_THREADS) k_sort_pass(const D* descs, int pass) {
   constexpr int R = 1 << BITS, NW = SORT_THREADS / 32, DPT = R / SORT_THREADS;  // digits per thread
-  const CloudDev& c = clouds[blockIdx.y];
+  const auto& d = descs[blockIdx.y];
+  const SortDev& c = sort_of(d);
   const int ntiles = sort_tiles(c.n);
   if ((int)blockIdx.x >= ntiles) return;
   __shared__ unsigned short cnt[NW][R];  // per-warp digit counts, then exclusive offsets inside the tile (<= SORT_TILE)
@@ -288,10 +291,10 @@ __global__ void __launch_bounds__(SORT_THREADS) k_sort_pass(const CloudDev* clou
       const uint32_t dig = (key[r] >> shift) & (R - 1);
       const uint32_t dst = gbase[dig] + cnt[w][dig] + rk[r];
       okeys[dst] = key[r];
-      if (GATHER) {
-        const float* p = c.raw + (size_t)val[r] * c.raw_stride;
-        c.pts[dst] = make_float4(p[0], p[1], p[2], __int_as_float((int)val[r]));
-        c.rank[val[r]] = (int)dst;
+      if constexpr (GATHER) {
+        const float* p = d.raw + (size_t)val[r] * d.raw_stride;
+        d.pts[dst] = make_float4(p[0], p[1], p[2], __int_as_float((int)val[r]));
+        d.rank[val[r]] = (int)dst;
       } else {
         ovals[dst] = val[r];
       }
@@ -299,18 +302,16 @@ __global__ void __launch_bounds__(SORT_THREADS) k_sort_pass(const CloudDev* clou
   }
 }
 
-// Stable LSD radix sort of (keys[0], vals[0]) of every descriptor; result in keys/vals[radix_sort_result_buf()].
-// Only the n / keys / vals / hist fields of the descriptors are used (also by the voxel grid, assemble.cu, and the
-// descriptor ordering, quatro.cu); hist must point to radix_sort_ws_bytes() ZEROED bytes.  key_bits <= 30: 3 x 10 bits,
-// otherwise 3 x 11 bits.
-int launch_radix_sort(const CloudDev* d_clouds, int count, int max_n, int key_bits, cudaStream_t s) {
+// Stable LSD radix sort of every descriptor (SortDev: the input in keys[0] / vals[0], the result in sorted_keys() /
+// sorted_vals(), hist = radix_sort_ws_bytes() ZEROED bytes).  key_bits <= 30: 3 x 10 bits, otherwise 3 x 11 bits.
+int launch_radix_sort(const SortDev* d_sorts, int count, int max_n, int key_bits, cudaStream_t s) {
   const dim3 grid(sort_tiles(max_n), count);
   if (key_bits <= 30) {
-    k_sort_ghist<10><<<grid, SORT_THREADS, SORT_PASSES * 1024 * 4, s>>>(d_clouds);
-    for (int p = 0; p < SORT_PASSES; p++) k_sort_pass<10, false><<<grid, SORT_THREADS, 0, s>>>(d_clouds, p);
+    k_sort_ghist<10><<<grid, SORT_THREADS, SORT_PASSES * 1024 * 4, s>>>(d_sorts);
+    for (int p = 0; p < SORT_PASSES; p++) k_sort_pass<10, false><<<grid, SORT_THREADS, 0, s>>>(d_sorts, p);
   } else {
-    k_sort_ghist<11><<<grid, SORT_THREADS, SORT_PASSES * 2048 * 4, s>>>(d_clouds);
-    for (int p = 0; p < SORT_PASSES; p++) k_sort_pass<11, false><<<grid, SORT_THREADS, 0, s>>>(d_clouds, p);
+    k_sort_ghist<11><<<grid, SORT_THREADS, SORT_PASSES * 2048 * 4, s>>>(d_sorts);
+    for (int p = 0; p < SORT_PASSES; p++) k_sort_pass<11, false><<<grid, SORT_THREADS, 0, s>>>(d_sorts, p);
   }
   return 1 + SORT_PASSES;
 }
@@ -322,12 +323,12 @@ __device__ __forceinline__ int delta(const uint32_t* __restrict__ keys, int n, i
   return x ? __clz(x) : 32 + __clz((uint32_t)i ^ (uint32_t)j);  // equal keys: fall back to the index
 }
 
-__global__ void __launch_bounds__(256) k_lbvh_topology(const CloudDev* clouds, int kbuf) {
-  const CloudDev& c = clouds[blockIdx.y];
+__global__ void __launch_bounds__(256) k_lbvh_topology(const BuildDev* builds) {
+  const BuildDev& c = builds[blockIdx.y];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n = c.n;
+  const int n = c.sort.n;
   if (i >= n - 1) return;
-  const uint32_t* __restrict__ keys = c.keys[kbuf];
+  const uint32_t* __restrict__ keys = c.sort.sorted_keys();
   const int d = (delta(keys, n, i, i + 1) - delta(keys, n, i, i - 1)) >= 0 ? 1 : -1;
   const int dmin = delta(keys, n, i, i - d);
   int lmax = 2;
@@ -358,10 +359,10 @@ __global__ void __launch_bounds__(256) k_lbvh_topology(const CloudDev* clouds, i
 // An item writes its box and its own reference into ITS half of the parent's traversal record and arrives at the
 // parent's flag; the second arrival owns the parent, reads the finished 64-byte record back, merges the two boxes and
 // carries on upwards.  (nbox, the separate per-node box array of round 1, is gone.)
-__global__ void __launch_bounds__(256) k_lbvh_aabb(const CloudDev* clouds) {
-  const CloudDev& c = clouds[blockIdx.y];
+__global__ void __launch_bounds__(256) k_lbvh_aabb(const BuildDev* builds) {
+  const BuildDev& c = builds[blockIdx.y];
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n = c.n;
+  const int n = c.sort.n;
   if (n <= LEAF || (int)(blockIdx.x * blockDim.x) >= 2 * n - 1) return;
   __shared__ int s_items[256];
   __shared__ int s_wcnt[8];
@@ -438,21 +439,20 @@ __global__ void __launch_bounds__(256) k_lbvh_aabb(const CloudDev* clouds) {
 }
 
 // ------------------------------------------------------------------------------------
-// host launcher: builds `count` clouds whose descriptors are already in device memory.
-// c.hist = zeroed sort work memory (radix_sort_ws_bytes(n, 30)), c.flags zeroed, c.bbox = 6 * BBOX_BLOCKS floats.
-// Returns the number of kernel launches issued.
-int launch_index_build(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s) {
+// host launcher: builds the `count` clouds whose BuildDevs are already in device memory (sort.hist = zeroed work memory
+// of radix_sort_ws_bytes(n, 30) bytes, flags zeroed).  Returns the number of kernel launches issued.
+int launch_index_build(const BuildDev* d_builds, int count, int max_n, cudaStream_t s) {
   int launches = 0;
   const int gx = max(1, min((max_n + 255) / 256, BBOX_BLOCKS));
-  k_bbox<<<dim3(gx, count), 256, 0, s>>>(d_clouds); launches++;
+  k_bbox<<<dim3(gx, count), 256, 0, s>>>(d_builds); launches++;
   const dim3 tiles(sort_tiles(max_n), count);
-  k_morton_ghist<<<tiles, SORT_THREADS, 0, s>>>(d_clouds, gx); launches++;
-  k_sort_pass<10, false><<<tiles, SORT_THREADS, 0, s>>>(d_clouds, 0); launches++;
-  k_sort_pass<10, false><<<tiles, SORT_THREADS, 0, s>>>(d_clouds, 1); launches++;
-  k_sort_pass<10, true><<<tiles, SORT_THREADS, 0, s>>>(d_clouds, 2); launches++;
+  k_morton_ghist<<<tiles, SORT_THREADS, 0, s>>>(d_builds, gx); launches++;
+  k_sort_pass<10, false><<<tiles, SORT_THREADS, 0, s>>>(d_builds, 0); launches++;
+  k_sort_pass<10, false><<<tiles, SORT_THREADS, 0, s>>>(d_builds, 1); launches++;
+  k_sort_pass<10, true><<<tiles, SORT_THREADS, 0, s>>>(d_builds, 2); launches++;
   if (max_n > 1) {
-    k_lbvh_topology<<<dim3((max_n + 254) / 256, count), 256, 0, s>>>(d_clouds, SORT_PASSES & 1); launches++;
-    k_lbvh_aabb<<<dim3((2 * max_n + 254) / 256, count), 256, 0, s>>>(d_clouds); launches++;
+    k_lbvh_topology<<<dim3((max_n + 254) / 256, count), 256, 0, s>>>(d_builds); launches++;
+    k_lbvh_aabb<<<dim3((2 * max_n + 254) / 256, count), 256, 0, s>>>(d_builds); launches++;
   }
   return launches;
 }

@@ -54,15 +54,27 @@ __device__ __forceinline__ NodeRec load_node(const float4* __restrict__ tnodes, 
   return {__ldg(&tnodes[4 * ref]), __ldg(&tnodes[4 * ref + 1]), __ldg(&tnodes[4 * ref + 2]), __ldg(&tnodes[4 * ref + 3])};
 }
 
+// One stable LSD radix sort of n (key, value) pairs (index_build.cu: launch_radix_sort).  The input is keys[0] / vals[0];
+// the passes ping-pong between the two halves and the result lands in sorted_keys() / sorted_vals().  hist is the sort's
+// work memory, radix_sort_ws_bytes(n, key_bits) bytes ZEROED by the caller.
+constexpr int SORT_PASSES = 3;
+struct SortDev {
+  int n;
+  uint32_t* keys[2];
+  uint32_t* vals[2];
+  uint32_t* hist;
+  __host__ __device__ uint32_t* sorted_keys() const { return keys[SORT_PASSES & 1]; }
+  __host__ __device__ uint32_t* sorted_vals() const { return vals[SORT_PASSES & 1]; }
+};
+
+// A built cloud: what persists for the life of the cloud.
 struct CloudDev {
-  const float* raw;    // device copy of the caller's records (xyz at stride)
-  int raw_stride;      // in floats
-  int n;               // points
-  int root_ref;        // 0 (internal root) or a leaf ref when n <= LEAF
   float4* pts;         // [n]
   float4* tnodes;      // [4 * (n - 1)]
   double* cov;         // [6 * n] (valid once has_cov)
   int* rank;           // [n]
+  int n;               // points
+  int root_ref;        // 0 (internal root) or a leaf ref when n <= LEAF
   // Quatro features (allocated by b200reg_clouds_fpfh; sorted order)
   float4* nrm;         // [n] unit normal, w = 1 valid / 0 invalid (< 3 neighbours)
   float* spfh;         // [FPAD * n]
@@ -75,15 +87,22 @@ struct CloudDev {
   float4* fproj_s;     // [n]
   float4* ftile;       // [2 * ceil(n / 64)] per tile: min and max filter coordinates of its base records (+inf / -inf if none)
   uint32_t* fcode_s;   // [n] sorted keys: 28-bit filter-space Morton code, 4 hash bits (0xFFFFFFFF for unusable records)
-  // build-time temporaries (freed after the build)
-  uint32_t* keys[2];   // sort ping-pong
-  uint32_t* vals[2];
-  uint32_t* hist;      // radix-sort work memory, ZEROED by the caller: radix_sort_ws_bytes(n, key_bits) (index_build.cu)
+};
+
+// What the index build (index_build.cu) of one cloud reads and writes, valid only while b200reg_clouds_create runs: the
+// Morton sort, the caller's records, the tree scratch, and the cloud's pts / tnodes / rank it fills.
+struct BuildDev {
+  SortDev sort;        // sort.n = points; Morton keys and point indices
+  const float* raw;    // device copy of the caller's records (xyz at stride)
+  int raw_stride;      // in floats
   uint32_t* flags;     // [n - 1] arrival flags of the bottom-up AABB pass, ZEROED by the caller
   int4* info;          // [n - 1] (first, last, leaf-child bits, split)
   int* parent_node;    // [n - 1]
   int* parent_leaf;    // [n]
   float* bbox;         // [6 * BBOX_BLOCKS] per-block min/max partials
+  float4* pts;         // the cloud's arrays (CloudDev)
+  float4* tnodes;
+  int* rank;
 };
 
 // phase of the per-pair LM state machine
@@ -186,12 +205,7 @@ struct KeyframeDev {
   int n;
   int pad;
 };
-struct SortBufs {  // what the radix sort needs (mirrors the CloudDev fields it reads)
-  uint32_t* keys[2];
-  uint32_t* vals[2];
-  uint32_t* hist;   // zeroed work memory, radix_sort_ws_bytes(total, 32)
-};
-struct AssembleJob {  // one output cloud of setSrcAndDstCloud
+struct AssembleJob {  // one output cloud of setSrcAndDstCloud; its voxel sort is the SortDev of the same index
   int nseg, total;
   int seg_kf[MAXSEG];
   int seg_off[MAXSEG + 1];
@@ -200,7 +214,6 @@ struct AssembleJob {  // one output cloud of setSrcAndDstCloud
   int* heads;       // [total]
   int* bbox;        // [6] ordered-int min/max
   int* counters;    // [0] voxels, [1] int32-overflow flag
-  SortBufs sort;
 };
 
 // ---- the transforms behind the output clouds, one definition each -----------------------------------------------------

@@ -180,7 +180,7 @@ __device__ __forceinline__ void kl_walk(const CloudDev& c, float qx, float qy, f
 // warp w of block b answers query b * KL_WARPS + w; SMEM_LIST: the list lives in shared memory (k <= KL_SMEM_K), else in
 // slab[query * k ...]
 template <bool SMEM_LIST>
-__global__ void __launch_bounds__(KL_THREADS) k_knn_large(CloudDev c, const float* q, int nq, int qstride, int k,
+__global__ void __launch_bounds__(KL_THREADS) k_knn_large(const __grid_constant__ CloudDev c, const float* q, int nq, int qstride, int k,
                                                           unsigned long long* slab, int* idx_out, float* d2_out) {
   __shared__ unsigned long long s_list[SMEM_LIST ? KL_WARPS * KL_SMEM_K : 1];
   __shared__ unsigned long long s_stage[KL_WARPS][KL_STAGE];

@@ -9,9 +9,8 @@ namespace b200 {
 
 // index_build.cu
 size_t radix_sort_ws_bytes(int n, int key_bits);
-int radix_sort_result_buf(int key_bits);
-int launch_radix_sort(const CloudDev* d_clouds, int count, int max_n, int key_bits, cudaStream_t s);
-int launch_index_build(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s);
+int launch_radix_sort(const SortDev* d_sorts, int count, int max_n, int key_bits, cudaStream_t s);
+int launch_index_build(const BuildDev* d_builds, int count, int max_n, cudaStream_t s);
 
 // gicp.cu.  launch_covariances: k <= 32 one thread per point; k > 32 goes to launch_covariance_large and needs
 // covariance_large_slab_bytes(count, max_n, k) of device scratch in slab (nullptr when that is 0)
@@ -32,13 +31,14 @@ void launch_transform_out(const CloudDev& c, const float* d_Tf, float* d_out3, c
 
 // quatro.cu
 cudaError_t quatro_init_device();
-int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2, float fpfh_r2, cudaStream_t s);
+// d_sorts[i]: the sort of cloud i's descriptor order (launch_feature_order), 32-bit keys
+int launch_fpfh(const CloudDev* d_clouds, const SortDev* d_sorts, int count, int max_n, float normal_r2, float fpfh_r2, cudaStream_t s);
 // the stages of launch_fpfh and launch_quatro_match_solve that b200reg_match_tap runs on caller descriptors:
 //   launch_load_records   rows of 33 bins in c.fpfh (stride FPAD) -> records, original index = row (the k_fpfh tail)
-//   launch_feature_order  k_fcode, radix sort, k_fgather (keys / vals / hist as for launch_radix_sort)
+//   launch_feature_order  k_fcode, radix sort of d_sorts, k_fgather
 //   launch_feature_match  k_match_init, k_feat_nn both ways, k_first_hit, k_mutual
 int launch_load_records(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s);
-int launch_feature_order(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s);
+int launch_feature_order(const CloudDev* d_clouds, const SortDev* d_sorts, int count, int max_n, cudaStream_t s);
 int launch_feature_match(const MatchDev* d_pairs, int count, int max_ni, int max_nj, float thr2, int advanced, cudaStream_t s);
 // optimizedMatching: k_teaser_solve solves the sets of at most MAXC and leaves larger ones (counters[2] > MAXC) to
 // launch_big_solve
@@ -93,11 +93,12 @@ void launch_pack_xyzi(const float* d_raw, int stride, int n, float4* d_out, cuda
 void launch_ingest_world(const float* d_raw, int stride, int n, const double* d_Tinv, float4* d_out, cudaStream_t s);
 int launch_fetch_closest(const double* d_pos, const double* d_stamp, const int* d_queries, int count, double radius, double tdiff,
                          int* d_out, cudaStream_t s);
-int launch_assemble_voxelize(const AssembleJob* d_jobs, const CloudDev* d_sort, int count, int max_total, const KeyframeDev* d_kfs,
+// d_sorts[j]: job j's voxel sort, 32-bit keys
+int launch_assemble_voxelize(const AssembleJob* d_jobs, const SortDev* d_sorts, int count, int max_total, const KeyframeDev* d_kfs,
                              const double* d_poses, float inv_leaf, cudaStream_t s);
-// loop-cloud capture: intensities of freshly uploaded clouds (raw records still valid) into d_inten[i][n_i]; then every
+// loop-cloud capture: intensities of the raw records of the clouds being built into d_inten[i][n_i]; then every
 // CaptureRow of a call (max_n = the longest row)
-void launch_gather_intensity(const CloudDev* d_clouds, int count, int max_n, float* const* d_inten, cudaStream_t s);
+void launch_gather_intensity(const BuildDev* d_builds, int count, int max_n, float* const* d_inten, cudaStream_t s);
 void launch_capture_rows(const CaptureRow* d_rows, int nrows, int max_n, cudaStream_t s);
 
 }  // namespace b200

@@ -281,22 +281,24 @@ __device__ __forceinline__ uint32_t fcode_of(const float4 f) {
 // sort key of sorted position p: 28-bit Morton code of the four filter coordinates, then 4 hash bits so that bitwise
 // identical descriptors (planar patches all produce the same histogram) end up next to each other; unusable
 // descriptors go to the end
-__global__ void __launch_bounds__(256) k_fcode(const CloudDev* clouds) {
+__global__ void __launch_bounds__(256) k_fcode(const CloudDev* clouds, const SortDev* sorts) {
   const CloudDev& c = clouds[blockIdx.y];
+  const SortDev& S = sorts[blockIdx.y];
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= c.n) return;
   const float4 tail = *reinterpret_cast<const float4*>(c.fpfh + (size_t)p * FPAD + 32);  // slots 32..35
   const bool ok = tail.z != 0.f;
-  c.keys[0][p] = ok ? ((fcode_of(c.fproj[p]) << 4) | (__float_as_uint(tail.w) & 15u)) : 0xFFFFFFFFu;
-  c.vals[0][p] = (uint32_t)p;
+  S.keys[0][p] = ok ? ((fcode_of(c.fproj[p]) << 4) | (__float_as_uint(tail.w) & 15u)) : 0xFFFFFFFFu;
+  S.vals[0][p] = (uint32_t)p;
 }
 // gather the records into code order, collapse runs of bitwise identical descriptors and box every tile of NN_TILE
 // records in filter space.  One 64-thread block per tile.
 //   A run (consecutive identical records inside one tile) keeps its first record as a BASE record, carrying the run's
 //   lowest original index in slot 35 -- exactly what the lowest-index tie rule would pick among them; the others get
 //   flag 2: still queries, never candidates.  Runs that a tile border or a hash collision splits simply keep two heads.
-__global__ void __launch_bounds__(NN_TILE) k_fgather(const CloudDev* clouds) {
+__global__ void __launch_bounds__(NN_TILE) k_fgather(const CloudDev* clouds, const SortDev* sorts) {
   const CloudDev& c = clouds[blockIdx.y];
+  const SortDev& S = sorts[blockIdx.y];
   const int t = blockIdx.x;
   if (t * NN_TILE >= c.n) return;
   const int r = t * NN_TILE + threadIdx.x;
@@ -311,7 +313,7 @@ __global__ void __launch_bounds__(NN_TILE) k_fgather(const CloudDev* clouds) {
   int p = -1;
   bool usable = false;
   if (r < c.n) {
-    p = (int)c.vals[1][r];  // radix_sort_result_buf()
+    p = (int)S.sorted_vals()[r];
     const float4* s4 = reinterpret_cast<const float4*>(c.fpfh + (size_t)p * FPAD);
 #pragma unroll
     for (int k = 0; k < 9; k++) rec[k] = s4[k];
@@ -347,7 +349,7 @@ __global__ void __launch_bounds__(NN_TILE) k_fgather(const CloudDev* clouds) {
 #pragma unroll
     for (int k = 0; k < 9; k++) d4[k] = rec[k];
     c.fproj_s[r] = fp;
-    c.fcode_s[r] = c.keys[1][r];
+    c.fcode_s[r] = S.sorted_keys()[r];
     if (usable && !same) {
       lo[0] = hi[0] = fp.x; lo[1] = hi[1] = fp.y; lo[2] = hi[2] = fp.z; lo[3] = hi[3] = fp.w;
     }
@@ -1727,19 +1729,19 @@ __global__ void __launch_bounds__(256) k_transform_raw(const CloudDev* clouds, c
 // ------------------------------------------------------------------------------------------------
 // host launchers
 // ------------------------------------------------------------------------------------------------
-int launch_fpfh(const CloudDev* d_clouds, int count, int max_n, float normal_r2, float fpfh_r2, cudaStream_t s) {
+int launch_fpfh(const CloudDev* d_clouds, const SortDev* d_sorts, int count, int max_n, float normal_r2, float fpfh_r2, cudaStream_t s) {
   dim3 grid((max_n + STEP_THREADS - 1) / STEP_THREADS, count);
   k_normals<<<grid, STEP_THREADS, 0, s>>>(d_clouds, normal_r2);
   k_spfh<<<grid, STEP_THREADS, 0, s>>>(d_clouds, fpfh_r2);
   k_fpfh<<<grid, STEP_THREADS, 0, s>>>(d_clouds, fpfh_r2);
-  return 3 + launch_feature_order(d_clouds, count, max_n, s);
+  return 3 + launch_feature_order(d_clouds, d_sorts, count, max_n, s);
 }
 
 // the matcher's view: records in the order of their filter-space Morton code, duplicates collapsed, boxed per tile
-int launch_feature_order(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s) {
-  k_fcode<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_clouds);
-  const int ls = launch_radix_sort(d_clouds, count, max_n, 32, s);  // 32-bit keys, 3 passes of 11 bits: result in keys[1] / vals[1]
-  k_fgather<<<dim3((max_n + NN_TILE - 1) / NN_TILE, count), NN_TILE, 0, s>>>(d_clouds);
+int launch_feature_order(const CloudDev* d_clouds, const SortDev* d_sorts, int count, int max_n, cudaStream_t s) {
+  k_fcode<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_clouds, d_sorts);
+  const int ls = launch_radix_sort(d_sorts, count, max_n, 32, s);  // 32-bit keys, 3 passes of 11 bits
+  k_fgather<<<dim3((max_n + NN_TILE - 1) / NN_TILE, count), NN_TILE, 0, s>>>(d_clouds, d_sorts);
   return 2 + ls;
 }
 
