@@ -421,7 +421,7 @@ static int assemble_clouds(b200reg_ctx* c, const KfState& kf, int count, const i
     if (J.total <= 0) return fail(B200REG_EINVAL, "empty merged cloud");
     const size_t n = J.total;
     Layout l;
-    const size_t o_m = l.take(n * 16), o_o = l.take(n * 16), o_h = l.take(n * 4), o_b = l.take(32), o_c = l.take(16);
+    const size_t o_m = l.take(n * 16), o_o = l.take(n * 16), o_h = l.take(n * 4), o_b = l.take(32), o_c = l.take(sizeof(AssembleCounters));
     const SortLayout sl(l, l, J.total, 32);
     char* slab = nullptr;
     CU(scratch.alloc((void**)&slab, l.size));
@@ -429,7 +429,7 @@ static int assemble_clouds(b200reg_ctx* c, const KfState& kf, int count, const i
     J.out = (float4*)(slab + o_o);
     J.heads = (int*)(slab + o_h);
     J.bbox = (int*)(slab + o_b);
-    J.counters = (int*)(slab + o_c);
+    J.counters = (AssembleCounters*)(slab + o_c);
     sorts[j] = sl.bind(slab, slab);
     CU(cudaMemsetAsync(sorts[j].hist, 0, sl.ws, s));
     max_total = std::max(max_total, J.total);
@@ -452,16 +452,16 @@ static int assemble_clouds(b200reg_ctx* c, const KfState& kf, int count, const i
     for (int j = 0; j < njobs; j++) c->prof_bytes[CLS_MISC] += 68.0 * jobs[j].total;  // 16 in + 16 merged + 36 sort/centroid
   }
   CU(cudaGetLastError());
-  std::vector<int> counters(4 * (size_t)njobs);
-  for (int j = 0; j < njobs; j++) CU(cudaMemcpyAsync(&counters[4 * j], jobs[j].counters, 8, cudaMemcpyDeviceToHost, s));
+  std::vector<AssembleCounters> counters(njobs);
+  for (int j = 0; j < njobs; j++) CU(cudaMemcpyAsync(&counters[j], jobs[j].counters, sizeof(AssembleCounters), cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
   // index the voxelised clouds (records are (x, y, z, intensity), 16-byte stride, already on the device)
   std::vector<const float*> ptrs(njobs);
   std::vector<size_t> ns(njobs);
   for (int j = 0; j < njobs; j++) {
-    const bool overflow = counters[4 * j + 1] != 0;  // PCL returns the input unchanged in that case
+    const bool overflow = counters[j].overflow != 0;  // PCL returns the input unchanged in that case
     ptrs[j] = (const float*)(overflow ? jobs[j].merged : jobs[j].out);
-    ns[j] = overflow ? (size_t)jobs[j].total : (size_t)counters[4 * j];
+    ns[j] = overflow ? (size_t)jobs[j].total : (size_t)counters[j].voxels;
   }
   std::vector<b200reg_cloud*> clouds(njobs, nullptr);
   int rc = clouds_create(c, njobs, ptrs.data(), ns.data(), 16, 1, keep_intensity, clouds.data());

@@ -92,19 +92,25 @@ int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* sr
   return B200REG_OK;
 }
 
-static int pow2_at_least(int n) {
-  int p = 1;
-  while (p < n) p <<= 1;
-  return p;
+// BigSolveWs::cap for a set of up to n correspondences on each solve tier, the one sizing rule b200reg_quatro_align and
+// b200reg_quatro_solve_tap share.  first: the batched advancedMatching pass, n the bound nj on the cross-checked set;
+// opt_big: the batched pass over optimizedMatching sets beyond MAXC; wide: the advancedMatching sets beyond BIGC, solved
+// one pair at a time in one workspace, n the largest.
+enum class SolveTier { first, opt_big, wide };
+static int solve_ws_cap(SolveTier tier, int n) {
+  if (tier == SolveTier::wide) return (n + 1023) / 1024 * 1024;
+  int cap = 1024;  // the power of two >= n, at least 1024; at most BIGC on the first pass
+  while (cap < n && (tier == SolveTier::opt_big || cap < BIGC)) cap <<= 1;
+  return cap;
 }
 
-// The one sizing of the global-memory solver workspace (BigSolveWs) for up to `cap` correspondences, cap a multiple of
-// 1024.  nsrc > 0 adds k_adv_select_wide's scatter array for a source cloud of nsrc points.
+// The global-memory solver workspace (BigSolveWs) for up to `cap` correspondences, cap a multiple of 1024 from
+// solve_ws_cap.  nsrc > 0 adds k_adv_select_wide's scatter array for a source cloud of nsrc points.
 struct BigWsLayout {
   int cap, words, p2;
   size_t o_S = 0, o_D = 0, o_adj = 0, o_radj = 0, o_int = 0, o_skey = 0, o_w = 0, o_res = 0, o_hval = 0, o_hidx = 0, o_best = 0,
          o_slot = 0;
-  BigWsLayout(Layout& l, int cap_, int nsrc) : cap(cap_), words(cap_ / 32), p2(pow2_at_least(cap_)) {
+  BigWsLayout(Layout& l, int cap_, int nsrc) : cap(cap_), words(cap_ / 32), p2(cap_ > 1 ? 1 << (32 - __builtin_clz(cap_ - 1)) : 1) {
     if (cap == 0) return;  // no workspace (optimizedMatching)
     o_S = l.take((size_t)cap * 24);
     o_D = l.take((size_t)cap * 24);
@@ -142,6 +148,39 @@ struct BigWsLayout {
   }
 };
 
+// A cloud's descriptor tables (CloudDev::fpfh ... fcode_s) for n points.  with_spfh adds the normals and the SPFH table
+// b200reg_clouds_fpfh computes them from; the SPFH table is dead once k_fpfh has consumed it, so fpfh_s reuses it.
+// Offsets first, pointers at bind().
+struct FeatureLayout {
+  bool spfh;
+  size_t o_nrm, o_spfh, o_fpfh, o_fproj, o_fpfh_s, o_fproj_s, o_ftile, o_fcode_s;
+  FeatureLayout(Layout& l, size_t n, bool with_spfh)
+      : spfh(with_spfh), o_nrm(spfh ? l.take(n * 16) : 0), o_spfh(spfh ? l.take(n * FPAD * 4) : 0), o_fpfh(l.take(n * FPAD * 4)),
+        o_fproj(l.take(n * 16)), o_fpfh_s(spfh ? o_spfh : l.take(n * FPAD * 4)), o_fproj_s(l.take(n * 16)),
+        o_ftile(l.take(2 * ((n + 63) / 64) * 16)), o_fcode_s(l.take(n * 4)) {}
+  void bind(char* slab, CloudDev& d) const {
+    if (spfh) { d.nrm = (float4*)(slab + o_nrm); d.spfh = (float*)(slab + o_spfh); }
+    d.fpfh = (float*)(slab + o_fpfh); d.fproj = (float4*)(slab + o_fproj); d.fpfh_s = (float*)(slab + o_fpfh_s);
+    d.fproj_s = (float4*)(slab + o_fproj_s); d.ftile = (float4*)(slab + o_ftile); d.fcode_s = (uint32_t*)(slab + o_fcode_s);
+  }
+};
+
+// The matcher's per-pair arrays (MatchDev::nn ... stats) for ni >= nj descriptors, and the solve's outputs: T, and
+// out_corr of corr_cap pairs unless that is 0.  ni = nj = 0 leaves the matcher's arrays empty, for a solve of given
+// correspondences.  Offsets first, pointers at bind().
+struct MatchLayout {
+  size_t o_nn, o_dis, o_fj, o_rnn, o_cor, o_tk, o_cnt, o_st, o_oc, o_T;
+  MatchLayout(Layout& l, size_t ni, size_t nj, size_t corr_cap)
+      : o_nn(l.take(nj * 4)), o_dis(l.take(nj * 4)), o_fj(l.take(ni * 4)), o_rnn(l.take(ni * 4)), o_cor(l.take(2 * nj * 4)),
+        o_tk(l.take(nj * 4)), o_cnt(l.take(sizeof(MatchCounters))), o_st(l.take(8 * 8)), o_oc(corr_cap ? l.take(2 * corr_cap * 4) : 0),
+        o_T(l.take(16 * 8)) {}
+  void bind(char* slab, MatchDev& m) const {
+    m.nn = (int*)(slab + o_nn); m.dis = (float*)(slab + o_dis); m.first_j = (int*)(slab + o_fj); m.rnn = (int*)(slab + o_rnn);
+    m.corres = (int*)(slab + o_cor); m.tkey = (unsigned*)(slab + o_tk); m.counters = (MatchCounters*)(slab + o_cnt);
+    m.stats = (double*)(slab + o_st); m.out_corr = o_oc ? (int*)(slab + o_oc) : nullptr; m.T = (double*)(slab + o_T);
+  }
+};
+
 // squared feature distance gate of the matcher (dis > thr2 is dropped, matcher.cc:422,444).  advancedMatching searches
 // without a gate: FLT_MAX makes every finite distance qualify.  A square that overflows, or a NaN threshold, drops nothing
 // in the reference either: +inf.
@@ -167,20 +206,184 @@ static QuatroParamsDev quatro_params_dev(const b200reg_quatro_params* prm, bool 
   return q;
 }
 
+// one b200reg_quatro_align call: every pair's device workspace and, after each pass, its counters and out[i].T
+struct QuatroCall {
+  b200reg_ctx* c;
+  Scratch& scratch;
+  QuatroParamsDev q;
+  b200reg_quatro_info* out;
+  std::vector<MatchDev> pairs;
+  std::vector<MatchCounters> counters;
+};
+
+// the size of a pair's final correspondence set: n_wide while the wide tier has the pair pending
+static int set_size(const MatchCounters& k) { return k.n_wide > 0 ? k.n_wide : k.n_corr; }
+
+// queues the copy of pair i's counters and T to the host
+static cudaError_t fetch_result(QuatroCall& qc, int i) {
+  const cudaError_t e = cudaMemcpyAsync(&qc.counters[i], qc.pairs[i].counters, sizeof(MatchCounters), cudaMemcpyDeviceToHost, qc.c->stream);
+  return e != cudaSuccess ? e : cudaMemcpyAsync(qc.out[i].T, qc.pairs[i].T, 128, cudaMemcpyDeviceToHost, qc.c->stream);
+}
+
+static void fill_info(const MatchCounters& k, b200reg_quatro_info& o) {
+  o.valid = k.valid;
+  o.n_mutual = k.n_mutual;
+  o.n_corr = k.n_corr;
+  o.clique_size = k.clique_size;
+  o.gnc_iterations = k.gnc_iterations;
+  o.reserved = 0;
+}
+
+// Matches every pair and solves, in one batched pass, each set of at most MAXC (optimizedMatching, k_teaser_solve) or
+// BIGC (advancedMatching, the global-memory chain).  corr_fixed (count x 2 x corr_stride ints) receives each pair's
+// out_corr as this pass leaves it.
+static int match_and_solve_first(QuatroCall& qc, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst, int corr_stride,
+                                 int32_t* corr_fixed) {
+  b200reg_ctx* c = qc.c;
+  cudaStream_t s = c->stream;
+  const bool advanced = qc.q.advanced;
+  // optimizedMatching's out_corr: MAXC pairs, or max_corres + 3 when that is more
+  const int opt_cap = std::max(MAXC, qc.q.max_corres + 3);
+  qc.pairs.resize(count);
+  qc.counters.resize(count);
+  std::vector<BigSolveWs> big_host;
+  big_host.reserve(count);  // addresses stay valid for the async copies below
+  int max_ni = 0, max_nj = 0;
+  for (int i = 0; i < count; i++) {
+    MatchDev& m = qc.pairs[i];
+    const bool swapped = dst[i]->dev.n > src[i]->dev.n;  // fi = larger cloud (matcher.cc:364-369)
+    m.fi = swapped ? dst[i]->dev : src[i]->dev;
+    m.fj = swapped ? src[i]->dev : dst[i]->dev;
+    m.swapped = swapped ? 1 : 0;
+    const size_t ni = m.fi.n, nj = m.fj.n;
+    const int cap = advanced ? solve_ws_cap(SolveTier::first, (int)nj) : 0;
+    Layout l;
+    const MatchLayout ml(l, ni, nj, advanced ? cap : opt_cap);
+    const size_t o_big = advanced ? l.take(sizeof(BigSolveWs)) : 0;
+    const BigWsLayout wl(l, cap, 0);  // empty when !advanced
+    char* slab = nullptr;
+    CU(qc.scratch.alloc((void**)&slab, l.size));
+    ml.bind(slab, m);
+    if (advanced) {
+      m.big = (BigSolveWs*)(slab + o_big);
+      big_host.push_back(wl.bind(slab));
+      CU(cudaMemcpyAsync(m.big, &big_host.back(), sizeof(BigSolveWs), cudaMemcpyHostToDevice, s));
+    }
+    max_ni = std::max(max_ni, (int)ni);
+    max_nj = std::max(max_nj, (int)nj);
+  }
+  MatchDev* d_pairs = nullptr;
+  CU(qc.scratch.upload(&d_pairs, qc.pairs.data(), sizeof(MatchDev) * count));
+  {
+    ProfScope ps(c, CLS_MATCH);
+    c->launches += launch_quatro_match_solve(d_pairs, count, max_ni, max_nj, qc.q, s);
+    for (const MatchDev& m : qc.pairs) c->prof_bytes[CLS_MATCH] += 132.0 * (m.fi.n + m.fj.n) + 8.0 * m.fj.n;  // SURVEY §8(d) Q4
+  }
+  CU(cudaGetLastError());
+  for (int i = 0; i < count; i++) {
+    CU(fetch_result(qc, i));
+    if (corr_fixed) {
+      const size_t have = advanced ? (size_t)big_host[i].cap : (size_t)MAXC;  // what this pair's buffer holds
+      CU(cudaMemcpyAsync(&corr_fixed[2 * (size_t)corr_stride * i], qc.pairs[i].out_corr, 2 * have * 4, cudaMemcpyDeviceToHost, s));
+    }
+  }
+  CU(cudaStreamSynchronize(s));
+  return B200REG_OK;
+}
+
+// The optimizedMatching sets beyond MAXC, which k_teaser_solve left unsolved: each gets a workspace for its own size, and
+// all of them are solved in one batched pass; each pair's view reads its own out_corr and writes its own counters and T.
+static int solve_opt_big(QuatroCall& qc, const std::vector<int>& big) {
+  cudaStream_t s = qc.c->stream;
+  const int nb = (int)big.size();
+  int max_big = 0;
+  Layout l;
+  const size_t o_views = l.take(sizeof(MatchDev) * nb), o_ws = l.take(sizeof(BigSolveWs) * nb);
+  std::vector<BigWsLayout> wls;
+  for (int i : big) {
+    max_big = std::max(max_big, qc.counters[i].n_corr);
+    wls.emplace_back(l, solve_ws_cap(SolveTier::opt_big, qc.counters[i].n_corr), 0);
+  }
+  char* slab = nullptr;
+  if (qc.scratch.alloc((void**)&slab, l.size) != cudaSuccess) {
+    cudaGetLastError();
+    char msg[200];
+    snprintf(msg, sizeof msg, "optimizedMatching kept up to %d correspondences; solving them needs a workspace of %zu bytes, "
+             "which could not be allocated", max_big, l.size);
+    return fail(B200REG_ECUDA, msg);
+  }
+  std::vector<MatchDev> views(nb);
+  std::vector<BigSolveWs> ws(nb);
+  for (int k = 0; k < nb; k++) {
+    ws[k] = wls[k].bind(slab);
+    views[k] = qc.pairs[big[k]];
+    views[k].big = (BigSolveWs*)(slab + o_ws) + k;
+  }
+  CU(cudaMemcpyAsync(slab + o_ws, ws.data(), sizeof(BigSolveWs) * nb, cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(slab + o_views, views.data(), sizeof(MatchDev) * nb, cudaMemcpyHostToDevice, s));
+  {
+    ProfScope ps(qc.c, CLS_MATCH);
+    qc.c->launches += launch_big_solve((const MatchDev*)(slab + o_views), nb, max_big, qc.q, s);
+  }
+  CU(cudaGetLastError());
+  for (int i : big) CU(fetch_result(qc, i));
+  CU(cudaStreamSynchronize(s));  // views and ws stay alive until their copies are done
+  return B200REG_OK;
+}
+
+// The advancedMatching sets beyond BIGC, which k_adv_select left unsolved: solved one pair after another in one workspace
+// sized for the largest, so device memory stays bounded by the largest.  corr_csr receives pair i's set at offsets[i].
+static int solve_wide(QuatroCall& qc, const std::vector<int>& wide, int32_t* corr_csr, const std::vector<int64_t>& offsets) {
+  cudaStream_t s = qc.c->stream;
+  int max_wide = 0, max_src = 0;
+  for (int i : wide) {
+    max_wide = std::max(max_wide, qc.counters[i].n_wide);
+    max_src = std::max(max_src, qc.pairs[i].swapped ? qc.pairs[i].fj.n : qc.pairs[i].fi.n);
+  }
+  const int cap = solve_ws_cap(SolveTier::wide, max_wide);
+  Layout l;
+  const size_t o_big = l.take(sizeof(BigSolveWs)), o_pair = l.take(sizeof(MatchDev)), o_oc = l.take((size_t)cap * 8);
+  const BigWsLayout wl(l, cap, max_src);
+  char* slab = nullptr;
+  if (qc.scratch.alloc((void**)&slab, l.size) != cudaSuccess) {
+    cudaGetLastError();
+    char msg[200];
+    snprintf(msg, sizeof msg, "advancedMatching kept %d correspondences; solving them needs a workspace of %zu bytes, which "
+             "could not be allocated", max_wide, l.size);
+    return fail(B200REG_ECUDA, msg);
+  }
+  const BigSolveWs w = wl.bind(slab);
+  CU(cudaMemcpyAsync(slab + o_big, &w, sizeof w, cudaMemcpyHostToDevice, s));
+  std::vector<MatchDev> views(wide.size());  // each pair with its selection and solve redirected to the shared workspace;
+                                             // stream order keeps one pair's use of it from overlapping the next
+  {
+    ProfScope ps(qc.c, CLS_MATCH);
+    for (size_t k = 0; k < wide.size(); k++) {
+      const int i = wide[k], n = qc.counters[i].n_wide;
+      views[k] = qc.pairs[i];
+      views[k].out_corr = (int*)(slab + o_oc);
+      views[k].big = (BigSolveWs*)(slab + o_big);
+      CU(cudaMemcpyAsync(slab + o_pair, &views[k], sizeof(MatchDev), cudaMemcpyHostToDevice, s));
+      qc.c->launches += launch_adv_wide((const MatchDev*)(slab + o_pair), n, qc.q, s);
+      CU(cudaGetLastError());
+      CU(fetch_result(qc, i));
+      if (corr_csr) CU(cudaMemcpyAsync(corr_csr + 2 * offsets[i], views[k].out_corr, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+    }
+  }
+  CU(cudaStreamSynchronize(s));  // w and views stay alive until their copies are done
+  return B200REG_OK;
+}
+
 // b200reg_quatro_align (corr_fixed: count x 2 x CAP ints, or NULL) and b200reg_quatro_align_ex (offsets_out non-NULL;
 // corr_csr: `capacity` pairs, or NULL).  Every pair is matched and, if its set holds at most BIGC correspondences,
-// solved in one batched pass.  A larger advancedMatching set is then solved on its own in one workspace shared by all
-// such pairs of the call (sized for the largest), one pair after another, so device memory stays bounded by the largest.
-// optimizedMatching keeps at most max_corres + 3 <= BIGC: k_teaser_solve solves the sets of at most MAXC in that pass,
-// and the larger ones are solved afterwards in one batched pass of the global-memory chain.
+// solved in one batched pass.  A larger advancedMatching set is then solved by solve_wide.  optimizedMatching keeps at
+// most max_corres + 3 <= BIGC: k_teaser_solve solves the sets of at most MAXC in that pass, and solve_opt_big the rest.
 static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst, const b200reg_quatro_params* prm,
                       b200reg_quatro_info* out, int32_t* corr_fixed, int64_t* offsets_out, size_t capacity, int32_t* corr_csr) {
   if (!c || count <= 0 || !src || !dst || !prm || !out) return fail(B200REG_EINVAL, "bad argument");
   if (prm->estimate_scale) return fail(B200REG_EINVAL, "estimate_scale is not supported (the deployment sets it false)");
   const bool advanced = !prm->use_optimized_matching;  // Matcher::advancedMatching (matcher.cc:118-356)
   if (!advanced && (prm->max_corres < 1 || prm->max_corres > OPT_MAX_CORRES)) return fail(B200REG_EINVAL, "max_corres must be in 1..8189");
-  // optimizedMatching's out_corr: MAXC pairs, or max_corres + 3 when that is more
-  const int opt_cap = advanced ? 0 : std::max(MAXC, prm->max_corres + 3);
   const int corr_stride = advanced ? BIGC : MAXC;  // B200REG_ADV_CORR_CAPACITY / B200REG_CORR_CAPACITY
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
@@ -195,107 +398,32 @@ static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* sr
     }
     if ((rc = b200reg_clouds_fpfh(c, (int)all.size(), all.data(), prm->fpfh_normal_radius, prm->fpfh_radius))) return rc;
   }
-  std::vector<MatchDev> pairs(count);
-  std::vector<BigSolveWs> big_host;
-  big_host.reserve(count);  // addresses stay valid for the async copies below
-  int max_ni = 0, max_nj = 0;
+  QuatroCall qc{c, scratch, quatro_params_dev(prm, advanced), out, {}, {}};
+  if ((rc = match_and_solve_first(qc, count, src, dst, corr_stride, corr_fixed))) return rc;
+  std::vector<int> big, wide;
   for (int i = 0; i < count; i++) {
-    MatchDev& m = pairs[i];
-    const bool swapped = dst[i]->dev.n > src[i]->dev.n;  // fi = larger cloud (matcher.cc:364-369)
-    m.fi = swapped ? dst[i]->dev : src[i]->dev;
-    m.fj = swapped ? src[i]->dev : dst[i]->dev;
-    m.swapped = swapped ? 1 : 0;
-    const size_t ni = m.fi.n, nj = m.fj.n;
-    Layout l;
-    const size_t o_nn = l.take(nj * 4), o_dis = l.take(nj * 4), o_fj = l.take(ni * 4), o_rnn = l.take(ni * 4);
-    // advancedMatching: the cross-checked set has at most nj members; the solver workspace is sized for the next
-    // power of two (>= 1024, <= BIGC)
-    int cap = 1024;
-    while (advanced && cap < (int)nj && cap < BIGC) cap <<= 1;
-    const size_t o_cor = l.take(2 * nj * 4), o_tk = l.take(nj * 4), o_cnt = l.take(8 * 4), o_st = l.take(8 * 8),
-                 o_oc = l.take(2 * (size_t)(advanced ? cap : opt_cap) * 4), o_T = l.take(16 * 8);
-    const size_t o_big = advanced ? l.take(sizeof(BigSolveWs)) : 0;
-    const BigWsLayout wl(l, advanced ? cap : 0, 0);  // empty when !advanced
-    char* slab = nullptr;
-    CU(scratch.alloc((void**)&slab, l.size));
-    m.nn = (int*)(slab + o_nn);
-    m.dis = (float*)(slab + o_dis);
-    m.first_j = (int*)(slab + o_fj);
-    m.rnn = (int*)(slab + o_rnn);
-    m.corres = (int*)(slab + o_cor);
-    m.tkey = (unsigned*)(slab + o_tk);
-    m.counters = (int*)(slab + o_cnt);
-    m.stats = (double*)(slab + o_st);
-    m.out_corr = (int*)(slab + o_oc);
-    m.T = (double*)(slab + o_T);
-    m.big = nullptr;
-    if (advanced) {
-      m.big = (BigSolveWs*)(slab + o_big);
-      big_host.push_back(wl.bind(slab));
-      CU(cudaMemcpyAsync(m.big, &big_host.back(), sizeof(BigSolveWs), cudaMemcpyHostToDevice, s));
+    const int n = set_size(qc.counters[i]);
+    if (corr_fixed && n > corr_stride) {
+      char msg[200];
+      snprintf(msg, sizeof msg, "%s kept %d correspondences for pair %d; corr_out holds %d per pair "
+               "(b200reg_quatro_align_ex returns any number)", advanced ? "advancedMatching" : "optimizedMatching", n, i, corr_stride);
+      return fail(B200REG_ESTATE, msg);
     }
-    max_ni = std::max(max_ni, (int)ni);
-    max_nj = std::max(max_nj, (int)nj);
-  }
-  MatchDev* d_pairs = nullptr;
-  CU(scratch.upload(&d_pairs, pairs.data(), sizeof(MatchDev) * count));
-  const QuatroParamsDev q = quatro_params_dev(prm, advanced);
-  {
-    ProfScope ps(c, CLS_MATCH);
-    c->launches += launch_quatro_match_solve(d_pairs, count, max_ni, max_nj, q, s);
-    for (int i = 0; i < count; i++) c->prof_bytes[CLS_MATCH] += 132.0 * (pairs[i].fi.n + pairs[i].fj.n) + 8.0 * pairs[i].fj.n;  // SURVEY §8(d) Q4
-  }
-  CU(cudaGetLastError());
-  std::vector<int> counters(8 * (size_t)count);
-  for (int i = 0; i < count; i++) {
-    CU(cudaMemcpyAsync(&counters[8 * i], pairs[i].counters, 32, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(out[i].T, pairs[i].T, 128, cudaMemcpyDeviceToHost, s));
-    if (corr_fixed) {
-      const size_t have = advanced ? (size_t)big_host[i].cap : (size_t)MAXC;  // what this pair's buffer holds
-      CU(cudaMemcpyAsync(&corr_fixed[2 * (size_t)corr_stride * i], pairs[i].out_corr, 2 * have * 4, cudaMemcpyDeviceToHost, s));
-    }
-  }
-  CU(cudaStreamSynchronize(s));
-  // counters[6] > 0: k_adv_select found more than BIGC correspondences and left the pair unsolved
-  std::vector<int> wide;
-  int max_wide = 0, max_src = 0;
-  for (int i = 0; i < count; i++)
-    if (counters[8 * i + 6] > 0) {
-      const int n = counters[8 * i + 6];
-      if (corr_fixed) {
-        char msg[200];
-        snprintf(msg, sizeof msg, "advancedMatching kept %d correspondences for pair %d; corr_out holds %d per pair "
-                 "(b200reg_quatro_align_ex returns any number)", n, i, BIGC);
-        return fail(B200REG_ESTATE, msg);
-      }
+    if (qc.counters[i].n_wide > 0) {
       if (n >= BIG_NMAX) {
         char msg[160];
         snprintf(msg, sizeof msg, "advancedMatching kept %d correspondences for pair %d; the solver takes fewer than %d", n, i, BIG_NMAX);
         return fail(B200REG_ESTATE, msg);
       }
       wide.push_back(i);
-      max_wide = std::max(max_wide, n);
-      max_src = std::max(max_src, pairs[i].swapped ? pairs[i].fj.n : pairs[i].fi.n);
-    }
-  // optimizedMatching sets beyond MAXC: k_teaser_solve left them unsolved
-  std::vector<int> big;
-  int max_big = 0;
-  for (int i = 0; i < count && !advanced; i++)
-    if (counters[8 * i + 2] > MAXC) {
-      const int n = counters[8 * i + 2];
-      if (corr_fixed) {
-        char msg[200];
-        snprintf(msg, sizeof msg, "optimizedMatching kept %d correspondences for pair %d; corr_out holds %d per pair "
-                 "(b200reg_quatro_align_ex returns any number)", n, i, MAXC);
-        return fail(B200REG_ESTATE, msg);
-      }
+    } else if (!advanced && n > MAXC) {
       big.push_back(i);
-      max_big = std::max(max_big, n);
     }
+  }
   std::vector<int64_t> offsets;
   if (offsets_out) {
     offsets.assign(count + 1, 0);
-    for (int i = 0; i < count; i++) offsets[i + 1] = offsets[i] + (counters[8 * i + 6] > 0 ? counters[8 * i + 6] : counters[8 * i + 2]);
+    for (int i = 0; i < count; i++) offsets[i + 1] = offsets[i] + set_size(qc.counters[i]);
     memcpy(offsets_out, offsets.data(), sizeof(int64_t) * (count + 1));
     if (corr_csr && (uint64_t)offsets[count] > capacity) {
       char msg[160];
@@ -304,85 +432,13 @@ static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* sr
     }
     if (corr_csr)
       for (int i = 0; i < count; i++)
-        if (counters[8 * i + 6] == 0 && counters[8 * i + 2] > 0)
-          CU(cudaMemcpyAsync(corr_csr + 2 * offsets[i], pairs[i].out_corr, (size_t)counters[8 * i + 2] * 8, cudaMemcpyDeviceToHost, s));
+        if (qc.counters[i].n_wide == 0 && qc.counters[i].n_corr > 0)
+          CU(cudaMemcpyAsync(corr_csr + 2 * offsets[i], qc.pairs[i].out_corr, (size_t)qc.counters[i].n_corr * 8, cudaMemcpyDeviceToHost, s));
   }
-  // each optimizedMatching set beyond MAXC gets a workspace for its own size, and all of them are solved in one batched
-  // pass; each pair's view reads its own out_corr and writes its own counters and T
-  std::vector<MatchDev> big_views(big.size());
-  std::vector<BigSolveWs> big_ws(big.size());
-  if (!big.empty()) {
-    const int nb = (int)big.size();
-    Layout l;
-    const size_t o_views = l.take(sizeof(MatchDev) * nb), o_ws = l.take(sizeof(BigSolveWs) * nb);
-    std::vector<BigWsLayout> wls;
-    wls.reserve(nb);
-    for (int i : big) wls.emplace_back(l, std::max(1024, pow2_at_least(counters[8 * i + 2])), 0);
-    char* slab = nullptr;
-    if (scratch.alloc((void**)&slab, l.size) != cudaSuccess) {
-      cudaGetLastError();
-      char msg[200];
-      snprintf(msg, sizeof msg, "optimizedMatching kept up to %d correspondences; solving them needs a workspace of %zu bytes, "
-               "which could not be allocated", max_big, l.size);
-      return fail(B200REG_ECUDA, msg);
-    }
-    for (int k = 0; k < nb; k++) {
-      big_ws[k] = wls[k].bind(slab);
-      big_views[k] = pairs[big[k]];
-      big_views[k].big = (BigSolveWs*)(slab + o_ws) + k;
-    }
-    CU(cudaMemcpyAsync(slab + o_ws, big_ws.data(), sizeof(BigSolveWs) * nb, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(slab + o_views, big_views.data(), sizeof(MatchDev) * nb, cudaMemcpyHostToDevice, s));
-    {
-      ProfScope ps(c, CLS_MATCH);
-      c->launches += launch_big_solve((const MatchDev*)(slab + o_views), nb, max_big, q, s);
-    }
-    CU(cudaGetLastError());
-    for (int i : big) {
-      CU(cudaMemcpyAsync(&counters[8 * i], pairs[i].counters, 32, cudaMemcpyDeviceToHost, s));
-      CU(cudaMemcpyAsync(out[i].T, pairs[i].T, 128, cudaMemcpyDeviceToHost, s));
-    }
-  }
-  if (!wide.empty()) {
-    const int cap = (max_wide + 1023) / 1024 * 1024;
-    Layout l;
-    const size_t o_big = l.take(sizeof(BigSolveWs)), o_pair = l.take(sizeof(MatchDev)), o_oc = l.take((size_t)cap * 8);
-    const BigWsLayout wl(l, cap, max_src);
-    char* slab = nullptr;
-    if (scratch.alloc((void**)&slab, l.size) != cudaSuccess) {
-      cudaGetLastError();
-      char msg[200];
-      snprintf(msg, sizeof msg, "advancedMatching kept %d correspondences; solving them needs a workspace of %zu bytes, which "
-               "could not be allocated", max_wide, l.size);
-      return fail(B200REG_ECUDA, msg);
-    }
-    const BigSolveWs w = wl.bind(slab);
-    CU(cudaMemcpyAsync(slab + o_big, &w, sizeof w, cudaMemcpyHostToDevice, s));
-    std::vector<MatchDev> views(wide.size());  // each pair with its selection and solve redirected to the shared workspace;
-                                               // stream order keeps one pair's use of it from overlapping the next
-    ProfScope ps(c, CLS_MATCH);
-    for (size_t k = 0; k < wide.size(); k++) {
-      const int i = wide[k], n = counters[8 * i + 6];
-      views[k] = pairs[i];
-      views[k].out_corr = (int*)(slab + o_oc);
-      views[k].big = (BigSolveWs*)(slab + o_big);
-      CU(cudaMemcpyAsync(slab + o_pair, &views[k], sizeof(MatchDev), cudaMemcpyHostToDevice, s));
-      c->launches += launch_adv_wide((const MatchDev*)(slab + o_pair), n, q, s);
-      CU(cudaGetLastError());
-      CU(cudaMemcpyAsync(&counters[8 * i], pairs[i].counters, 32, cudaMemcpyDeviceToHost, s));
-      CU(cudaMemcpyAsync(out[i].T, pairs[i].T, 128, cudaMemcpyDeviceToHost, s));
-      if (corr_csr) CU(cudaMemcpyAsync(corr_csr + 2 * offsets[i], views[k].out_corr, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
-    }
-  }
+  if (!big.empty() && (rc = solve_opt_big(qc, big))) return rc;
+  if (!wide.empty() && (rc = solve_wide(qc, wide, corr_csr, offsets))) return rc;
   CU(cudaStreamSynchronize(s));
-  for (int i = 0; i < count; i++) {
-    out[i].valid = counters[8 * i + 3];
-    out[i].n_mutual = counters[8 * i + 1];
-    out[i].n_corr = counters[8 * i + 2];
-    out[i].clique_size = counters[8 * i + 4];
-    out[i].gnc_iterations = counters[8 * i + 5];
-    out[i].reserved = 0;
-  }
+  for (int i = 0; i < count; i++) fill_info(qc.counters[i], out[i]);
   return B200REG_OK;
 }
 }  // namespace b200
@@ -419,22 +475,12 @@ int b200reg_clouds_fpfh(b200reg_ctx* c, int count, b200reg_cloud* const* clouds,
     if (cl->has_fpfh && cl->normal_r == normal_radius && cl->fpfh_r == fpfh_radius) continue;
     if (std::find(todo.begin(), todo.end(), cl) != todo.end()) continue;
     if (!cl->fslab) {
-      const size_t n = cl->dev.n;
       Layout l;
-      const size_t o_n = l.take(n * sizeof(float4)), o_s = l.take(n * FPAD * sizeof(float)), o_f = l.take(n * FPAD * sizeof(float)),
-                   o_fn = l.take(n * sizeof(float4)), o_fns = l.take(n * sizeof(float4)),
-                   o_ft = l.take(2 * ((n + 63) / 64) * sizeof(float4)), o_fc = l.take(n * sizeof(uint32_t));
+      const FeatureLayout fl(l, cl->dev.n, true);
       char* fs = nullptr;
       CU(cudaMallocFromPoolAsync((void**)&fs, l.size, c->pool, s));
       cl->fslab = fs;
-      cl->dev.nrm = (float4*)(fs + o_n);
-      cl->dev.spfh = (float*)(fs + o_s);
-      cl->dev.fpfh = (float*)(fs + o_f);
-      cl->dev.fproj = (float4*)(fs + o_fn);
-      cl->dev.fpfh_s = cl->dev.spfh;  // the SPFH table is dead once k_fpfh has consumed it
-      cl->dev.fproj_s = (float4*)(fs + o_fns);
-      cl->dev.ftile = (float4*)(fs + o_ft);
-      cl->dev.fcode_s = (uint32_t*)(fs + o_fc);
+      fl.bind(fs, cl->dev);
     }
     todo.push_back(cl);
     descs.push_back(cl->dev);
@@ -516,7 +562,8 @@ int b200reg_quatro_solve_tap(b200reg_ctx* c, int n, const float* src_xyz, const 
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Scratch scratch(c);
-  const int counters[8] = {0, n, n, 0, 0, 0, 0, 0};
+  MatchCounters counters{};  // as the matcher leaves a set of n mutual pairs, all of them kept
+  counters.n_mutual = counters.n_corr = n;
   MatchDev m{};
   const MatchDev* d_pair = nullptr;
   const int* d_clique = nullptr;
@@ -534,25 +581,24 @@ int b200reg_quatro_solve_tap(b200reg_ctx* c, int n, const float* src_xyz, const 
       corr[2 * i] = corr[2 * i + 1] = i;
     }
     Layout l;
-    const size_t o_pts = l.take(pts.size() * 16), o_rank = l.take((size_t)n * 4), o_oc = l.take(corr.size() * 4),
-                 o_cnt = l.take(8 * 4), o_T = l.take(16 * 8), o_clq = l.take((size_t)n * 4), o_pair = l.take(sizeof(MatchDev));
+    const MatchLayout ml(l, 0, 0, n);
+    const size_t o_pts = l.take(pts.size() * 16), o_rank = l.take((size_t)n * 4), o_clq = l.take((size_t)n * 4),
+                 o_pair = l.take(sizeof(MatchDev));
     char* slab = nullptr;
     CU(scratch.alloc((void**)&slab, l.size));
+    ml.bind(slab, m);
     m.fi.n = m.fj.n = n;
     m.fi.pts = (float4*)(slab + o_pts);
     m.fj.pts = m.fi.pts + n;
     m.fi.rank = m.fj.rank = (int*)(slab + o_rank);
     m.swapped = 0;
-    m.out_corr = (int*)(slab + o_oc);
-    m.counters = (int*)(slab + o_cnt);
-    m.T = (double*)(slab + o_T);
     m.clique = (int*)(slab + o_clq);
     d_clique = m.clique;
     d_pair = (const MatchDev*)(slab + o_pair);
     CU(cudaMemcpyAsync(m.fi.pts, pts.data(), pts.size() * 16, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(m.fi.rank, ident.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(m.out_corr, corr.data(), corr.size() * 4, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(m.counters, counters, sizeof counters, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(m.counters, &counters, sizeof counters, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(slab + o_pair, &m, sizeof m, cudaMemcpyHostToDevice, s));
     c->launches += launch_teaser_solve(d_pair, 1, quatro_params_dev(prm, false), s);
   } else {
@@ -561,16 +607,14 @@ int b200reg_quatro_solve_tap(b200reg_ctx* c, int n, const float* src_xyz, const 
       S[k] = src_xyz[k];  // k_big_gather's float -> double
       D[k] = dst_xyz[k];
     }
-    // the workspace b200reg_quatro_align gives a set of this size on each path
-    const int cap = wide ? (n + 1023) / 1024 * 1024 : std::max(1024, pow2_at_least(n));
     Layout l;
-    const size_t o_big = l.take(sizeof(BigSolveWs)), o_cnt = l.take(8 * 4), o_T = l.take(16 * 8), o_pair = l.take(sizeof(MatchDev));
-    const BigWsLayout wl(l, cap, 0);
+    const MatchLayout ml(l, 0, 0, 0);
+    const size_t o_big = l.take(sizeof(BigSolveWs)), o_pair = l.take(sizeof(MatchDev));
+    const BigWsLayout wl(l, solve_ws_cap(wide ? SolveTier::wide : SolveTier::first, n), 0);
     char* slab = nullptr;
     CU(scratch.alloc((void**)&slab, l.size));
     const BigSolveWs w = wl.bind(slab);
-    m.counters = (int*)(slab + o_cnt);
-    m.T = (double*)(slab + o_T);
+    ml.bind(slab, m);
     m.big = (BigSolveWs*)(slab + o_big);
     d_clique = w.clique;
     d_pair = (const MatchDev*)(slab + o_pair);
@@ -579,25 +623,20 @@ int b200reg_quatro_solve_tap(b200reg_ctx* c, int n, const float* src_xyz, const 
     CU(cudaMemcpyAsync(w.S, S.data(), S.size() * 8, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(w.D, D.data(), D.size() * 8, cudaMemcpyHostToDevice, s));
     CU(cudaMemsetAsync(w.deg, 0, (size_t)n * 4, s));
-    CU(cudaMemcpyAsync(m.counters, counters, sizeof counters, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(m.counters, &counters, sizeof counters, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(m.T, T, sizeof T, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(m.big, &w, sizeof w, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(slab + o_pair, &m, sizeof m, cudaMemcpyHostToDevice, s));
     c->launches += launch_big_graph_solve(d_pair, 1, quatro_params_dev(prm, true), wide ? n : 0, s);
   }
   CU(cudaGetLastError());
-  int got[8];
-  CU(cudaMemcpyAsync(got, m.counters, sizeof got, cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(&counters, m.counters, sizeof counters, cudaMemcpyDeviceToHost, s));
   CU(cudaMemcpyAsync(info->T, m.T, 128, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
-  if (clique_out && got[4] > 0) CU(cudaMemcpyAsync(clique_out, d_clique, (size_t)got[4] * 4, cudaMemcpyDeviceToHost, s));
+  if (clique_out && counters.clique_size > 0)
+    CU(cudaMemcpyAsync(clique_out, d_clique, (size_t)counters.clique_size * 4, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
-  info->valid = got[3];
-  info->n_mutual = n;
-  info->n_corr = n;
-  info->clique_size = got[4];
-  info->gnc_iterations = got[5];
-  info->reserved = 0;
+  fill_info(counters, *info);  // the solve leaves n_mutual and n_corr as uploaded: n
   return B200REG_OK;
 }
 
@@ -619,56 +658,34 @@ int b200reg_match_tap(b200reg_ctx* c, int count, const float* const* fi, const i
   std::vector<SortDev> sorts(2 * (size_t)count);
   std::vector<MatchDev> pairs(count);
   Layout l;
-  std::vector<size_t> o_c(2 * (size_t)count), o_p(count);
-  auto cloud_bytes = [](size_t n) {
-    Layout x;
-    for (size_t b : {n * FPAD * 4, n * 16, n * FPAD * 4, n * 16, 2 * ((n + 63) / 64) * 16, n * 4}) x.take(b);
-    SortLayout(x, x, (int)n, 32);
-    return x.size;
-  };
-  int max_n = 0, max_ni = 0, max_nj = 0;
+  std::vector<FeatureLayout> fls;
+  std::vector<SortLayout> sls;
+  std::vector<MatchLayout> mls;
+  int max_ni = 0, max_nj = 0;
+  for (int q = 0; q < 2 * count; q++) {
+    cl[q].n = q & 1 ? nj[q / 2] : ni[q / 2];
+    fls.emplace_back(l, cl[q].n, false);
+    sls.emplace_back(l, l, cl[q].n, 32);
+  }
   for (int k = 0; k < count; k++) {
-    o_c[2 * k] = l.take(cloud_bytes(ni[k]));
-    o_c[2 * k + 1] = l.take(cloud_bytes(nj[k]));
-    o_p[k] = l.take(((size_t)nj[k] * 5 + (size_t)ni[k] * 2) * 4 + 32 + 64 + 256);
+    mls.emplace_back(l, ni[k], nj[k], 0);
     max_ni = std::max(max_ni, (int)ni[k]);
     max_nj = std::max(max_nj, (int)nj[k]);
   }
-  max_n = max_ni;
   char* slab = nullptr;
   CU(scratch.alloc((void**)&slab, l.size));
   for (int q = 0; q < 2 * count; q++) {
-    const size_t n = q & 1 ? nj[q / 2] : ni[q / 2];
     CloudDev& d = cl[q];
-    char* b = slab + o_c[q];
-    Layout x;
-    d.n = (int)n;
-    d.fpfh = (float*)(b + x.take(n * FPAD * 4));
-    d.fproj = (float4*)(b + x.take(n * 16));
-    d.fpfh_s = (float*)(b + x.take(n * FPAD * 4));
-    d.fproj_s = (float4*)(b + x.take(n * 16));
-    d.ftile = (float4*)(b + x.take(2 * ((n + 63) / 64) * 16));
-    d.fcode_s = (uint32_t*)(b + x.take(n * 4));
-    const SortLayout sl(x, x, (int)n, 32);
-    sorts[q] = sl.bind(b, b);
-    CU(cudaMemsetAsync(sorts[q].hist, 0, sl.ws, s));
+    fls[q].bind(slab, d);
+    sorts[q] = sls[q].bind(slab, slab);
+    CU(cudaMemsetAsync(sorts[q].hist, 0, sls[q].ws, s));
     // the caller's rows into slots 0..32 of the record table; k_load_records completes the records in place
-    CU(cudaMemcpy2DAsync(d.fpfh, FPAD * 4, q & 1 ? fj[q / 2] : fi[q / 2], FDIM * 4, FDIM * 4, n, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpy2DAsync(d.fpfh, FPAD * 4, q & 1 ? fj[q / 2] : fi[q / 2], FDIM * 4, FDIM * 4, d.n, cudaMemcpyHostToDevice, s));
   }
   for (int k = 0; k < count; k++) {
-    MatchDev& m = pairs[k];
-    m.fi = cl[2 * k];
-    m.fj = cl[2 * k + 1];
-    const size_t a = ni[k], b = nj[k];
-    char* p = slab + o_p[k];
-    m.nn = (int*)p;
-    m.dis = (float*)(p + b * 4);
-    m.corres = (int*)(p + b * 8);
-    m.tkey = (unsigned*)(p + b * 16);
-    m.first_j = (int*)(p + b * 20);
-    m.rnn = (int*)(p + b * 20 + a * 4);
-    m.counters = (int*)(p + b * 20 + a * 8);
-    m.stats = (double*)(p + (b * 20 + a * 8 + 32 + 63) / 64 * 64);
+    pairs[k].fi = cl[2 * k];
+    pairs[k].fj = cl[2 * k + 1];
+    mls[k].bind(slab, pairs[k]);
   }
   CloudDev* d_cl = nullptr;
   SortDev* d_sorts = nullptr;
@@ -678,21 +695,21 @@ int b200reg_match_tap(b200reg_ctx* c, int count, const float* const* fi, const i
   CU(scratch.upload(&d_pairs, pairs.data(), sizeof(MatchDev) * count));
   {
     ProfScope ps(c, CLS_MATCH);
-    c->launches += launch_load_records(d_cl, 2 * count, max_n, s);
-    c->launches += launch_feature_order(d_cl, d_sorts, 2 * count, max_n, s);
+    c->launches += launch_load_records(d_cl, 2 * count, max_ni, s);
+    c->launches += launch_feature_order(d_cl, d_sorts, 2 * count, max_ni, s);
     c->launches += launch_feature_match(d_pairs, count, max_ni, max_nj, match_thr2(distance_threshold, !!advanced), advanced ? 1 : 0, s);
   }
   CU(cudaGetLastError());
-  std::vector<int> counters(8 * (size_t)count);
+  std::vector<MatchCounters> counters(count);
   for (int k = 0; k < count; k++) {
     CU(cudaMemcpyAsync(nn_out[k], pairs[k].nn, (size_t)nj[k] * 4, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(dis_out[k], pairs[k].dis, (size_t)nj[k] * 4, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(rnn_out[k], pairs[k].rnn, (size_t)ni[k] * 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&counters[8 * k], pairs[k].counters, 32, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&counters[k], pairs[k].counters, sizeof(MatchCounters), cudaMemcpyDeviceToHost, s));
   }
   CU(cudaStreamSynchronize(s));
   for (int k = 0; k < count; k++) {
-    n_mutual_out[k] = counters[8 * k + 1];
+    n_mutual_out[k] = counters[k].n_mutual;
     if (n_mutual_out[k] > 0)
       CU(cudaMemcpyAsync(mutual_out[k], pairs[k].corres, (size_t)n_mutual_out[k] * 8, cudaMemcpyDeviceToHost, s));
   }

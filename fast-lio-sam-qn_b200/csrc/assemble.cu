@@ -42,8 +42,8 @@ __global__ void k_assemble_init(const AssembleJob* jobs) {
   if (threadIdx.x < 3) J.bbox[threadIdx.x] = f2ord(INFINITY);
   else if (threadIdx.x < 6) J.bbox[threadIdx.x] = f2ord(-INFINITY);
   if (threadIdx.x == 6) {
-    J.counters[0] = 0;  // number of voxels
-    J.counters[1] = 0;  // overflow flag
+    J.counters->voxels = 0;
+    J.counters->overflow = 0;
   }
 }
 
@@ -99,7 +99,7 @@ __global__ void __launch_bounds__(256) k_voxel_keys(const AssembleJob* jobs, con
     cells *= (long long)((hi - lo) * inv_leaf) + 1;
   }
   if (cells > 2147483647LL) {  // PCL: "Leaf size is too small ... Integer indices would overflow" -> input returned as is
-    if (i == 0) J.counters[1] = 1;
+    if (i == 0) J.counters->overflow = 1;
     S.keys[0][i] = (uint32_t)i;
     S.vals[0][i] = (uint32_t)i;
     return;
@@ -150,14 +150,14 @@ __global__ void __launch_bounds__(1024) k_voxel_heads(const AssembleJob* jobs, c
     if (threadIdx.x == 1023) carry = pos + head;
     __syncthreads();
   }
-  if (threadIdx.x == 0) J.counters[0] = carry;
+  if (threadIdx.x == 0) J.counters->voxels = carry;
 }
 
 // centroid of x, y, z, intensity per voxel: fp32 running sums in sorted (= ascending point index) order
 __global__ void __launch_bounds__(256) k_voxel_centroid(const AssembleJob* jobs, const SortDev* sorts) {
   const AssembleJob& J = jobs[blockIdx.y];
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  const int nv = J.counters[0];
+  const int nv = J.counters->voxels;
   if (v >= nv) return;
   const int a = J.heads[v], b = v + 1 < nv ? J.heads[v + 1] : J.total;
   const uint32_t* vals = sorts[blockIdx.y].sorted_vals();

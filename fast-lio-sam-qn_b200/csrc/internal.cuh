@@ -205,15 +205,18 @@ struct KeyframeDev {
   int n;
   int pad;
 };
+struct AssembleCounters {
+  int voxels, overflow;  // centroids written to `out`; 1 when the voxel grid's int32 index would overflow
+};
 struct AssembleJob {  // one output cloud of setSrcAndDstCloud; its voxel sort is the SortDev of the same index
   int nseg, total;
   int seg_kf[MAXSEG];
   int seg_off[MAXSEG + 1];
   float4* merged;   // [total] transformed, merged points
-  float4* out;      // [total] voxel centroids (counters[0] of them)
+  float4* out;      // [total] voxel centroids (counters->voxels of them)
   int* heads;       // [total]
   int* bbox;        // [6] ordered-int min/max
-  int* counters;    // [0] voxels, [1] int32-overflow flag
+  AssembleCounters* counters;
 };
 
 // ---- the transforms behind the output clouds, one definition each -----------------------------------------------------
@@ -246,6 +249,13 @@ struct CaptureRow {
 };
 
 // ---- Quatro matcher / solver workspace ---------------------------------------------------
+// The matcher's and solver's counters of one pair, named after the b200reg_quatro_info fields they feed.  n_wide > 0:
+// k_adv_select found that many (> BIGC) correspondences and left the pair unsolved, with n_corr = 0.
+struct MatchCounters {
+  int unused0, n_mutual, n_corr, valid, clique_size, gnc_iterations, n_wide, unused7;
+};
+static_assert(sizeof(MatchCounters) == 32, "the host copies 32 bytes and k_match_init zeroes 8 ints");
+
 // per-pair device workspace of the matcher / solver
 struct MatchDev {
   CloudDev fi, fj;     // fi = larger cloud (base of the forward search), fj = smaller
@@ -256,7 +266,7 @@ struct MatchDev {
   int* rnn;            // [ni] original j returned by the reverse search (by ORIGINAL i)
   int* corres;         // [2 * nj] mutual (i, j) pairs, ascending j
   unsigned* tkey;      // [nj] first (trial*4 + slot) at which correspondence r would be added
-  int* counters;       // [0] unused, [1] ncorr, [2] n_out, [3] valid, [4] clique size, [5] gnc iterations
+  MatchCounters* counters;
   double* stats;       // [0..2] sum fi, [3..5] sum fj, then floats: mean fi(3) mean fj(3) scale (as float bits in doubles)
   int* out_corr;       // [2 * corr_cap] final (src, dst) pairs (corr_cap = max(MAXC, max_corres + 3) for
                        // optimizedMatching, BigSolveWs::cap for advancedMatching)

@@ -40,10 +40,10 @@ int launch_fpfh(const CloudDev* d_clouds, const SortDev* d_sorts, int count, int
 int launch_load_records(const CloudDev* d_clouds, int count, int max_n, cudaStream_t s);
 int launch_feature_order(const CloudDev* d_clouds, const SortDev* d_sorts, int count, int max_n, cudaStream_t s);
 int launch_feature_match(const MatchDev* d_pairs, int count, int max_ni, int max_nj, float thr2, int advanced, cudaStream_t s);
-// optimizedMatching: k_teaser_solve solves the sets of at most MAXC and leaves larger ones (counters[2] > MAXC) to
+// optimizedMatching: k_teaser_solve solves the sets of at most MAXC and leaves larger ones (n_corr > MAXC) to
 // launch_big_solve
 int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, int max_nj, const QuatroParamsDev& prm, cudaStream_t s);
-// k_teaser_solve alone (one block of solve_smem_bytes() per pair): counters[2] correspondences listed in out_corr
+// k_teaser_solve alone (one block of solve_smem_bytes() per pair): n_corr correspondences listed in out_corr
 size_t solve_smem_bytes();
 int launch_teaser_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, cudaStream_t s);
 // k_big_gather + launch_big_graph_solve(n_wide = 0): pairs of at most max_n <= BIGC correspondences, `big` bound

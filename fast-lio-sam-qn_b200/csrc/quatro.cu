@@ -661,7 +661,7 @@ __global__ void __launch_bounds__(256) k_match_init(const MatchDev* pairs) {
     P.rnn[i] = -1;
   }
   if (i < P.fj.n) P.tkey[i] = 0xFFFFFFFFu;
-  if (i < 8) P.counters[i] = 0;
+  if (i < 8) reinterpret_cast<int*>(P.counters)[i] = 0;  // the whole MatchCounters record
   if (i < 8) P.stats[i] = 0.0;
 }
 
@@ -719,7 +719,7 @@ __global__ void __launch_bounds__(1024) k_mutual(const MatchDev* pairs, float th
     if (threadIdx.x == 1023) carry = pos + keep;
     __syncthreads();
   }
-  if (threadIdx.x == 0) P.counters[1] = carry;
+  if (threadIdx.x == 0) P.counters->n_mutual = carry;
 }
 
 // Matcher::normalizePoints: per-cloud mean (fp64 fixed-shape tree sum, cast to fp32) and the larger max radius.
@@ -792,7 +792,7 @@ __device__ __forceinline__ float len3(const float a[3], const float b[3]) {
 // the earliest (trial, slot) at which the serial loop would have added it (matcher.cc:484-536)
 __global__ void __launch_bounds__(256) k_tuple_trials(const MatchDev* pairs, QuatroParamsDev prm) {
   const MatchDev& P = pairs[blockIdx.y];
-  const int ncorr = P.counters[1];
+  const int ncorr = P.counters->n_mutual;
   // tuple_scale == 0: no trial runs.  optimizedMatching then keeps nothing (its tuple block is the only writer of corres_,
   // matcher.cc:461), so k_tuple_select finds no key; advancedMatching keeps every pair (k_adv_select's keepall).
   if (ncorr == 0 || prm.tuple_scale == 0.f) return;
@@ -856,13 +856,13 @@ struct KeyCmpSwap {
 __global__ void __launch_bounds__(1024) k_tuple_select(const MatchDev* pairs, QuatroParamsDev prm) {
   extern __shared__ __align__(16) unsigned long long keys[];  // [tuple_sort_len(prm.max_corres)]
   const MatchDev& P = pairs[blockIdx.x];
-  const int ncorr = P.counters[1];
+  const int ncorr = P.counters->n_mutual;
   const int L = tuple_sort_len(prm.max_corres);
   __shared__ unsigned hist[256];
   __shared__ unsigned prefix, remaining, tstar;
   __shared__ int nsel;
   if (ncorr == 0) {
-    if (threadIdx.x == 0) P.counters[2] = 0;
+    if (threadIdx.x == 0) P.counters->n_corr = 0;
     return;
   }
   // (max_corres+1)-th smallest key by 4-pass radix select; none => keep everything
@@ -927,7 +927,7 @@ __global__ void __launch_bounds__(1024) k_tuple_select(const MatchDev* pairs, Qu
     P.out_corr[2 * s] = P.swapped ? j : i;      // always (src, dst) (matcher.cc:527-535)
     P.out_corr[2 * s + 1] = P.swapped ? i : j;
   }
-  if (threadIdx.x == 0) P.counters[2] = n;
+  if (threadIdx.x == 0) P.counters->n_corr = n;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -994,9 +994,9 @@ __device__ __forceinline__ bool tim_edge(const double* si, const double* di, con
 __device__ __forceinline__ void reset_result(const MatchDev& P, int i) {
   if (i < 16) P.T[i] = (i % 5 == 0) ? 1.0 : 0.0;
   if (i == 0) {
-    P.counters[3] = 0;
-    P.counters[4] = 0;
-    P.counters[5] = 0;
+    P.counters->valid = 0;
+    P.counters->clique_size = 0;
+    P.counters->gnc_iterations = 0;
   }
 }
 
@@ -1006,8 +1006,8 @@ __device__ __forceinline__ void write_result(const MatchDev& P, const double* R2
   P.T[4] = R2[2]; P.T[5] = R2[3]; P.T[6] = 0; P.T[7] = t[1];
   P.T[8] = 0; P.T[9] = 0; P.T[10] = 1; P.T[11] = t[2];
   P.T[12] = 0; P.T[13] = 0; P.T[14] = 0; P.T[15] = 1;
-  P.counters[3] = 1;
-  P.counters[5] = iters;
+  P.counters->valid = 1;
+  P.counters->gnc_iterations = iters;
 }
 
 // block-wide state of the GNC-TLS rotation, in shared memory
@@ -1189,7 +1189,7 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
   extern __shared__ __align__(16) unsigned char smraw[];
   SolveSmem& sm = *reinterpret_cast<SolveSmem*>(smraw);
   const MatchDev& P = pairs[blockIdx.x];
-  const int n = P.counters[2];
+  const int n = P.counters->n_corr;
   const int tid = threadIdx.x;
   reset_result(P, tid);
   // a set beyond MAXC (optimizedMatching with max_corres > 509) does not fit here: quatro_align_impl hands it to the
@@ -1295,7 +1295,7 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
     for (int v = 0; v < n; v++)
       if ((Cm[v >> 5] >> (v & 31)) & 1u) sm.clique[m++] = v;
     sm.m = m;
-    P.counters[4] = m;
+    P.counters->clique_size = m;
     if (P.clique)
       for (int k = 0; k < m; k++) P.clique[k] = sm.clique[k];
   }
@@ -1330,7 +1330,7 @@ __global__ void __launch_bounds__(SV_THREADS) k_teaser_solve(const MatchDev* pai
 __global__ void __launch_bounds__(1024) k_adv_select(const MatchDev* pairs, QuatroParamsDev prm) {
   extern __shared__ __align__(16) unsigned long long akeys[];  // [BIGC]
   const MatchDev& P = pairs[blockIdx.x];
-  const int ncorr = P.counters[1];
+  const int ncorr = P.counters->n_mutual;
   const int cap = P.big->cap;
   __shared__ int nsel;
   if (threadIdx.x == 0) nsel = 0;
@@ -1348,8 +1348,8 @@ __global__ void __launch_bounds__(1024) k_adv_select(const MatchDev* pairs, Quat
   const int total = nsel;
   if (total > cap) {  // reported as B200REG_ESTATE by the host; nothing is solved
     if (threadIdx.x == 0) {
-      P.counters[2] = 0;
-      P.counters[6] = total;
+      P.counters->n_corr = 0;
+      P.counters->n_wide = total;
     }
     return;
   }
@@ -1362,7 +1362,7 @@ __global__ void __launch_bounds__(1024) k_adv_select(const MatchDev* pairs, Quat
     P.out_corr[2 * i] = (int)(akeys[i] >> 32);
     P.out_corr[2 * i + 1] = (int)(akeys[i] & 0xFFFFFFFFull);
   }
-  if (threadIdx.x == 0) P.counters[2] = total;
+  if (threadIdx.x == 0) P.counters->n_corr = total;
 }
 
 // ordered compaction by one block of 1024 threads: emit(pos, v) for every v < n with keep(v), pos ascending with v.
@@ -1412,7 +1412,7 @@ __device__ int block_compact(int n, Keep keep, Emit emit) {
 __global__ void __launch_bounds__(1024) k_adv_select_wide(const MatchDev* pairs, QuatroParamsDev prm) {
   const MatchDev& P = pairs[blockIdx.x];
   const BigSolveWs& W = *P.big;
-  const int ncorr = P.counters[1];
+  const int ncorr = P.counters->n_mutual;
   const int nsrc = P.swapped ? P.fj.n : P.fi.n;
   const bool keepall = prm.tuple_scale == 0.f;
   for (int v = threadIdx.x; v < nsrc; v += 1024) W.slot[v] = -1;
@@ -1429,13 +1429,13 @@ __global__ void __launch_bounds__(1024) k_adv_select_wide(const MatchDev* pairs,
         P.out_corr[2 * pos] = v;
         P.out_corr[2 * pos + 1] = W.slot[v];
       });
-  if (threadIdx.x == 0) P.counters[2] = total;
+  if (threadIdx.x == 0) P.counters->n_corr = total;
 }
 
 __global__ void __launch_bounds__(256) k_big_gather(const MatchDev* pairs) {
   const MatchDev& P = pairs[blockIdx.y];
   const BigSolveWs& W = *P.big;
-  const int n = P.counters[2];
+  const int n = P.counters->n_corr;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   reset_result(P, i);
   if (i >= n) return;
@@ -1452,7 +1452,7 @@ __global__ void __launch_bounds__(256) k_big_gather(const MatchDev* pairs) {
 __global__ void __launch_bounds__(256) k_big_tim(const MatchDev* pairs, QuatroParamsDev prm) {
   const MatchDev& P = pairs[blockIdx.y];
   const BigSolveWs& W = *P.big;
-  const int n = P.counters[2];
+  const int n = P.counters->n_corr;
   const int wn = (n + 31) >> 5;
   const double beta = 2.0 * prm.noise_bound;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < (long long)n * wn; idx += (long long)gridDim.x * blockDim.x) {
@@ -1477,7 +1477,7 @@ __global__ void __launch_bounds__(256) k_big_tim(const MatchDev* pairs, QuatroPa
 __global__ void __launch_bounds__(1024) k_big_core(const MatchDev* pairs) {
   const MatchDev& P = pairs[blockIdx.x];
   const BigSolveWs& W = *P.big;
-  const int n = P.counters[2];
+  const int n = P.counters->n_corr;
   if (n == 0) return;
   const int wn = (n + 31) >> 5;
   const int tid = threadIdx.x;
@@ -1537,7 +1537,7 @@ __global__ void __launch_bounds__(1024) k_big_core(const MatchDev* pairs) {
 __global__ void __launch_bounds__(256) k_big_radj(const MatchDev* pairs) {
   const MatchDev& P = pairs[blockIdx.y];
   const BigSolveWs& W = *P.big;
-  const int n = P.counters[2];
+  const int n = P.counters->n_corr;
   const int wn = (n + 31) >> 5;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < (long long)n * wn; idx += (long long)gridDim.x * blockDim.x) {
     const int rv = (int)(idx / wn), w = (int)(idx % wn);
@@ -1593,7 +1593,7 @@ __device__ __forceinline__ int warp_greedy_clique(const BigSolveWs& W, int wn, i
 __global__ void __launch_bounds__(256) k_big_greedy(const MatchDev* pairs) {
   const MatchDev& P = pairs[blockIdx.y];
   const BigSolveWs& W = *P.big;
-  const int n = P.counters[2];
+  const int n = P.counters->n_corr;
   const int wn = (n + 31) >> 5;
   const int nwarps = gridDim.x * (blockDim.x >> 5);
   for (int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n; r += nwarps) {
@@ -1643,7 +1643,7 @@ __global__ void __launch_bounds__(256) k_big_greedy_wide(const MatchDev* pairs) 
   extern __shared__ unsigned cand[];  // [warps per block][wn]
   const MatchDev& P = pairs[blockIdx.y];
   const BigSolveWs& W = *P.big;
-  const int n = P.counters[2];
+  const int n = P.counters->n_corr;
   const int wn = (n + 31) >> 5;
   const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (r >= n) return;
@@ -1660,7 +1660,7 @@ __global__ void __launch_bounds__(256) k_big_greedy_wide(const MatchDev* pairs) 
 __global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, QuatroParamsDev prm, int wide) {
   const MatchDev& P = pairs[blockIdx.x];
   const BigSolveWs& W = *P.big;
-  const int n = P.counters[2];
+  const int n = P.counters->n_corr;
   if (n == 0) return;
   const int wn = (n + 31) >> 5;
   const int tid = threadIdx.x;
@@ -1687,7 +1687,7 @@ __global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, Quat
   // members in ascending ORIGINAL correspondence index
   const int m = block_compact(
       n, [&](int v) { return W.alive[v] != 0; }, [&](int pos, int v) { W.clique[pos] = v; });
-  if (tid == 0) P.counters[4] = m;
+  if (tid == 0) P.counters->clique_size = m;
   if (m <= 1) return;  // solution_.valid stays false
   const int iters = gnc_tls_yaw<1024>(W.S, W.D, W.clique, m, W.w, W.res, red, gnc, prm);
   const double range = prm.noise_bound;
@@ -1771,7 +1771,7 @@ int launch_teaser_solve(const MatchDev* d_pairs, int count, const QuatroParamsDe
   return 1;
 }
 
-// the feature matcher up to the mutual list (nn, dis, first_j, rnn, corres, counters[1]); also zeroes counters and stats
+// the feature matcher up to the mutual list (nn, dis, first_j, rnn, corres, n_mutual); also zeroes the counters and stats
 int launch_feature_match(const MatchDev* d_pairs, int count, int max_ni, int max_nj, float thr2, int advanced, cudaStream_t s) {
   int l = 0;
   k_match_init<<<dim3((max_ni + 255) / 256, count), 256, 0, s>>>(d_pairs); l++;
@@ -1796,14 +1796,14 @@ int launch_quatro_match_solve(const MatchDev* d_pairs, int count, int max_ni, in
   return l + launch_big_solve(d_pairs, count, BIGC, prm, s);
 }
 
-// the global-memory TEASER++ solve of sets of at most BIGC correspondences (out_corr listed, counters[2] set, each
+// the global-memory TEASER++ solve of sets of at most BIGC correspondences (out_corr listed, n_corr set, each
 // pair's `big` workspace bound), max_n the largest set of the batch: gather, then one batched pass
 int launch_big_solve(const MatchDev* d_pairs, int count, int max_n, const QuatroParamsDev& prm, cudaStream_t s) {
   k_big_gather<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_pairs);
   return 1 + launch_big_graph_solve(d_pairs, count, prm, 0, s);
 }
 
-// one pair whose advancedMatching set outgrew k_adv_select (n > BIGC correspondences, counters[6] = n): select into the
+// one pair whose advancedMatching set outgrew k_adv_select (n > BIGC correspondences, n_wide = n): select into the
 // pair's own workspace, gather, solve
 int launch_adv_wide(const MatchDev* d_pair, int n, const QuatroParamsDev& prm, cudaStream_t s) {
   k_adv_select_wide<<<1, 1024, 0, s>>>(d_pair, prm);
@@ -1811,7 +1811,7 @@ int launch_adv_wide(const MatchDev* d_pair, int n, const QuatroParamsDev& prm, c
   return 2 + launch_big_graph_solve(d_pair, 1, prm, n, s);
 }
 
-// TEASER++ solve over the global-memory workspace (S / D gathered, counters[2] set): TIM graph, core order, greedy
+// TEASER++ solve over the global-memory workspace (S / D gathered, n_corr set): TIM graph, core order, greedy
 // cliques, GNC-TLS.  n_wide == 0: sets of at most BIGC, candidate sets in registers, any batch; n_wide > 0: one pair of
 // n_wide correspondences, candidate sets in shared memory and pruned starts (k_big_greedy_wide).
 int launch_big_graph_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, int n_wide, cudaStream_t s) {
