@@ -116,7 +116,8 @@ EXPORTS = [
     "b200reg_allgather_results", "b200reg_radius_search", "b200reg_quatro_align_ex", "b200reg_quatro_solve_tap",
     "b200reg_ctx_set_lm_trace", "b200reg_lm_trace", "b200reg_ctx_set_loop_clouds", "b200reg_loop_clouds",
     "b200reg_match_tap", "b200reg_lm_step_tap", "b200reg_index_tap", "b200reg_sort_tap",
-    "b200reg_batch_submit_perform_loop_closure",
+    "b200reg_batch_submit_perform_loop_closure", "b200reg_batch_set_loop_clouds", "b200reg_batch_set_lm_trace",
+    "b200reg_batch_loop_clouds", "b200reg_batch_lm_trace", "b200reg_batch_release",
 ]
 ESTATE = -4  # B200REG_ESTATE
 # B200REG_CLOUD_*: the loop clouds (Context.set_loop_clouds / Context.loop_clouds)
@@ -173,6 +174,32 @@ class B200RegError(RuntimeError):
 def _check(rc):
     if rc != 0:
         raise B200RegError("b200reg error %d: %s" % (rc, lib().b200reg_last_error().decode()))
+
+
+def _lm_trace(get):
+    """The CSR trace behind get(offsets, capacity, trials) (b200reg_lm_trace's rules) -> one LM_TRIAL_DTYPE array per pair."""
+    n = get(None, C.c_size_t(0), None)
+    _check(min(n, 0))
+    offsets = np.empty(n + 1, np.int64)
+    rc = get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None)  # offsets only
+    if rc != ESTATE:
+        _check(rc)
+    trials = np.empty(int(offsets[-1]), LM_TRIAL_DTYPE)
+    _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(trials)), trials.ctypes.data_as(C.c_void_p)))
+    return [trials[offsets[i]:offsets[i + 1]] for i in range(n)]
+
+
+def _loop_clouds(get):
+    """The CSR clouds behind get(offsets, capacity, xyzi) (b200reg_loop_clouds' rules) -> one (n, 4) float32 array per pair."""
+    n = get(None, C.c_size_t(0), None)
+    _check(min(n, 0))
+    offsets = np.empty(n + 1, np.int64)
+    rc = get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None)  # offsets only
+    if rc != ESTATE:
+        _check(rc)
+    pts = np.empty((int(offsets[-1]), 4), np.float32)
+    _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(pts)), pts.ctypes.data_as(C.c_void_p)))
+    return [pts[offsets[i]:offsets[i + 1]] for i in range(n)]
 
 
 def loop_factor_from_poses(T_between, pose_latest, pose_closest, score, valid=True, from_idx=0, to_idx=0):
@@ -263,16 +290,7 @@ class Context:
     def lm_trace(self):
         """The trials of the last call that ran the LM solve: one LM_TRIAL_DTYPE array per pair of that call (the caller's
         pair order; empty for a pair whose fine stage did not run), each in execution order."""
-        n = lib().b200reg_lm_trace(self.h, None, C.c_size_t(0), None)
-        _check(min(n, 0))
-        offsets = np.empty(n + 1, np.int64)
-        rc = lib().b200reg_lm_trace(self.h, offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None)  # offsets only
-        if rc != ESTATE:
-            _check(rc)
-        trials = np.empty(int(offsets[-1]), LM_TRIAL_DTYPE)
-        _check(lib().b200reg_lm_trace(self.h, offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(trials)),
-                                      trials.ctypes.data_as(C.c_void_p)))
-        return [trials[offsets[i]:offsets[i + 1]] for i in range(n)]
+        return _lm_trace(lambda *a: lib().b200reg_lm_trace(self.h, *a))
 
     def set_loop_clouds(self, mask):
         """Capture the clouds loopTimerFunc publishes (an OR of CLOUD_SOURCE, CLOUD_TARGET, CLOUD_COARSE, CLOUD_FINAL; 0 turns
@@ -282,16 +300,7 @@ class Context:
     def loop_clouds(self, kind):
         """The clouds of one kind from the last capturing call: one (n, 4) float32 array (x, y, z, intensity) per pair of
         that call, in its pair order; empty where the reference has no such cloud (include/b200reg.h)."""
-        n = lib().b200reg_loop_clouds(self.h, int(kind), None, C.c_size_t(0), None)
-        _check(min(n, 0))
-        offsets = np.empty(n + 1, np.int64)
-        rc = lib().b200reg_loop_clouds(self.h, int(kind), offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None)  # offsets only
-        if rc != ESTATE:
-            _check(rc)
-        pts = np.empty((int(offsets[-1]), 4), np.float32)
-        _check(lib().b200reg_loop_clouds(self.h, int(kind), offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(pts)),
-                                         pts.ctypes.data_as(C.c_void_p)))
-        return [pts[offsets[i]:offsets[i + 1]] for i in range(n)]
+        return _loop_clouds(lambda *a: lib().b200reg_loop_clouds(self.h, int(kind), *a))
 
     # -- the path's one collective: all-gather of the result records over NCCL (SURVEY §8e) --------
     def comm_init(self, unique_id, rank, world):
@@ -714,10 +723,34 @@ class Batch:
         return t
 
     def wait_all(self):
-        """Waits for every job in flight; their results are dropped (wait() per ticket keeps them)."""
+        """Waits for every job in flight; their results, loop clouds and LM traces are dropped (wait() per ticket keeps
+        them)."""
         rc = lib().b200reg_batch_wait_all(self.h)
+        for t in self._keep:
+            lib().b200reg_batch_release(self.h, C.c_int64(t))
         self._keep.clear()
         _check(rc)
+
+    def set_loop_clouds(self, mask):
+        """Capture the clouds loopTimerFunc publishes (an OR of CLOUD_*; 0 turns capture off) in the jobs submitted from now
+        on; each job copies the setting at submit.  Results do not change."""
+        _check(lib().b200reg_batch_set_loop_clouds(self.h, int(mask)))
+
+    def set_lm_trace(self, enable):
+        """Record every LM trial of the jobs submitted from now on; each job copies the setting at submit."""
+        _check(lib().b200reg_batch_set_lm_trace(self.h, int(bool(enable))))
+
+    def loop_clouds(self, ticket, kind):
+        """The clouds of one kind a waited-for job captured, as Context.loop_clouds returns them after the synchronous call."""
+        return _loop_clouds(lambda *a: lib().b200reg_batch_loop_clouds(self.h, C.c_int64(ticket), int(kind), *a))
+
+    def lm_trace(self, ticket):
+        """The LM trace of a waited-for job that traced, as Context.lm_trace returns it after the synchronous call."""
+        return _lm_trace(lambda *a: lib().b200reg_batch_lm_trace(self.h, C.c_int64(ticket), *a))
+
+    def release(self, ticket):
+        """Frees the loop clouds and LM trace a waited-for job holds (nothing to free is no error)."""
+        _check(lib().b200reg_batch_release(self.h, C.c_int64(ticket)))
 
     def wait(self, ticket, want_latency=False, want_quatro=False):
         lat = C.c_double()

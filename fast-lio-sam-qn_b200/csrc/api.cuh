@@ -224,6 +224,15 @@ int kf_job_run(b200reg_ctx* c, KfJob* j, b200reg_result* out, b200reg_quatro_inf
 // others get no records.  Does nothing but keep the trace invalid when tracing is off.  (api_gicp.cu)
 void lm_trace_remap(b200reg_ctx* c, int count, const std::vector<int>& where);
 
+// The copy-out rules of b200reg_lm_trace / b200reg_loop_clouds over one stored trace or set of clouds: a context's, or a
+// batch-driver job's (b200reg_batch_lm_trace / b200reg_batch_loop_clouds).  A kind that is not one B200REG_CLOUD_* bit is
+// B200REG_EINVAL; a null `tr` / `lc`, an invalid trace or a kind not held is B200REG_ESTATE with the message `none`;
+// then the CSR offsets and the capacity rule of include/b200reg.h.  (api_gicp.cu, api_loop_clouds.cu)
+int lm_trace_copy(const b200reg_ctx::LmTrace* tr, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out,
+                  const std::string& none);
+int loop_clouds_copy(const b200reg_ctx::LoopClouds* lc, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out,
+                     const std::string& none);
+
 // LoopClosure::coarseToFineAlignment on cloud handles (api_quatro.cu).  fine_tf16 (optional, count x 16): the fine stage's
 // own fp32 final transformation of each pair whose coarse stage is valid (the transform of align()'s output cloud)
 int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst,

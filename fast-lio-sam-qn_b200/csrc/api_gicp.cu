@@ -94,6 +94,18 @@ void lm_trace_remap(b200reg_ctx* c, int count, const std::vector<int>& where) {
   tr.trials.swap(trials);
   tr.valid = true;
 }
+
+int lm_trace_copy(const b200reg_ctx::LmTrace* tr, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out,
+                  const std::string& none) {
+  if (!tr || !tr->valid) return fail(B200REG_ESTATE, none);
+  const int pairs = (int)tr->offsets.size() - 1;
+  if (!offsets_out) return pairs;
+  memcpy(offsets_out, tr->offsets.data(), sizeof(int64_t) * tr->offsets.size());
+  if (tr->trials.size() > capacity)
+    return fail(B200REG_ESTATE, "LM trace holds " + std::to_string(tr->trials.size()) + " records, capacity " + std::to_string(capacity));
+  if (trials_out && !tr->trials.empty()) memcpy(trials_out, tr->trials.data(), sizeof(b200reg_lm_trial) * tr->trials.size());
+  return B200REG_OK;
+}
 }  // namespace b200
 
 // make the arena hold `count` pairs and make sure its graph exists
@@ -183,15 +195,8 @@ int b200reg_ctx_set_lm_trace(b200reg_ctx* c, int enable) {
 
 int b200reg_lm_trace(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out) {
   if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
-  const auto& tr = c->lm_trace;
-  if (!tr.valid) return fail(B200REG_ESTATE, "no LM trace: the context's last LM solve was not traced (b200reg_ctx_set_lm_trace)");
-  const int pairs = (int)tr.offsets.size() - 1;
-  if (!offsets_out) return pairs;
-  memcpy(offsets_out, tr.offsets.data(), sizeof(int64_t) * tr.offsets.size());
-  if (tr.trials.size() > capacity)
-    return fail(B200REG_ESTATE, "LM trace holds " + std::to_string(tr.trials.size()) + " records, capacity " + std::to_string(capacity));
-  if (trials_out && !tr.trials.empty()) memcpy(trials_out, tr.trials.data(), sizeof(b200reg_lm_trial) * tr.trials.size());
-  return B200REG_OK;
+  return lm_trace_copy(&c->lm_trace, offsets_out, capacity, trials_out,
+                       "no LM trace: the context's last LM solve was not traced (b200reg_ctx_set_lm_trace)");
 }
 
 int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* tgt,

@@ -104,6 +104,22 @@ int LoopCapture::finish(const b200reg_quatro_info* qi, const float* fine_tf16) {
   return B200REG_OK;
 }
 
+int loop_clouds_copy(const b200reg_ctx::LoopClouds* lc, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out,
+                     const std::string& none) {
+  int s = -1;
+  for (int b = 0; b < 4; b++)
+    if (kind == 1 << b) s = b;
+  if (s < 0) return fail(B200REG_EINVAL, "kind: one of B200REG_CLOUD_SOURCE, _TARGET, _COARSE, _FINAL");
+  if (!lc || !(lc->stored & kind)) return fail(B200REG_ESTATE, none);
+  const int pairs = (int)lc->offsets[s].size() - 1;
+  if (!offsets_out) return pairs;
+  memcpy(offsets_out, lc->offsets[s].data(), sizeof(int64_t) * lc->offsets[s].size());
+  if (lc->pts[s].size() > capacity)
+    return fail(B200REG_ESTATE, "loop clouds hold " + std::to_string(lc->pts[s].size()) + " points, capacity " + std::to_string(capacity));
+  if (xyzi_out && !lc->pts[s].empty()) memcpy(xyzi_out, lc->pts[s].data(), sizeof(float4) * lc->pts[s].size());
+  return B200REG_OK;
+}
+
 }  // namespace b200
 
 extern "C" {
@@ -118,20 +134,8 @@ int b200reg_ctx_set_loop_clouds(b200reg_ctx* c, int mask) {
 
 int b200reg_loop_clouds(b200reg_ctx* c, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out) {
   if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
-  int s = -1;
-  for (int b = 0; b < 4; b++)
-    if (kind == 1 << b) s = b;
-  if (s < 0) return fail(B200REG_EINVAL, "kind: one of B200REG_CLOUD_SOURCE, _TARGET, _COARSE, _FINAL");
-  const auto& lc = c->loop_clouds;
-  if (!(lc.stored & kind))
-    return fail(B200REG_ESTATE, "no such loop clouds: the context's last loop-closure call did not capture this kind (b200reg_ctx_set_loop_clouds)");
-  const int pairs = (int)lc.offsets[s].size() - 1;
-  if (!offsets_out) return pairs;
-  memcpy(offsets_out, lc.offsets[s].data(), sizeof(int64_t) * lc.offsets[s].size());
-  if (lc.pts[s].size() > capacity)
-    return fail(B200REG_ESTATE, "loop clouds hold " + std::to_string(lc.pts[s].size()) + " points, capacity " + std::to_string(capacity));
-  if (xyzi_out && !lc.pts[s].empty()) memcpy(xyzi_out, lc.pts[s].data(), sizeof(float4) * lc.pts[s].size());
-  return B200REG_OK;
+  return loop_clouds_copy(&c->loop_clouds, kind, offsets_out, capacity, xyzi_out,
+                          "no such loop clouds: the context's last loop-closure call did not capture this kind (b200reg_ctx_set_loop_clouds)");
 }
 
 }  // extern "C"

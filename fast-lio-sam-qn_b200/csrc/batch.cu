@@ -2,7 +2,8 @@
 // own host thread with its own CUDA streams and memory pool, take alternate jobs.  While one context waits for a PCIe
 // upload or polls its LM loop, the kernels of the others keep the SMs busy -- the batch-level concurrency SURVEY.md §8(d)
 // names as the lever for the HBM fraction.  Host code only; everything it calls is the public C ABI, except the jobs over
-// the keyframe store, which go through the job interface of api_keyframes.cu (api.cuh).
+// the keyframe store, which go through the job interface of api_keyframes.cu (api.cuh), and the loop clouds and LM trace
+// of a capturing job, which it moves out of the worker's context and reads with the context getters' copy-out (api.cuh).
 //
 // Reference context: the reference registers ONE pair per 2 Hz timer tick, serially, on one thread
 // (fast_lio_sam_qn/src/fast_lio_sam_qn.cpp:203-219, LoopClosure is not re-entrant, :81).
@@ -10,6 +11,7 @@
 #include <chrono>
 #include <condition_variable>
 #include <deque>
+#include <iterator>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -20,6 +22,20 @@
 #include "api.cuh"
 
 namespace {
+
+// A job's loop clouds and LM trace, moved out of its worker's context when the job ends: they outlive the wait, until
+// b200reg_batch_release or b200reg_batch_destroy
+struct Captured {
+  b200reg_ctx::LoopClouds clouds;
+  b200reg_ctx::LmTrace trace;
+};
+
+struct Capture {  // the capture settings of a job
+  int cloud_mask = 0;
+  bool lm_trace = false;
+  bool on() const { return cloud_mask || lm_trace; }
+  bool operator!=(const Capture& o) const { return cloud_mask != o.cloud_mask || lm_trace != o.lm_trace; }
+};
 
 struct Job {
   int kind = 0;  // 0 icpAlignment, 1 coarseToFineAlignment, 2 performLoopClosure over a keyframe store
@@ -33,6 +49,9 @@ struct Job {
   std::shared_ptr<KfJob> kfjob;  // kind 2: its arguments and the store's state at submit
   b200reg_result* out = nullptr;
   b200reg_quatro_info* qout = nullptr;
+  // the driver's capture settings at submit (b200reg_batch_set_loop_clouds / _set_lm_trace), and what the job captured
+  Capture capture;
+  std::shared_ptr<Captured> captured;
   // completion
   int status = 0;
   std::string error;
@@ -56,9 +75,14 @@ struct b200reg_batch {
   std::vector<std::unique_ptr<Worker>> workers;
   std::mutex mu;  // tickets / completion
   std::condition_variable cv_done;
-  std::map<int64_t, std::shared_ptr<Job>> jobs;
+  std::map<int64_t, std::shared_ptr<Job>> jobs;  // submitted, not waited for yet
   int64_t next_ticket = 0;
   size_t rr = 0;
+  // capture: the settings the next submit copies; the settings of every ticket (an entry where they changed, so a driver
+  // that never captures keeps none); the outputs of the waited-for jobs that captured (null: the job failed), until released
+  Capture capture;
+  std::map<int64_t, Capture> capture_from;
+  std::map<int64_t, std::shared_ptr<Captured>> kept;
 };
 
 static thread_local std::string g_batch_err;
@@ -73,16 +97,31 @@ static void run_worker(b200reg_batch* b, Worker* w) {
       j = w->q.front();
       w->q.pop_front();
     }
+    b200reg_ctx* c = w->ctx;
+    const bool capture = j->capture.on();
+    if (capture) {  // for this job only
+      c->loop_clouds.mask = j->capture.cloud_mask;
+      c->lm_trace.enabled = j->capture.lm_trace;
+    }
     int rc;
     if (j->kind == 0)
-      rc = b200reg_icp_alignment(w->ctx, j->count, j->src.data(), j->src_n.data(), j->tgt.data(), j->tgt_n.data(), j->stride, j->on_device,
+      rc = b200reg_icp_alignment(c, j->count, j->src.data(), j->src_n.data(), j->tgt.data(), j->tgt_n.data(), j->stride, j->on_device,
                                  &j->gp, j->out);
     else if (j->kind == 1)
-      rc = b200reg_loop_closure(w->ctx, j->count, j->src.data(), j->src_n.data(), j->tgt.data(), j->tgt_n.data(), j->stride, j->on_device,
+      rc = b200reg_loop_closure(c, j->count, j->src.data(), j->src_n.data(), j->tgt.data(), j->tgt_n.data(), j->stride, j->on_device,
                                 &j->qp, &j->gp, j->out, j->qout);
     else
-      rc = kf_job_run(w->ctx, j->kfjob.get(), j->out, j->qout);
+      rc = kf_job_run(c, j->kfjob.get(), j->out, j->qout);
     j->kfjob.reset();  // the store no longer counts the job as in flight: a wait that returns sees it finished
+    if (capture) {  // the job takes the stored outputs without a copy; nothing carries over to the worker's next job
+      if (!rc) {
+        j->captured = std::make_shared<Captured>();
+        std::swap(j->captured->clouds, c->loop_clouds);
+        std::swap(j->captured->trace, c->lm_trace);
+      }
+      c->loop_clouds = b200reg_ctx::LoopClouds();
+      c->lm_trace = b200reg_ctx::LmTrace();
+    }
     {
       std::lock_guard<std::mutex> lk(b->mu);
       j->status = rc;
@@ -134,9 +173,12 @@ static int64_t submit(b200reg_batch* b, std::shared_ptr<Job> j) {
   j->t_submit = std::chrono::steady_clock::now();
   int64_t ticket;
   Worker* w;
+  j->capture = b->capture;
   {
     std::lock_guard<std::mutex> lk(b->mu);
     ticket = b->next_ticket++;
+    const Capture prev = b->capture_from.empty() ? Capture() : b->capture_from.rbegin()->second;
+    if (b->capture != prev) b->capture_from[ticket] = b->capture;
     b->jobs[ticket] = j;
     w = b->workers[b->rr].get();
     b->rr = (b->rr + 1) % b->workers.size();
@@ -210,6 +252,7 @@ int b200reg_batch_wait(b200reg_batch* b, int64_t ticket, double* latency_ms) {
     j = it->second;
     b->cv_done.wait(lk, [&] { return j->done; });
     b->jobs.erase(it);
+    if (j->capture.on()) b->kept[ticket] = std::move(j->captured);
   }
   if (latency_ms) *latency_ms = std::chrono::duration<double, std::milli>(j->t_done - j->t_submit).count();
   if (j->status) b200reg_set_last_error(j->error.c_str());
@@ -230,6 +273,80 @@ int b200reg_batch_wait_all(b200reg_batch* b) {
     if (rc && !first) first = rc;
   }
   return first;
+}
+
+int b200reg_batch_set_loop_clouds(b200reg_batch* b, int mask) {
+  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
+  if (mask & ~(B200REG_CLOUD_SOURCE | B200REG_CLOUD_TARGET | B200REG_CLOUD_COARSE | B200REG_CLOUD_FINAL))
+    return fail(B200REG_EINVAL, "mask: an OR of B200REG_CLOUD_SOURCE, _TARGET, _COARSE, _FINAL");
+  b->capture.cloud_mask = mask;
+  return B200REG_OK;
+}
+
+int b200reg_batch_set_lm_trace(b200reg_batch* b, int enable) {
+  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
+  b->capture.lm_trace = enable != 0;
+  return B200REG_OK;
+}
+
+}  // extern "C"
+
+// The outputs the getters read for `ticket` (the pointer keeps them alive while they are copied out, outside the lock), or
+// null; `none` is the getters' message when the output is missing, saying why.  kind: a B200REG_CLOUD_* bit, or 0 for the
+// LM trace.  B200REG_EINVAL for a ticket never handed out.
+static int find_captured(b200reg_batch* b, int64_t ticket, int kind, std::shared_ptr<Captured>* out, std::string* none) {
+  const std::string missing = std::string(kind ? "no such loop clouds: " : "no LM trace: ") + "batch job " + std::to_string(ticket);
+  const std::string off = kind ? " did not capture this kind (b200reg_batch_set_loop_clouds at its submit)"
+                               : " was not traced (b200reg_batch_set_lm_trace at its submit)";
+  std::lock_guard<std::mutex> lk(b->mu);
+  if (ticket < 0 || ticket >= b->next_ticket) return fail(B200REG_EINVAL, "ticket " + std::to_string(ticket) + " was never handed out");
+  if (b->jobs.count(ticket)) {
+    *none = missing + " has not been waited for yet (b200reg_batch_wait)";
+    return B200REG_OK;
+  }
+  const auto k = b->kept.find(ticket);
+  if (k != b->kept.end()) {
+    *out = k->second;
+    *none = missing + (k->second ? off : " failed");
+    return B200REG_OK;
+  }
+  const auto s = b->capture_from.upper_bound(ticket);  // the settings the job copied at its submit
+  const Capture cap = s == b->capture_from.begin() ? Capture() : std::prev(s)->second;
+  const bool wanted = kind ? (cap.cloud_mask & kind) != 0 : cap.lm_trace;
+  *none = missing + (wanted ? " was released (b200reg_batch_release)" : off);
+  return B200REG_OK;
+}
+
+extern "C" {
+
+int b200reg_batch_loop_clouds(b200reg_batch* b, int64_t ticket, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out) {
+  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
+  std::shared_ptr<Captured> cap;
+  std::string none;
+  if (const int rc = find_captured(b, ticket, kind, &cap, &none)) return rc;
+  return loop_clouds_copy(cap ? &cap->clouds : nullptr, kind, offsets_out, capacity, xyzi_out, none);
+}
+
+int b200reg_batch_lm_trace(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out) {
+  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
+  std::shared_ptr<Captured> cap;
+  std::string none;
+  if (const int rc = find_captured(b, ticket, 0, &cap, &none)) return rc;
+  return lm_trace_copy(cap ? &cap->trace : nullptr, offsets_out, capacity, trials_out, none);
+}
+
+int b200reg_batch_release(b200reg_batch* b, int64_t ticket) {
+  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
+  std::shared_ptr<Captured> drop;  // freed after the lock is released
+  std::lock_guard<std::mutex> lk(b->mu);
+  if (ticket < 0 || ticket >= b->next_ticket) return fail(B200REG_EINVAL, "ticket " + std::to_string(ticket) + " was never handed out");
+  if (b->jobs.count(ticket)) return fail(B200REG_ESTATE, "batch job " + std::to_string(ticket) + " has not been waited for yet (b200reg_batch_wait)");
+  const auto k = b->kept.find(ticket);
+  if (k != b->kept.end()) {
+    drop = std::move(k->second);
+    b->kept.erase(k);
+  }
+  return B200REG_OK;
 }
 
 int64_t b200reg_batch_launch_count(const b200reg_batch* b) {

@@ -443,8 +443,8 @@ int64_t b200reg_batch_submit_loop_closure(b200reg_batch* b, int count, const flo
  *     with a candidate), a candidate above its query, num_submap_keyframes or voxel_res out of range, and a store on
  *     another device than the driver.  Everything else (Quatro and GICP parameter refusals, device failures) comes back
  *     from b200reg_batch_wait with its message.
- *   Threads: submits, keyframe adds and pose rewrites of a store that jobs read come from ONE host thread.  Loop-cloud
- *     capture and LM tracing belong to a caller's context and are not available on driver jobs.                      */
+ *   Threads: submits, keyframe adds and pose rewrites of a store that jobs read come from ONE host thread.
+ *   Loop clouds and LM trace: as for the other two job kinds, b200reg_batch_set_loop_clouds / _set_lm_trace (below).  */
 int64_t b200reg_batch_submit_perform_loop_closure(b200reg_batch* b, b200reg_keyframes* kf, int count,
                                                   const int32_t* query_idx, const int32_t* closest_idx,
                                                   const b200reg_loop_config* cfg, b200reg_result* out,
@@ -453,6 +453,36 @@ int64_t b200reg_batch_submit_perform_loop_closure(b200reg_batch* b, b200reg_keyf
  * latency_ms (optional): submit -> completion on the host clock.  A ticket can be waited for once.               */
 int b200reg_batch_wait(b200reg_batch* b, int64_t ticket, double* latency_ms);
 int b200reg_batch_wait_all(b200reg_batch* b);
+/* Loop clouds and LM trace of driver jobs, all three kinds: what b200reg_ctx_set_loop_clouds / b200reg_ctx_set_lm_trace
+ * capture on a context, per job.
+ *   Settings: the kinds to capture (an OR of B200REG_CLOUD_*) and the tracing flag, both off by default, set from the
+ *     submitting thread.  A job copies them at submit, as it copies the store's state, and applies them to its worker's
+ *     context for its own run; changing them later does not affect it.
+ *   Same bytes: a job's clouds of each kind and its trace equal, byte for byte, what b200reg_loop_clouds / b200reg_lm_trace
+ *     return on a context after the synchronous call with the same inputs, mask and tracing -- at every driver depth,
+ *     empty rows included (e.g. SOURCE / TARGET of an icpAlignment job), rows in the caller's pair or query order.  A
+ *     b200reg_batch_submit_perform_loop_closure job with closest_idx NULL compares with b200reg_fetch_closest_keyframes
+ *     followed by b200reg_perform_loop_closure.  Capture changes no result or Quatro record.
+ *   Off costs nothing: a job with both settings off allocates nothing more, launches nothing more and keeps nothing.
+ *   No carry-over: a worker runs jobs of different settings back to back; each job sees its own outputs only, moved out of
+ *     the worker's context (no copy) when it ends.  No new kernel: the same capture and trace run on the worker.
+ *   Lifetime: the outputs of a job that captured are readable once b200reg_batch_wait (or _wait_all) has returned for its
+ *     ticket, until b200reg_batch_release(ticket) or b200reg_batch_destroy.  Errors inside a job (e.g. a trace or capture
+ *     buffer that cannot be allocated) come back from b200reg_batch_wait with their message; such a job keeps nothing.
+ *   Getters: the rules of b200reg_loop_clouds / b200reg_lm_trace (CSR over the job's pairs, offsets_out NULL returns the
+ *     pair count, a total above `capacity` fills offsets_out only and returns B200REG_ESTATE; a kind that is not one
+ *     B200REG_CLOUD_* bit: B200REG_EINVAL).  A ticket never handed out: B200REG_EINVAL.  A ticket not waited for yet, a
+ *     job that failed, a kind it did not capture, tracing off at its submit, or a released ticket: B200REG_ESTATE, the
+ *     message says which.
+ *   Release: B200REG_OK for any waited-for ticket, also one that holds nothing, and again for a released one;
+ *     B200REG_ESTATE before its wait; B200REG_EINVAL for a ticket never handed out.                                   */
+int b200reg_batch_set_loop_clouds(b200reg_batch* b, int mask);
+int b200reg_batch_set_lm_trace(b200reg_batch* b, int enable);
+int b200reg_batch_loop_clouds(b200reg_batch* b, int64_t ticket, int kind, int64_t* offsets_out, size_t capacity,
+                              float* xyzi_out);
+int b200reg_batch_lm_trace(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity,
+                           b200reg_lm_trial* trials_out);
+int b200reg_batch_release(b200reg_batch* b, int64_t ticket);
 int64_t b200reg_batch_launch_count(const b200reg_batch* b);
 int b200reg_batch_depth(const b200reg_batch* b);
 
