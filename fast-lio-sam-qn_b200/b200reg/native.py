@@ -118,6 +118,7 @@ EXPORTS = [
     "b200reg_match_tap", "b200reg_lm_step_tap", "b200reg_index_tap", "b200reg_sort_tap",
     "b200reg_batch_submit_perform_loop_closure", "b200reg_batch_set_loop_clouds", "b200reg_batch_set_lm_trace",
     "b200reg_batch_loop_clouds", "b200reg_batch_lm_trace", "b200reg_batch_release",
+    "b200reg_ctx_set_quatro_matches", "b200reg_quatro_matches", "b200reg_batch_set_quatro_matches", "b200reg_batch_quatro_matches",
 ]
 ESTATE = -4  # B200REG_ESTATE
 # B200REG_CLOUD_*: the loop clouds (Context.set_loop_clouds / Context.loop_clouds)
@@ -200,6 +201,22 @@ def _loop_clouds(get):
     pts = np.empty((int(offsets[-1]), 4), np.float32)
     _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(pts)), pts.ctypes.data_as(C.c_void_p)))
     return [pts[offsets[i]:offsets[i + 1]] for i in range(n)]
+
+
+def _quatro_matches(get):
+    """The CSR matches behind get(offsets, capacity, corr, inlier, src_xyz, dst_xyz) (b200reg_quatro_matches' rules) -> one
+    dict per pair: corr (m, 2) int32 (src, dst), inlier (m,) int32, src_xyz and dst_xyz (m, 3) float32."""
+    n = get(None, C.c_size_t(0), None, None, None, None)
+    _check(min(n, 0))
+    offsets = np.empty(n + 1, np.int64)
+    rc = get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None, None, None, None)  # offsets only
+    if rc != ESTATE:
+        _check(rc)
+    m = int(offsets[-1])
+    corr, inlier = np.empty((m, 2), np.int32), np.empty(m, np.int32)
+    sx, dx = np.empty((m, 3), np.float32), np.empty((m, 3), np.float32)
+    _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(m), *(a.ctypes.data_as(C.c_void_p) for a in (corr, inlier, sx, dx))))
+    return [dict(corr=corr[a:b], inlier=inlier[a:b], src_xyz=sx[a:b], dst_xyz=dx[a:b]) for a, b in zip(offsets[:-1], offsets[1:])]
 
 
 def loop_factor_from_poses(T_between, pose_latest, pose_closest, score, valid=True, from_idx=0, to_idx=0):
@@ -301,6 +318,16 @@ class Context:
         """The clouds of one kind from the last capturing call: one (n, 4) float32 array (x, y, z, intensity) per pair of
         that call, in its pair order; empty where the reference has no such cloud (include/b200reg.h)."""
         return _loop_clouds(lambda *a: lib().b200reg_loop_clouds(self.h, int(kind), *a))
+
+    def set_quatro_matches(self, enable):
+        """Record the Quatro correspondences and max-clique inliers of the following quatro_align / loop_closure /
+        perform_loop_closure calls; results do not change."""
+        _check(lib().b200reg_ctx_set_quatro_matches(self.h, int(bool(enable))))
+
+    def quatro_matches(self):
+        """The matches of the last recording call: per pair of that call (its pair or query order) a dict of corr (m, 2),
+        inlier (m,), src_xyz (m, 3) and dst_xyz (m, 3); empty where no Quatro stage ran (include/b200reg.h)."""
+        return _quatro_matches(lambda *a: lib().b200reg_quatro_matches(self.h, *a))
 
     # -- the path's one collective: all-gather of the result records over NCCL (SURVEY §8e) --------
     def comm_init(self, unique_id, rank, world):
@@ -747,6 +774,15 @@ class Batch:
     def lm_trace(self, ticket):
         """The LM trace of a waited-for job that traced, as Context.lm_trace returns it after the synchronous call."""
         return _lm_trace(lambda *a: lib().b200reg_batch_lm_trace(self.h, C.c_int64(ticket), *a))
+
+    def set_quatro_matches(self, enable):
+        """Record the Quatro matches of the jobs submitted from now on (copied at submit)."""
+        _check(lib().b200reg_batch_set_quatro_matches(self.h, int(bool(enable))))
+
+    def quatro_matches(self, ticket):
+        """The Quatro matches of a waited-for job that recorded them, as Context.quatro_matches returns them after the
+        synchronous call."""
+        return _quatro_matches(lambda *a: lib().b200reg_batch_quatro_matches(self.h, C.c_int64(ticket), *a))
 
     def release(self, ticket):
         """Frees the loop clouds and LM trace a waited-for job holds (nothing to free is no error)."""

@@ -70,6 +70,15 @@ struct b200reg_ctx {
     std::vector<int64_t> offsets[4];  // pairs + 1 each
     std::vector<float4> pts[4];       // (x, y, z, intensity)
   } loop_clouds;
+  // Quatro matches (b200reg_ctx_set_quatro_matches / b200reg_quatro_matches) of the most recent call that reached the Quatro
+  // stage with recording on, CSR over its pairs, on the host.  `words` holds four blocks over all `total` matches, as the
+  // capture slab does: corr (2 per match), inlier (1), src xyz (3 float bits), dst xyz (3 float bits)
+  struct QuatroMatches {
+    bool enabled = false;
+    bool valid = false;  // false before a recording call, after one that did not record and after one that failed
+    std::vector<int64_t> offsets;  // pairs + 1
+    std::vector<int32_t> words;    // 9 per match
+  } quatro_matches;
   // the path's one collective (b200reg_comm_*): NCCL communicator of this rank
   ncclComm_t comm = nullptr;
   int rank = -1, world = 1;
@@ -232,6 +241,15 @@ int lm_trace_copy(const b200reg_ctx::LmTrace* tr, int64_t* offsets_out, size_t c
                   const std::string& none);
 int loop_clouds_copy(const b200reg_ctx::LoopClouds* lc, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out,
                      const std::string& none);
+
+// The stored Quatro matches belong to the pairs of the last b200reg_quatro_align.  A caller that ran it on a subset of its
+// `count` pairs (Quatro pair k = its pair where[k]; `where` empty when no Quatro stage ran) renumbers them to its own pairs;
+// the others get empty rows.  Does nothing but keep them invalid when recording is off.  (api_quatro.cu)
+void quatro_matches_remap(b200reg_ctx* c, int count, const std::vector<int>& where);
+// The copy-out rules of b200reg_quatro_matches over a context's or a batch-driver job's record (b200reg_batch_quatro_matches):
+// a null or invalid record is B200REG_ESTATE with the message `none`; then the CSR offsets and the capacity rule.
+int quatro_matches_copy(const b200reg_ctx::QuatroMatches* qm, int64_t* offsets_out, size_t capacity, int32_t* corr_out,
+                        int32_t* inlier_out, float* src_xyz_out, float* dst_xyz_out, const std::string& none);
 
 // LoopClosure::coarseToFineAlignment on cloud handles (api_quatro.cu).  fine_tf16 (optional, count x 16): the fine stage's
 // own fp32 final transformation of each pair whose coarse stage is valid (the transform of align()'s output cloud)

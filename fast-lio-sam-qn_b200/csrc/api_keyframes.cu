@@ -476,6 +476,7 @@ extern "C" {
 
 int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
                                  const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out) {
+  if (c) c->quatro_matches.valid = false;  // a refused call holds no matches either
   if (!c || !kf || count <= 0 || !query_idx || !closest_idx || !cfg || !out) return fail(B200REG_EINVAL, "bad argument");
   return perform_loop_closure(c, kf->st, count, query_idx, closest_idx, cfg, out, quatro_out);
 }
@@ -486,6 +487,7 @@ int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int coun
 static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
                                 const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out) {
   LoopCapture cap(c, count);
+  c->quatro_matches.valid = false;  // its Quatro stage records them for its subset; renumbered below, dropped on failure
   std::vector<int32_t> qs, cs;
   std::vector<int> where;
   for (int i = 0; i < count; i++) {
@@ -499,7 +501,10 @@ static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, co
   }
   if (qs.empty()) {
     lm_trace_remap(c, count, where);
-    return cap.finish(nullptr, nullptr);
+    quatro_matches_remap(c, count, where);
+    const int rc = cap.finish(nullptr, nullptr);
+    if (rc) c->quatro_matches.valid = false;
+    return rc;
   }
   const int m = (int)qs.size();
   // at the time query q was the latest keyframe the vector held q + 1 keyframes (fast_lio_sam_qn.cpp:205-219); a batch
@@ -527,7 +532,9 @@ static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, co
     if (quatro_out && cfg->enable_quatro) quatro_out[where[k]] = qi[k];
   }
   if (!rc) lm_trace_remap(c, count, where);
+  if (!rc) quatro_matches_remap(c, count, cfg->enable_quatro ? where : std::vector<int>());
   if (!rc) rc = cap.finish(cfg->enable_quatro ? qi.data() : nullptr, fine_tf.data());
+  if (rc) c->quatro_matches.valid = false;
   return rc;
 }
 

@@ -206,7 +206,9 @@ static QuatroParamsDev quatro_params_dev(const b200reg_quatro_params* prm, bool 
   return q;
 }
 
-// one b200reg_quatro_align call: every pair's device workspace and, after each pass, its counters and out[i].T
+// one b200reg_quatro_align call: every pair's device workspace and, after each pass, its counters and out[i].T.  A call
+// that records its matches (b200reg_ctx_set_quatro_matches) also keeps where each pair's clique list lives, the CSR
+// offsets of its matches and the slab the capture writes.
 struct QuatroCall {
   b200reg_ctx* c;
   Scratch& scratch;
@@ -214,6 +216,10 @@ struct QuatroCall {
   b200reg_quatro_info* out;
   std::vector<MatchDev> pairs;
   std::vector<MatchCounters> counters;
+  bool record;
+  std::vector<const int*> clique_at;  // pair i's clique list once it is solved
+  std::vector<int64_t> rec_offsets;   // pairs + 1
+  char* rec_slab = nullptr;
 };
 
 // the size of a pair's final correspondence set: n_wide while the wide tier has the pair pending
@@ -246,6 +252,7 @@ static int match_and_solve_first(QuatroCall& qc, int count, b200reg_cloud* const
   const int opt_cap = std::max(MAXC, qc.q.max_corres + 3);
   qc.pairs.resize(count);
   qc.counters.resize(count);
+  qc.clique_at.assign(count, nullptr);
   std::vector<BigSolveWs> big_host;
   big_host.reserve(count);  // addresses stay valid for the async copies below
   int max_ni = 0, max_nj = 0;
@@ -257,16 +264,23 @@ static int match_and_solve_first(QuatroCall& qc, int count, b200reg_cloud* const
     m.swapped = swapped ? 1 : 0;
     const size_t ni = m.fi.n, nj = m.fj.n;
     const int cap = advanced ? solve_ws_cap(SolveTier::first, (int)nj) : 0;
+    // a recording call gives each optimizedMatching pair a clique row as long as its out_corr: k_teaser_solve, or
+    // k_big_finish for a set beyond MAXC, lists the clique there.  advancedMatching's stays in its workspace.
+    const bool clique_row = qc.record && !advanced;
     Layout l;
     const MatchLayout ml(l, ni, nj, advanced ? cap : opt_cap);
     const size_t o_big = advanced ? l.take(sizeof(BigSolveWs)) : 0;
     const BigWsLayout wl(l, cap, 0);  // empty when !advanced
+    const size_t o_clq = clique_row ? l.take((size_t)opt_cap * 4) : 0;
     char* slab = nullptr;
     CU(qc.scratch.alloc((void**)&slab, l.size));
     ml.bind(slab, m);
+    if (clique_row) m.clique = (int*)(slab + o_clq);
+    qc.clique_at[i] = m.clique;
     if (advanced) {
       m.big = (BigSolveWs*)(slab + o_big);
       big_host.push_back(wl.bind(slab));
+      qc.clique_at[i] = big_host.back().clique;
       CU(cudaMemcpyAsync(m.big, &big_host.back(), sizeof(BigSolveWs), cudaMemcpyHostToDevice, s));
     }
     max_ni = std::max(max_ni, (int)ni);
@@ -361,7 +375,7 @@ static int solve_wide(QuatroCall& qc, const std::vector<int>& wide, int32_t* cor
     for (size_t k = 0; k < wide.size(); k++) {
       const int i = wide[k], n = qc.counters[i].n_wide;
       views[k] = qc.pairs[i];
-      views[k].out_corr = (int*)(slab + o_oc);
+      if (!qc.record) views[k].out_corr = (int*)(slab + o_oc);  // a recording call gave each pair rows of its own (record_begin)
       views[k].big = (BigSolveWs*)(slab + o_big);
       CU(cudaMemcpyAsync(slab + o_pair, &views[k], sizeof(MatchDev), cudaMemcpyHostToDevice, s));
       qc.c->launches += launch_adv_wide((const MatchDev*)(slab + o_pair), n, qc.q, s);
@@ -374,12 +388,88 @@ static int solve_wide(QuatroCall& qc, const std::vector<int>& wide, int32_t* cor
   return B200REG_OK;
 }
 
+// A recording call, once every pair is matched: the CSR offsets of the final sets, and one slab for the capture's rows
+// and, ahead of solve_wide, for each wide pair's set and clique list (its workspace is shared with the next wide pair).
+static int record_begin(QuatroCall& qc, int count) {
+  qc.rec_offsets.assign(count + 1, 0);
+  for (int i = 0; i < count; i++) qc.rec_offsets[i + 1] = qc.rec_offsets[i] + set_size(qc.counters[i]);
+  const size_t total = (size_t)qc.rec_offsets[count];
+  Layout l;
+  l.take(total * 9 * 4);  // corr, inlier, src xyz, dst xyz: MatchCaptureOut
+  std::vector<size_t> o_wide(count, 0);
+  for (int i = 0; i < count; i++)
+    if (qc.counters[i].n_wide > 0) o_wide[i] = l.take((size_t)qc.counters[i].n_wide * 3 * 4);
+  if (qc.scratch.alloc((void**)&qc.rec_slab, l.size) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(B200REG_ECUDA, "Quatro matches: cannot allocate " + std::to_string(l.size) + " bytes");
+  }
+  for (int i = 0; i < count; i++)
+    if (qc.counters[i].n_wide > 0) {
+      qc.pairs[i].out_corr = (int*)(qc.rec_slab + o_wide[i]);
+      qc.pairs[i].clique = qc.pairs[i].out_corr + 2 * (size_t)qc.counters[i].n_wide;
+      qc.clique_at[i] = qc.pairs[i].clique;
+    }
+  return B200REG_OK;
+}
+
+// A recording call, once every pair is solved: every match row into the slab in one launch, one copy to the host, and
+// the context's record replaced
+static int record_finish(QuatroCall& qc, int count) {
+  b200reg_ctx* c = qc.c;
+  const int64_t total = qc.rec_offsets[count];
+  MatchCaptureOut o;
+  o.corr = (int*)qc.rec_slab;
+  o.inlier = o.corr + 2 * total;
+  o.sxyz = (float*)(o.inlier + total);
+  o.dxyz = o.sxyz + 3 * total;
+  std::vector<MatchCaptureRow> rows;
+  int max_n = 0;
+  for (int i = 0; i < count; i++) {
+    const int n = (int)(qc.rec_offsets[i + 1] - qc.rec_offsets[i]);
+    if (n == 0) continue;
+    const MatchDev& p = qc.pairs[i];
+    const CloudDev& sd = p.swapped ? p.fj : p.fi;
+    const CloudDev& dd = p.swapped ? p.fi : p.fj;
+    MatchCaptureRow r;
+    r.corr = p.out_corr;
+    r.clique = qc.clique_at[i];
+    r.spts = sd.pts;
+    r.srank = sd.rank;
+    r.dpts = dd.pts;
+    r.drank = dd.rank;
+    r.n = n;
+    r.m = qc.counters[i].clique_size;
+    r.off = qc.rec_offsets[i];
+    rows.push_back(r);
+    max_n = std::max(max_n, n);
+  }
+  auto& qm = c->quatro_matches;
+  qm.words.resize((size_t)total * 9);
+  if (!rows.empty()) {
+    MatchCaptureRow* d_rows = nullptr;
+    CU(qc.scratch.upload(&d_rows, rows.data(), sizeof(MatchCaptureRow) * rows.size()));
+    {
+      ProfScope ps(c, CLS_MISC);
+      launch_match_capture(d_rows, (int)rows.size(), max_n, o, c->stream);
+      c->launches++;
+      c->prof_bytes[CLS_MISC] += 76.0 * total;  // 8 corr + 32 points + ~4 clique in, 36 out
+    }
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(qm.words.data(), qc.rec_slab, qm.words.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+  }
+  CU(cudaStreamSynchronize(c->stream));
+  qm.offsets = qc.rec_offsets;
+  qm.valid = true;
+  return B200REG_OK;
+}
+
 // b200reg_quatro_align (corr_fixed: count x 2 x CAP ints, or NULL) and b200reg_quatro_align_ex (offsets_out non-NULL;
 // corr_csr: `capacity` pairs, or NULL).  Every pair is matched and, if its set holds at most BIGC correspondences,
 // solved in one batched pass.  A larger advancedMatching set is then solved by solve_wide.  optimizedMatching keeps at
 // most max_corres + 3 <= BIGC: k_teaser_solve solves the sets of at most MAXC in that pass, and solve_opt_big the rest.
 static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst, const b200reg_quatro_params* prm,
                       b200reg_quatro_info* out, int32_t* corr_fixed, int64_t* offsets_out, size_t capacity, int32_t* corr_csr) {
+  if (c) c->quatro_matches.valid = false;  // only a call that records and succeeds holds matches
   if (!c || count <= 0 || !src || !dst || !prm || !out) return fail(B200REG_EINVAL, "bad argument");
   if (prm->estimate_scale) return fail(B200REG_EINVAL, "estimate_scale is not supported (the deployment sets it false)");
   const bool advanced = !prm->use_optimized_matching;  // Matcher::advancedMatching (matcher.cc:118-356)
@@ -398,7 +488,7 @@ static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* sr
     }
     if ((rc = b200reg_clouds_fpfh(c, (int)all.size(), all.data(), prm->fpfh_normal_radius, prm->fpfh_radius))) return rc;
   }
-  QuatroCall qc{c, scratch, quatro_params_dev(prm, advanced), out, {}, {}};
+  QuatroCall qc{c, scratch, quatro_params_dev(prm, advanced), out, {}, {}, c->quatro_matches.enabled, {}, {}};
   if ((rc = match_and_solve_first(qc, count, src, dst, corr_stride, corr_fixed))) return rc;
   std::vector<int> big, wide;
   for (int i = 0; i < count; i++) {
@@ -435,10 +525,59 @@ static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* sr
         if (qc.counters[i].n_wide == 0 && qc.counters[i].n_corr > 0)
           CU(cudaMemcpyAsync(corr_csr + 2 * offsets[i], qc.pairs[i].out_corr, (size_t)qc.counters[i].n_corr * 8, cudaMemcpyDeviceToHost, s));
   }
+  if (qc.record && (rc = record_begin(qc, count))) return rc;
   if (!big.empty() && (rc = solve_opt_big(qc, big))) return rc;
   if (!wide.empty() && (rc = solve_wide(qc, wide, corr_csr, offsets))) return rc;
   CU(cudaStreamSynchronize(s));
   for (int i = 0; i < count; i++) fill_info(qc.counters[i], out[i]);
+  return qc.record ? record_finish(qc, count) : B200REG_OK;
+}
+
+void quatro_matches_remap(b200reg_ctx* c, int count, const std::vector<int>& where) {
+  auto& qm = c->quatro_matches;
+  if (!qm.enabled) {
+    qm.valid = false;
+    return;
+  }
+  const size_t total = where.empty() ? 0 : (size_t)qm.offsets.back();
+  std::vector<int> solved(count, -1);  // caller pair -> Quatro pair
+  for (size_t k = 0; k < where.size(); k++) solved[where[k]] = (int)k;
+  std::vector<int64_t> offsets(count + 1, 0);
+  for (int i = 0; i < count; i++) offsets[i + 1] = offsets[i] + (solved[i] >= 0 ? qm.offsets[solved[i] + 1] - qm.offsets[solved[i]] : 0);
+  // each of the four blocks keeps its words per match; rows move from Quatro order to caller order within it
+  static const int kWords[4] = {2, 1, 3, 3};
+  std::vector<int32_t> words(9 * (size_t)offsets[count]);
+  size_t from = 0, to = 0;
+  for (int b = 0; b < 4; b++) {
+    const int w = kWords[b];
+    for (int i = 0; i < count; i++) {
+      const int k = solved[i];
+      if (k < 0) continue;
+      std::copy(qm.words.begin() + from + w * qm.offsets[k], qm.words.begin() + from + w * qm.offsets[k + 1],
+                words.begin() + to + w * offsets[i]);
+    }
+    from += w * total;
+    to += w * (size_t)offsets[count];
+  }
+  qm.offsets.swap(offsets);
+  qm.words.swap(words);
+  qm.valid = true;
+}
+
+int quatro_matches_copy(const b200reg_ctx::QuatroMatches* qm, int64_t* offsets_out, size_t capacity, int32_t* corr_out,
+                        int32_t* inlier_out, float* src_xyz_out, float* dst_xyz_out, const std::string& none) {
+  if (!qm || !qm->valid) return fail(B200REG_ESTATE, none);
+  const int pairs = (int)qm->offsets.size() - 1;
+  if (!offsets_out) return pairs;
+  memcpy(offsets_out, qm->offsets.data(), sizeof(int64_t) * qm->offsets.size());
+  const size_t total = (size_t)qm->offsets.back();
+  if (total > capacity)
+    return fail(B200REG_ESTATE, "Quatro matches number " + std::to_string(total) + ", capacity " + std::to_string(capacity));
+  const int32_t* w = qm->words.data();
+  if (corr_out && total) memcpy(corr_out, w, total * 8);
+  if (inlier_out && total) memcpy(inlier_out, w + 2 * total, total * 4);
+  if (src_xyz_out && total) memcpy(src_xyz_out, w + 3 * total, total * 12);
+  if (dst_xyz_out && total) memcpy(dst_xyz_out, w + 6 * total, total * 12);
   return B200REG_OK;
 }
 }  // namespace b200
@@ -720,6 +859,7 @@ int b200reg_match_tap(b200reg_ctx* c, int count, const float* const* fi, const i
 int b200reg_loop_closure(b200reg_ctx* c, int count, const float* const* src_xyz, const size_t* src_n, const float* const* tgt_xyz,
                          const size_t* tgt_n, size_t stride_bytes, int on_device, const b200reg_quatro_params* qp,
                          const b200reg_gicp_params* gp, b200reg_result* out, b200reg_quatro_info* quatro_out) {
+  if (c) c->quatro_matches.valid = false;  // its Quatro stage records them, and a later failure drops them again
   if (!c || count <= 0 || !src_xyz || !src_n || !tgt_xyz || !tgt_n || !qp || !gp || !out) return fail(B200REG_EINVAL, "bad argument");
   CU(cudaSetDevice(c->device));
   LoopCapture cap(c, count);
@@ -732,7 +872,22 @@ int b200reg_loop_closure(b200reg_ctx* c, int count, const float* const* src_xyz,
   std::vector<float> fine_tf(cap.on() ? 16 * (size_t)count : 0);
   if (!rc) rc = coarse_to_fine_on_clouds(c, count, sc.data(), tc.data(), qp, gp, out, qi, cap.on() ? fine_tf.data() : nullptr);
   if (!rc) rc = cap.finish(qi, fine_tf.data());
+  if (rc) c->quatro_matches.valid = false;
   return rc;
+}
+
+int b200reg_ctx_set_quatro_matches(b200reg_ctx* c, int enable) {
+  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
+  c->quatro_matches.enabled = enable != 0;
+  return B200REG_OK;
+}
+
+int b200reg_quatro_matches(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, int32_t* corr_out, int32_t* inlier_out,
+                           float* src_xyz_out, float* dst_xyz_out) {
+  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
+  return quatro_matches_copy(&c->quatro_matches, offsets_out, capacity, corr_out, inlier_out, src_xyz_out, dst_xyz_out,
+                             "no Quatro matches: the context's last call with a Quatro stage did not record them, or failed "
+                             "(b200reg_ctx_set_quatro_matches)");
 }
 
 }  // extern "C"

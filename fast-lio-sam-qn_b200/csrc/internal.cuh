@@ -272,7 +272,26 @@ struct MatchDev {
                        // optimizedMatching, BigSolveWs::cap for advancedMatching)
   double* T;           // [16] row-major result
   struct BigSolveWs* big;  // global-memory solver workspace (advancedMatching only; nullptr otherwise)
-  int* clique;         // [MAXC] or nullptr: k_teaser_solve lists the clique here, ascending (b200reg_quatro_solve_tap)
+  int* clique;         // or nullptr: k_teaser_solve and k_big_finish also list the clique here, ascending
+                       // (b200reg_quatro_solve_tap; the rows of a call that records its matches)
+};
+
+// One pair of the Quatro-match capture (b200reg_quatro_matches): its final set of n (src, dst) ORIGINAL indices, the
+// ascending list of the m of them in the solve's max clique, the clouds they index, and its first row in the call's slab
+struct MatchCaptureRow {
+  const int* corr;     // [2 * n]
+  const int* clique;   // [m]
+  const float4 *spts, *dpts;  // sorted points; rank[original index] = sorted position
+  const int *srank, *drank;
+  int n, m;
+  long long off;
+};
+// the slab: four arrays over every row of the call
+struct MatchCaptureOut {
+  int* corr;     // [2 * rows]
+  int* inlier;   // [rows]
+  float* sxyz;   // [3 * rows]
+  float* dxyz;   // [3 * rows]
 };
 
 // Global-memory workspace of the multi-kernel TEASER++ solve used when the correspondence set is not capped at MAXC

@@ -51,6 +51,8 @@ int launch_big_solve(const MatchDev* d_pairs, int count, int max_n, const Quatro
 int launch_adv_wide(const MatchDev* d_pair, int n, const QuatroParamsDev& prm, cudaStream_t s);
 int launch_big_graph_solve(const MatchDev* d_pairs, int count, const QuatroParamsDev& prm, int n_wide, cudaStream_t s);
 void launch_transform_raw(const CloudDev* d_clouds, const double* d_T16s, int count, int max_n, float4* const* d_outs, cudaStream_t s);
+// Quatro-match capture: every row of every MatchCaptureRow of a call into `out` (max_n = the largest set)
+void launch_match_capture(const MatchCaptureRow* d_rows, int count, int max_n, MatchCaptureOut out, cudaStream_t s);
 
 // radius.cu: the stages of b200reg_radius_search (order, count, scan, fill, segmented sort); each returns its launches
 int launch_radius_query_keys(const CloudDev& c, const float* d_q, int nq, int qstride, uint32_t* keys, uint32_t* vals, cudaStream_t s);

@@ -1684,9 +1684,14 @@ __global__ void __launch_bounds__(1024) k_big_finish(const MatchDev* pairs, Quat
     }
     __syncthreads();
   }
-  // members in ascending ORIGINAL correspondence index
+  // members in ascending ORIGINAL correspondence index; also into the pair's own row when it has one (the wide tier shares
+  // W between pairs, so a call that records its matches keeps each clique there)
   const int m = block_compact(
-      n, [&](int v) { return W.alive[v] != 0; }, [&](int pos, int v) { W.clique[pos] = v; });
+      n, [&](int v) { return W.alive[v] != 0; },
+      [&](int pos, int v) {
+        W.clique[pos] = v;
+        if (P.clique) P.clique[pos] = v;
+      });
   if (tid == 0) P.counters->clique_size = m;
   if (m <= 1) return;  // solution_.valid stays false
   const int iters = gnc_tls_yaw<1024>(W.S, W.D, W.clique, m, W.w, W.res, red, gnc, prm);
@@ -1724,6 +1729,28 @@ __global__ void __launch_bounds__(256) k_transform_raw(const CloudDev* clouds, c
   const float4 p = src.pts[i];
   const float3 q = transform_pcd_point(T16s + 16 * blockIdx.y, p.x, p.y, p.z);
   outs[blockIdx.y][__float_as_int(p.w)] = make_float4(q.x, q.y, q.z, 1.f);
+}
+
+// The matches of a call that records them (b200reg_quatro_matches): row j of pair y is its correspondence j as
+// (src, dst), 1 iff j is in the ascending clique list, and the two points gathered as k_teaser_solve / k_big_gather do.
+__global__ void __launch_bounds__(256) k_match_capture(const MatchCaptureRow* rows, MatchCaptureOut out) {
+  const MatchCaptureRow& R = rows[blockIdx.y];
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= R.n) return;
+  const int s = R.corr[2 * j], d = R.corr[2 * j + 1];
+  const float4 a = R.spts[R.srank[s]], b = R.dpts[R.drank[d]];
+  int lo = 0, hi = R.m;  // first clique entry >= j
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (R.clique[mid] < j) lo = mid + 1;
+    else hi = mid;
+  }
+  const long long o = R.off + j;
+  out.corr[2 * o] = s;
+  out.corr[2 * o + 1] = d;
+  out.inlier[o] = lo < R.m && R.clique[lo] == j;
+  out.sxyz[3 * o] = a.x; out.sxyz[3 * o + 1] = a.y; out.sxyz[3 * o + 2] = a.z;
+  out.dxyz[3 * o] = b.x; out.dxyz[3 * o + 1] = b.y; out.dxyz[3 * o + 2] = b.z;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1833,6 +1860,10 @@ int launch_big_graph_solve(const MatchDev* d_pairs, int count, const QuatroParam
 
 void launch_transform_raw(const CloudDev* d_clouds, const double* d_T16s, int count, int max_n, float4* const* d_outs, cudaStream_t s) {
   k_transform_raw<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_clouds, d_T16s, d_outs);
+}
+
+void launch_match_capture(const MatchCaptureRow* d_rows, int count, int max_n, MatchCaptureOut out, cudaStream_t s) {
+  k_match_capture<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_rows, out);
 }
 
 }  // namespace b200

@@ -319,6 +319,34 @@ int b200reg_loop_closure(b200reg_ctx* ctx, int count, const float* const* src_xy
                          const b200reg_quatro_params* qparams, const b200reg_gicp_params* gparams,
                          b200reg_result* out, b200reg_quatro_info* quatro_out);
 
+/* Quatro matches: the correspondences the coarse stage solved (Matcher::calculateCorrespondences, quatro_module.cc:60-61)
+ * and which of them are in the solve's max clique (RobustRegistrationSolver::getInlierMaxClique, :69-76), per pair.
+ *   Which calls record.  Recording is off by default.  While it is on, every call that reaches the Quatro stage records:
+ *     b200reg_quatro_align, b200reg_quatro_align_ex, b200reg_loop_closure, b200reg_perform_loop_closure, and the batch
+ *     jobs of b200reg_batch_submit_loop_closure and b200reg_batch_submit_perform_loop_closure (b200reg_batch_set_quatro_matches).
+ *     Each such call replaces the stored matches.  Such a call with recording off discards them.  b200reg_quatro_solve_tap
+ *     and the calls without a Quatro stage leave them untouched.
+ *   Rows.  Rows follow the caller's pair or query order.  Pair i's matches are the solver's input set, in the order
+ *     b200reg_quatro_align_ex returns it.  A query with no candidate, b200reg_perform_loop_closure with enable_quatro = 0,
+ *     and a pair whose matcher kept nothing have empty rows.
+ *   Inliers.  inlier_out is 1 for the members of the pair's max clique and 0 otherwise.  The number of 1s of a pair equals
+ *     its b200reg_quatro_info::clique_size, also for an invalid solve with a clique of 0 or 1.
+ *   Indices and points.  The indices are rows of the clouds Quatro matched, in their original order.  For the raw-buffer
+ *     calls those are the caller's buffers.  For b200reg_perform_loop_closure they are the assembled, voxelised clouds, whose
+ *     rows are the rows of its SOURCE and TARGET loop clouds.  The xyz values are those rows' floats, bit for bit.
+ *   Cost.  With recording off nothing is allocated or launched.  With it on, a call allocates 36 bytes per match and one
+ *     clique row per pair for its own duration, and adds one kernel launch.  Results, Quatro records, LM traces and loop
+ *     clouds stay byte-identical.  If the slab cannot be allocated the call returns B200REG_ECUDA with the bytes needed.  */
+int b200reg_ctx_set_quatro_matches(b200reg_ctx* ctx, int enable);
+/* The matches of the context's most recent recording call, as CSR over that call's pairs: pair i's matches are rows
+ * offsets_out[i] .. offsets_out[i + 1]), offsets_out has count + 1 entries.  Row r is corr_out[2r] (src) and
+ * corr_out[2r + 1] (dst), inlier_out[r], src_xyz_out[3r .. 3r + 3) and dst_xyz_out[3r .. 3r + 3).  Any of the four output
+ * pointers may be NULL.  If the matches exceed `capacity` (in rows) the call fills offsets_out, writes nothing else and
+ * returns B200REG_ESTATE.  offsets_out == NULL: returns that call's pair count (>= 0) and writes nothing.  Before any
+ * recording call, after a call that did not record, and after a call that failed: B200REG_ESTATE.                      */
+int b200reg_quatro_matches(b200reg_ctx* ctx, int64_t* offsets_out, size_t capacity, int32_t* corr_out, int32_t* inlier_out,
+                           float* src_xyz_out, float* dst_xyz_out);
+
 /* ---- "next" rows (SURVEY.md §8f): device-resident keyframes, candidate search, cloud assembly ---------- */
 typedef struct b200reg_keyframes b200reg_keyframes;
 
@@ -482,6 +510,16 @@ int b200reg_batch_loop_clouds(b200reg_batch* b, int64_t ticket, int kind, int64_
                               float* xyzi_out);
 int b200reg_batch_lm_trace(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity,
                            b200reg_lm_trial* trials_out);
+/* Quatro matches of driver jobs (b200reg_ctx_set_quatro_matches / b200reg_quatro_matches per job).  The setting is off by
+ * default and is copied at submit like the two above.  A job of b200reg_batch_submit_loop_closure or
+ * _submit_perform_loop_closure that ran with it on returns, byte for byte, what b200reg_quatro_matches returns on a context
+ * after the synchronous call with the same inputs.  The record moves into the job's outputs without a copy and stays
+ * readable from b200reg_batch_wait until b200reg_batch_release or b200reg_batch_destroy.  The getter follows the rules of
+ * b200reg_quatro_matches and the ticket rules above; an icpAlignment job, or one submitted with recording off, holds no
+ * matches (B200REG_ESTATE).                                                                                            */
+int b200reg_batch_set_quatro_matches(b200reg_batch* b, int enable);
+int b200reg_batch_quatro_matches(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity, int32_t* corr_out,
+                                 int32_t* inlier_out, float* src_xyz_out, float* dst_xyz_out);
 int b200reg_batch_release(b200reg_batch* b, int64_t ticket);
 int64_t b200reg_batch_launch_count(const b200reg_batch* b);
 int b200reg_batch_depth(const b200reg_batch* b);
