@@ -10,11 +10,13 @@
 //   k_morton_ghist    partials -> bbox -> 30-bit Morton keys + the digit histograms of ALL sort passes
 //   k_sort_pass x3    stable LSD radix sort, 10 bits per pass, ONE kernel per pass: tile-local ranks, decoupled
 //                     look-back across the tiles of a cloud for the global offsets (no separate histogram / scan
-//                     kernels), scatter; the last pass writes the sorted float4 points and the rank array directly
+//                     kernels), the tile staged in shared memory in (digit, rank) order and written out in runs; the
+//                     last pass writes the sorted float4 points and the rank array directly
 //   k_lbvh_topology   Karras radix tree, one thread per node
-//   k_lbvh_aabb       bottom-up boxes: the work items (collapsed-leaf roots and lone points, ~1 in 6 candidates) are
-//                     compacted inside each block so that climbing warps are fully populated; a child writes its box
-//                     and its reference straight into its half of the parent's traversal record
+//   k_lbvh_aabb       bottom-up boxes: the work items (collapsed-leaf roots and lone points, ~1 in 6 candidates) of
+//                     four chunks of candidates are compacted inside each block so that climbing warps are fully
+//                     populated; a child writes its box and its reference straight into its half of the parent's
+//                     traversal record
 // The sort is stable, so the layout -- and with it every later reduction order -- is deterministic.
 // A mid-count split over the same Morton order was measured first and discarded: ranges that
 // straddle octant boundaries give huge overlapping boxes (195 node + 71 leaf visits per 15-NN
@@ -178,8 +180,12 @@ __global__ void __launch_bounds__(SORT_THREADS) k_sort_pass(const D* descs, int 
   const SortDev& c = sort_of(d);
   const int ntiles = sort_tiles(c.n);
   if ((int)blockIdx.x >= ntiles) return;
-  __shared__ unsigned short cnt[NW][R];  // per-warp digit counts, then exclusive offsets inside the tile (<= SORT_TILE)
-  __shared__ uint32_t gbase[R];          // first output slot of (digit, this tile)
+  // per-warp digit counts, then exclusive offsets inside the tile (<= SORT_TILE); last, the tile's keys and values staged
+  // in (digit, rank) order
+  __shared__ __align__(16) unsigned short cnt[NW][R];
+  static_assert(sizeof(cnt) >= 2 * SORT_TILE * sizeof(uint32_t), "the staged tile lives in cnt");
+  __shared__ uint32_t gbase[R];          // first output slot of (digit, this tile), then minus the digit's first tile slot
+  __shared__ unsigned short tstart[R];   // the tile's count of each digit, then its first slot inside the tile
   __shared__ uint32_t wtot[NW];
   __shared__ int s_tile;
   uint32_t* ws = c.hist;
@@ -254,6 +260,7 @@ __global__ void __launch_bounds__(SORT_THREADS) k_sort_pass(const D* descs, int 
         r += t;
       }
       run[k] = r;
+      tstart[d] = (unsigned short)r;
       excl[k] = 0;
       open_[k] = tile > 0;
       *(volatile uint32_t*)(look + (size_t)tile * R + d) = (tile == 0 ? LB_INC : LB_AGG) | r;
@@ -284,19 +291,69 @@ __global__ void __launch_bounds__(SORT_THREADS) k_sort_pass(const D* descs, int 
     }
   }
   __syncthreads();
+  // exclusive scan of the tile's digit counts: where each digit's run starts in the tile's sorted order
+  {
+    uint32_t hv[DPT], run = 0;
+#pragma unroll
+    for (int k = 0; k < DPT; k++) {
+      hv[k] = run;
+      run += tstart[threadIdx.x * DPT + k];
+    }
+    uint32_t incl = run;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += t;
+    }
+    if (lane == 31) wtot[w] = incl;
+    __syncthreads();
+    uint32_t woff = 0;
+    for (int ww = 0; ww < w; ww++) woff += wtot[ww];
+    const uint32_t excl = woff + incl - run;
+#pragma unroll
+    for (int k = 0; k < DPT; k++) {
+      const int dd = threadIdx.x * DPT + k;
+      tstart[dd] = (unsigned short)(excl + hv[k]);
+      gbase[dd] -= excl + hv[k];
+    }
+  }
+  __syncthreads();
+  // stage the tile in (digit, rank) order, then write it out in that order: consecutive threads store consecutive slots of
+  // a digit's run instead of one scattered word each.  Slot j of the staged tile goes to gbase[digit] + j.
 #pragma unroll
   for (int r = 0; r < SORT_ITEMS; r++) {
     const int i = base + (w * SORT_ITEMS + r) * 32 + lane;
     if (i < c.n) {
       const uint32_t dig = (key[r] >> shift) & (R - 1);
-      const uint32_t dst = gbase[dig] + cnt[w][dig] + rk[r];
-      okeys[dst] = key[r];
+      rk[r] += tstart[dig] + cnt[w][dig];
+    }
+  }
+  __syncthreads();
+  uint32_t* skey = reinterpret_cast<uint32_t*>(&cnt[0][0]);
+  uint32_t* sval = skey + SORT_TILE;
+#pragma unroll
+  for (int r = 0; r < SORT_ITEMS; r++) {
+    const int i = base + (w * SORT_ITEMS + r) * 32 + lane;
+    if (i < c.n) {
+      skey[rk[r]] = key[r];
+      sval[rk[r]] = val[r];
+    }
+  }
+  __syncthreads();
+  const int tile_n = min(SORT_TILE, c.n - base);
+#pragma unroll
+  for (int r = 0; r < SORT_ITEMS; r++) {
+    const int j = r * SORT_THREADS + threadIdx.x;
+    if (j < tile_n) {
+      const uint32_t k = skey[j], v = sval[j];
+      const uint32_t dst = gbase[(k >> shift) & (R - 1)] + j;
+      okeys[dst] = k;
       if constexpr (GATHER) {
-        const float* p = d.raw + (size_t)val[r] * d.raw_stride;
-        d.pts[dst] = make_float4(p[0], p[1], p[2], __int_as_float((int)val[r]));
-        d.rank[val[r]] = (int)dst;
+        const float* p = d.raw + (size_t)v * d.raw_stride;
+        d.pts[dst] = make_float4(p[0], p[1], p[2], __int_as_float((int)v));
+        d.rank[v] = (int)dst;
       } else {
-        ovals[dst] = val[r];
+        ovals[dst] = v;
       }
     }
   }
@@ -355,42 +412,17 @@ __global__ void __launch_bounds__(256) k_lbvh_topology(const BuildDev* builds) {
 // Bottom-up AABBs.  Work items: every point whose parent spans > LEAF points (a 1-point leaf) and every internal
 // node that is the root of a collapsed leaf (<= LEAF points, parent > LEAF): it reduces its <= 8 points directly.
 // Only about one candidate in six is a work item, and a climb is a chain of dependent atomics: the items of a block are
-// therefore compacted first (ballot + prefix), so the warps that stay resident for the climb are fully populated.
+// therefore compacted first (ballot + prefix), so the warps that stay resident for the climb are fully populated, and
+// the climbing threads are what fills the SM while the climbs wait on L2.
 // An item writes its box and its own reference into ITS half of the parent's traversal record and arrives at the
 // parent's flag; the second arrival owns the parent, reads the finished 64-byte record back, merges the two boxes and
 // carries on upwards.  (nbox, the separate per-node box array of round 1, is gone.)
-__global__ void __launch_bounds__(256) k_lbvh_aabb(const BuildDev* builds) {
-  const BuildDev& c = builds[blockIdx.y];
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n = c.sort.n;
-  if (n <= LEAF || (int)(blockIdx.x * blockDim.x) >= 2 * n - 1) return;
-  __shared__ int s_items[256];
-  __shared__ int s_wcnt[8];
-  bool is_item = false;
-  if (t < n) {  // point t
-    const int4 pi = c.info[c.parent_leaf[t]];
-    is_item = pi.y - pi.x + 1 > LEAF;  // otherwise it lives inside a collapsed leaf
-  } else if (t < 2 * n - 1) {  // internal node t - n
-    const int i = t - n;
-    const int4 inf = c.info[i];
-    if (i != 0 && inf.y - inf.x + 1 <= LEAF) {
-      const int4 pi = c.info[c.parent_node[i]];
-      is_item = pi.y - pi.x + 1 > LEAF;  // otherwise an ancestor is the collapsed-leaf root
-    }
-  }
-  const unsigned bal = __ballot_sync(0xffffffffu, is_item);
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) s_wcnt[w] = __popc(bal);
-  __syncthreads();
-  int off = 0, total = 0;
-  for (int k = 0; k < 8; k++) {
-    if (k < w) off += s_wcnt[k];
-    total += s_wcnt[k];
-  }
-  if (is_item) s_items[off + __popc(bal & ((1u << lane) - 1u))] = t;
-  __syncthreads();
-  if ((int)threadIdx.x >= total) return;
-  const int item = s_items[threadIdx.x];
+// Message passing between the two children of a node needs acquire / release ordering at device scope, not the sequential
+// consistency of __threadfence() (fence.sc), which costs more on every level of every climb.
+__device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
+
+// One work item's box and its climb towards the root.
+__device__ __forceinline__ void aabb_climb(const BuildDev& c, int n, int item) {
   // the item's own box, reference and parent
   float4 lo, hi;
   int ref, node, first;
@@ -417,25 +449,87 @@ __global__ void __launch_bounds__(256) k_lbvh_aabb(const BuildDev* builds) {
     node = c.parent_node[i];
     first = inf.x;
   }
+  // The climb is a chain of dependent L2 round trips, so it keeps everything it can off that chain: the descriptor's
+  // pointers live in registers (the fences below would otherwise force them to be re-read at every level), and the split
+  // and parent of the NEXT node are fetched before this level's store / fence / atomic, which they do not depend on.
+  const int4* __restrict__ info = c.info;
+  const int* __restrict__ parent_node = c.parent_node;
+  float4* tnodes = c.tnodes;
+  uint32_t* flags = c.flags;
+  int4 pinf = info[node];
+  int up = node != 0 ? parent_node[node] : 0;
   for (;;) {
     // which child of `node` am I?  child 0 covers [info.x, split], child 1 (split, info.y]: compare first points
-    const int4 pinf = c.info[node];
     const int k = first > pinf.w ? 1 : 0;
-    float4* rec = c.tnodes + 4 * (size_t)node + 2 * k;
+    const int4 uinf = info[up];  // next level's record (harmless re-read of the root at the top)
+    const int uup = up != 0 ? parent_node[up] : 0;
+    float4* rec = tnodes + 4 * (size_t)node + 2 * k;
     __stcg(&rec[0], make_float4(lo.x, lo.y, lo.z, __int_as_float(ref)));
     __stcg(&rec[1], make_float4(hi.x, hi.y, hi.z, 0.f));
-    __threadfence();
-    if (atomicAdd(&c.flags[node], 1u) == 0u) return;  // the sibling is still on its way: it will take the parent
-    __threadfence();
-    const float4 olo = __ldcg(&c.tnodes[4 * (size_t)node + 2 * (1 - k)]);
-    const float4 ohi = __ldcg(&c.tnodes[4 * (size_t)node + 2 * (1 - k) + 1]);
+    fence_acq_rel_gpu();  // release: this record half before the arrival
+    if (atomicAdd(&flags[node], 1u) == 0u) return;  // the sibling is still on its way: it will take the parent
+    fence_acq_rel_gpu();  // acquire: the sibling's half after its arrival
+    const float4 olo = __ldcg(&tnodes[4 * (size_t)node + 2 * (1 - k)]);
+    const float4 ohi = __ldcg(&tnodes[4 * (size_t)node + 2 * (1 - k) + 1]);
     if (node == 0) return;
     lo = make_float4(fminf(lo.x, olo.x), fminf(lo.y, olo.y), fminf(lo.z, olo.z), 0.f);
     hi = make_float4(fmaxf(hi.x, ohi.x), fmaxf(hi.y, ohi.y), fmaxf(hi.z, ohi.z), 0.f);
     ref = node;
     first = pinf.x;
-    node = c.parent_node[node];
+    node = up;
+    pinf = uinf;
+    up = uup;
   }
+}
+
+// AABB_CHUNKS chunks of 256 candidates per block: their work items, about one in six, are compacted together so that a
+// block keeps ~4x as many climbs in flight as with one chunk; a thread takes more than one item only when the chunks hold
+// more than 256.
+constexpr int AABB_CHUNKS = 4;
+__global__ void __launch_bounds__(256) k_lbvh_aabb(const BuildDev* builds) {
+  const BuildDev& c = builds[blockIdx.y];
+  const int n = c.sort.n;
+  const int t0 = blockIdx.x * AABB_CHUNKS * 256;
+  if (n <= LEAF || t0 >= 2 * n - 1) return;
+  __shared__ int s_items[AABB_CHUNKS * 256];
+  __shared__ int s_wcnt[AABB_CHUNKS][8];
+  bool is_item[AABB_CHUNKS];
+#pragma unroll
+  for (int ch = 0; ch < AABB_CHUNKS; ch++) {  // the chunks' loads are independent: all in flight together
+    const int t = t0 + ch * 256 + threadIdx.x;
+    is_item[ch] = false;
+    if (t < n) {  // point t
+      const int4 pi = c.info[c.parent_leaf[t]];
+      is_item[ch] = pi.y - pi.x + 1 > LEAF;  // otherwise it lives inside a collapsed leaf
+    } else if (t < 2 * n - 1) {  // internal node t - n
+      const int i = t - n;
+      const int4 inf = c.info[i];
+      if (i != 0 && inf.y - inf.x + 1 <= LEAF) {
+        const int4 pi = c.info[c.parent_node[i]];
+        is_item[ch] = pi.y - pi.x + 1 > LEAF;  // otherwise an ancestor is the collapsed-leaf root
+      }
+    }
+  }
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  unsigned bal[AABB_CHUNKS];
+#pragma unroll
+  for (int ch = 0; ch < AABB_CHUNKS; ch++) {
+    bal[ch] = __ballot_sync(0xffffffffu, is_item[ch]);
+    if (lane == 0) s_wcnt[ch][w] = __popc(bal[ch]);
+  }
+  __syncthreads();
+  int total = 0;
+#pragma unroll
+  for (int ch = 0; ch < AABB_CHUNKS; ch++) {
+    int off = total;
+    for (int k = 0; k < 8; k++) {
+      if (k < w) off += s_wcnt[ch][k];
+      total += s_wcnt[ch][k];
+    }
+    if (is_item[ch]) s_items[off + __popc(bal[ch] & ((1u << lane) - 1u))] = t0 + ch * 256 + threadIdx.x;
+  }
+  __syncthreads();
+  for (int it = threadIdx.x; it < total; it += 256) aabb_climb(c, n, s_items[it]);
 }
 
 // ------------------------------------------------------------------------------------
@@ -452,7 +546,7 @@ int launch_index_build(const BuildDev* d_builds, int count, int max_n, cudaStrea
   k_sort_pass<10, true><<<tiles, SORT_THREADS, 0, s>>>(d_builds, 2); launches++;
   if (max_n > 1) {
     k_lbvh_topology<<<dim3((max_n + 254) / 256, count), 256, 0, s>>>(d_builds); launches++;
-    k_lbvh_aabb<<<dim3((2 * max_n + 254) / 256, count), 256, 0, s>>>(d_builds); launches++;
+    k_lbvh_aabb<<<dim3((2 * max_n - 1 + AABB_CHUNKS * 256 - 1) / (AABB_CHUNKS * 256), count), 256, 0, s>>>(d_builds); launches++;
   }
   return launches;
 }
