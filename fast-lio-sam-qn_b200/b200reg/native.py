@@ -5,6 +5,7 @@ fallback; if the library or a GPU is missing these functions raise.
 """
 import ctypes as C
 import os
+import sys
 
 import numpy as np
 
@@ -119,6 +120,7 @@ EXPORTS = [
     "b200reg_batch_submit_perform_loop_closure", "b200reg_batch_set_loop_clouds", "b200reg_batch_set_lm_trace",
     "b200reg_batch_loop_clouds", "b200reg_batch_lm_trace", "b200reg_batch_release",
     "b200reg_ctx_set_quatro_matches", "b200reg_quatro_matches", "b200reg_batch_set_quatro_matches", "b200reg_batch_quatro_matches",
+    "b200reg_ctx_set_residuals", "b200reg_residuals", "b200reg_batch_set_residuals", "b200reg_batch_residuals",
 ]
 ESTATE = -4  # B200REG_ESTATE
 # B200REG_CLOUD_*: the loop clouds (Context.set_loop_clouds / Context.loop_clouds)
@@ -217,6 +219,33 @@ def _quatro_matches(get):
     sx, dx = np.empty((m, 3), np.float32), np.empty((m, 3), np.float32)
     _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(m), *(a.ctypes.data_as(C.c_void_p) for a in (corr, inlier, sx, dx))))
     return [dict(corr=corr[a:b], inlier=inlier[a:b], src_xyz=sx[a:b], dst_xyz=dx[a:b]) for a, b in zip(offsets[:-1], offsets[1:])]
+
+
+def _residuals(get):
+    """The CSR rows behind get(offsets, capacity, nn, d2) (b200reg_residuals' rules) -> one (nn int32[n], d2 float32[n])
+    pair per pair."""
+    n = get(None, C.c_size_t(0), None, None)
+    _check(min(n, 0))
+    offsets = np.empty(n + 1, np.int64)
+    rc = get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None, None)  # offsets only
+    if rc != ESTATE:
+        _check(rc)
+    m = int(offsets[-1])
+    nn, d2 = np.empty(m, np.int32), np.empty(m, np.float32)
+    _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(m), nn.ctypes.data_as(C.c_void_p), d2.ctypes.data_as(C.c_void_p)))
+    return [(nn[a:b], d2[a:b]) for a, b in zip(offsets[:-1], offsets[1:])]
+
+
+def fitness_score(d2, max_range=float("inf")):
+    """pcl::Registration::getFitnessScore(max_range) over one pair's residual rows: the mean of the squared distances d2
+    with d2 <= max_range (PCL compares the SQUARED distance with max_range), summed in point order in float64;
+    sys.float_info.max (DBL_MAX) when no point is kept, as for a NaN max_range."""
+    total, nr = 0.0, 0
+    for v in np.asarray(d2, np.float32).tolist():
+        if v <= max_range:
+            total += v
+            nr += 1
+    return total / nr if nr > 0 else sys.float_info.max
 
 
 def loop_factor_from_poses(T_between, pose_latest, pose_closest, score, valid=True, from_idx=0, to_idx=0):
@@ -328,6 +357,16 @@ class Context:
         """The matches of the last recording call: per pair of that call (its pair or query order) a dict of corr (m, 2),
         inlier (m,), src_xyz (m, 3) and dst_xyz (m, 3); empty where no Quatro stage ran (include/b200reg.h)."""
         return _quatro_matches(lambda *a: lib().b200reg_quatro_matches(self.h, *a))
+
+    def set_residuals(self, enable):
+        """Record each source point's nearest target point and squared distance from the fitness pass of the following
+        gicp_align / icp_alignment / loop_closure / perform_loop_closure calls; results do not change."""
+        _check(lib().b200reg_ctx_set_residuals(self.h, int(bool(enable))))
+
+    def residuals(self):
+        """The rows of the last recording call: per pair of that call (its pair or query order) (nn int32[n], d2 float32[n])
+        in the source cloud's original point order; empty where no fine stage ran (include/b200reg.h)."""
+        return _residuals(lambda *a: lib().b200reg_residuals(self.h, *a))
 
     # -- the path's one collective: all-gather of the result records over NCCL (SURVEY §8e) --------
     def comm_init(self, unique_id, rank, world):
@@ -783,6 +822,15 @@ class Batch:
         """The Quatro matches of a waited-for job that recorded them, as Context.quatro_matches returns them after the
         synchronous call."""
         return _quatro_matches(lambda *a: lib().b200reg_batch_quatro_matches(self.h, C.c_int64(ticket), *a))
+
+    def set_residuals(self, enable):
+        """Record the residuals of the jobs submitted from now on (copied at submit)."""
+        _check(lib().b200reg_batch_set_residuals(self.h, int(bool(enable))))
+
+    def residuals(self, ticket):
+        """The residuals of a waited-for job that recorded them, as Context.residuals returns them after the synchronous
+        call."""
+        return _residuals(lambda *a: lib().b200reg_batch_residuals(self.h, C.c_int64(ticket), *a))
 
     def release(self, ticket):
         """Frees the loop clouds and LM trace a waited-for job holds (nothing to free is no error)."""

@@ -79,6 +79,18 @@ struct b200reg_ctx {
     std::vector<int64_t> offsets;  // pairs + 1
     std::vector<int32_t> words;    // 9 per match
   } quatro_matches;
+  // residuals (b200reg_ctx_set_residuals / b200reg_residuals) of the most recent call that ran the fine stage with recording
+  // on, CSR over its pairs, on the host: per source point in original order, the fitness pass's nearest target point
+  // (original index) and fp32 squared distance
+  struct Residuals {
+    bool enabled = false;
+    bool valid = false;  // false before a recording call, after one that did not record and after one that failed
+    std::vector<int64_t> offsets;  // pairs + 1
+    std::vector<int32_t> nn;
+    std::vector<float> d2;
+    int32_t* slab = nullptr;  // device rows reserved by the call in flight (ResidualSlab): nn block, then d2 block
+    size_t slab_points = 0;
+  } residuals;
   // the path's one collective (b200reg_comm_*): NCCL communicator of this rank
   ncclComm_t comm = nullptr;
   int rank = -1, world = 1;
@@ -250,6 +262,32 @@ void quatro_matches_remap(b200reg_ctx* c, int count, const std::vector<int>& whe
 // a null or invalid record is B200REG_ESTATE with the message `none`; then the CSR offsets and the capacity rule.
 int quatro_matches_copy(const b200reg_ctx::QuatroMatches* qm, int64_t* offsets_out, size_t capacity, int32_t* corr_out,
                         int32_t* inlier_out, float* src_xyz_out, float* dst_xyz_out, const std::string& none);
+
+// The stored residuals belong to the pairs of the last b200reg_gicp_align.  A caller that ran that solve on a subset of its
+// `count` pairs (solve pair k = its pair where[k]) renumbers them to its own pairs; the others get empty rows.  Does
+// nothing but keep them invalid when recording is off.  (api_gicp.cu)
+void residuals_remap(b200reg_ctx* c, int count, const std::vector<int>& where);
+// The copy-out rules of b200reg_residuals over a context's or a batch-driver job's record (b200reg_batch_residuals): a null
+// or invalid record is B200REG_ESTATE with the message `none`; then the CSR offsets and the capacity rule.
+int residuals_copy(const b200reg_ctx::Residuals* r, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out,
+                   const std::string& none);
+// The device rows of the residual capture of one b200reg_icp_alignment, b200reg_loop_closure or
+// b200reg_perform_loop_closure call, reserved as soon as its source clouds exist, so that a failed allocation costs no
+// registration: one row per source point of every pair that can run the fine stage.  The call's b200reg_gicp_align writes
+// into them instead of allocating its own.  Returned at the end of the scope; with recording off nothing is allocated.
+class ResidualSlab {
+ public:
+  explicit ResidualSlab(b200reg_ctx* c) : c_(c), scratch_(c) {}
+  int reserve(int count, const size_t* src_n);
+  ~ResidualSlab() {
+    c_->residuals.slab = nullptr;
+    c_->residuals.slab_points = 0;
+  }
+
+ private:
+  b200reg_ctx* c_;
+  Scratch scratch_;
+};
 
 // LoopClosure::coarseToFineAlignment on cloud handles (api_quatro.cu).  fine_tf16 (optional, count x 16): the fine stage's
 // own fp32 final transformation of each pair whose coarse stage is valid (the transform of align()'s output cloud)

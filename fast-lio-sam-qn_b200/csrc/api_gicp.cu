@@ -1,5 +1,5 @@
-// api_gicp.cu -- the C ABI of the Nano-GICP path: the context's LM arena, b200reg_gicp_align, b200reg_icp_alignment and the
-// linearize / compute_error / LM controller taps.
+// api_gicp.cu -- the C ABI of the Nano-GICP path: the context's LM arena, b200reg_gicp_align, b200reg_icp_alignment, the
+// residual capture and the linearize / compute_error / LM controller taps.
 #include <algorithm>
 #include <cstddef>
 #include <cstdlib>
@@ -106,6 +106,60 @@ int lm_trace_copy(const b200reg_ctx::LmTrace* tr, int64_t* offsets_out, size_t c
   if (trials_out && !tr->trials.empty()) memcpy(trials_out, tr->trials.data(), sizeof(b200reg_lm_trial) * tr->trials.size());
   return B200REG_OK;
 }
+
+void residuals_remap(b200reg_ctx* c, int count, const std::vector<int>& where) {
+  auto& r = c->residuals;
+  if (!r.enabled) {
+    r.valid = false;
+    return;
+  }
+  std::vector<int> solved(count, -1);  // caller pair -> solve pair
+  for (size_t k = 0; k < where.size(); k++) solved[where[k]] = (int)k;
+  std::vector<int64_t> offsets(count + 1, 0);
+  std::vector<int32_t> nn;
+  std::vector<float> d2;
+  for (int i = 0; i < count; i++) {
+    const int k = solved[i];
+    if (k >= 0) {
+      nn.insert(nn.end(), r.nn.begin() + r.offsets[k], r.nn.begin() + r.offsets[k + 1]);
+      d2.insert(d2.end(), r.d2.begin() + r.offsets[k], r.d2.begin() + r.offsets[k + 1]);
+    }
+    offsets[i + 1] = (int64_t)nn.size();
+  }
+  r.offsets.swap(offsets);
+  r.nn.swap(nn);
+  r.d2.swap(d2);
+  r.valid = true;
+}
+
+int residuals_copy(const b200reg_ctx::Residuals* r, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out,
+                   const std::string& none) {
+  if (!r || !r->valid) return fail(B200REG_ESTATE, none);
+  const int pairs = (int)r->offsets.size() - 1;
+  if (!offsets_out) return pairs;
+  memcpy(offsets_out, r->offsets.data(), sizeof(int64_t) * r->offsets.size());
+  if (r->nn.size() > capacity)
+    return fail(B200REG_ESTATE, "residuals hold " + std::to_string(r->nn.size()) + " rows, capacity " + std::to_string(capacity));
+  if (nn_out && !r->nn.empty()) memcpy(nn_out, r->nn.data(), sizeof(int32_t) * r->nn.size());
+  if (d2_out && !r->d2.empty()) memcpy(d2_out, r->d2.data(), sizeof(float) * r->d2.size());
+  return B200REG_OK;
+}
+
+int ResidualSlab::reserve(int count, const size_t* src_n) {
+  auto& r = c_->residuals;
+  r.slab = nullptr;
+  r.slab_points = 0;
+  if (!r.enabled) return B200REG_OK;
+  size_t points = 0;
+  for (int i = 0; i < count; i++) points += src_n[i];
+  void* p = nullptr;
+  const cudaError_t e = scratch_.alloc(&p, 8 * points);
+  if (e != cudaSuccess)
+    return fail(B200REG_ECUDA, "residuals: cannot allocate " + std::to_string(8 * points) + " bytes: " + cudaGetErrorString(e));
+  r.slab = (int32_t*)p;
+  r.slab_points = points;
+  return B200REG_OK;
+}
 }  // namespace b200
 
 // make the arena hold `count` pairs and make sure its graph exists
@@ -199,8 +253,21 @@ int b200reg_lm_trace(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, b200
                        "no LM trace: the context's last LM solve was not traced (b200reg_ctx_set_lm_trace)");
 }
 
+int b200reg_ctx_set_residuals(b200reg_ctx* c, int enable) {
+  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
+  c->residuals.enabled = enable != 0;
+  return B200REG_OK;
+}
+
+int b200reg_residuals(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out) {
+  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
+  return residuals_copy(&c->residuals, offsets_out, capacity, nn_out, d2_out,
+                        "no residuals: the context's last registration did not record them, or failed (b200reg_ctx_set_residuals)");
+}
+
 int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* tgt,
                        const double* guess16, const b200reg_gicp_params* params, b200reg_result* out) {
+  if (c) c->residuals.valid = false;  // only a call that records and succeeds holds residuals
   if (!c || count <= 0 || !src || !tgt || !params || !out) return fail(B200REG_EINVAL, "bad argument");
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
@@ -221,6 +288,23 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
     if (!need.empty() &&
         (rc = b200reg_clouds_covariances_ex(c, (int)need.size(), need.data(), params->k_correspondences, params->regularization)))
       return rc;
+  }
+  // residual rows: those the enclosing call reserved (ResidualSlab), else this call's own, before the solve
+  auto& rs = c->residuals;
+  std::vector<int64_t> res_offsets;
+  ResidualOut res_out{nullptr, nullptr};
+  if (rs.enabled) {
+    res_offsets.assign(count + 1, 0);
+    for (int i = 0; i < count; i++) res_offsets[i + 1] = res_offsets[i] + src[i]->dev.n;
+    const size_t total = (size_t)res_offsets[count];
+    int32_t* slab = rs.slab;
+    if (!slab || rs.slab_points < total) {
+      const cudaError_t e = scratch.alloc((void**)&slab, 8 * total);
+      if (e != cudaSuccess)
+        return fail(B200REG_ECUDA, "residuals: cannot allocate " + std::to_string(8 * total) + " bytes: " + cudaGetErrorString(e));
+    }
+    res_out.nn = slab;
+    res_out.d2 = (float*)(slab + total);
   }
   const GicpParamsDev prm = to_dev(*params);
   std::vector<PairDev> pairs;
@@ -298,6 +382,34 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
       std::copy(rows.begin() + (size_t)i * widest, rows.begin() + (size_t)i * widest + states[i].n_err, tr.trials.begin() + tr.offsets[i]);
     tr.valid = true;
   }
+  if (rs.enabled) {  // the fitness pass's per-point values of every pair, in one launch and one copy per array
+    const size_t total = (size_t)res_offsets[count];
+    std::vector<ResidualRow> rows;
+    int max_n = 0;
+    for (int i = 0; i < count; i++) {
+      if (pairs[i].src.n == 0) continue;
+      rows.push_back(ResidualRow{pairs[i].src.pts, pairs[i].tgt.pts, pairs[i].corr, pairs[i].sqd, pairs[i].src.n, res_offsets[i]});
+      max_n = std::max(max_n, pairs[i].src.n);
+    }
+    rs.nn.resize(total);
+    rs.d2.resize(total);
+    if (!rows.empty()) {
+      ResidualRow* d_rows = nullptr;
+      CU(scratch.upload(&d_rows, rows.data(), sizeof(ResidualRow) * rows.size()));
+      {
+        ProfScope ps(c, CLS_MISC);
+        launch_residual_rows(d_rows, (int)rows.size(), max_n, res_out, s);
+        c->launches++;
+        c->prof_bytes[CLS_MISC] += 48.0 * total;  // 16 source + 8 corr / sqd + 16 target in, 8 out
+      }
+      CU(cudaGetLastError());
+      CU(cudaMemcpyAsync(rs.nn.data(), res_out.nn, total * 4, cudaMemcpyDeviceToHost, s));
+      CU(cudaMemcpyAsync(rs.d2.data(), res_out.d2, total * 4, cudaMemcpyDeviceToHost, s));
+      CU(cudaStreamSynchronize(s));
+    }
+    rs.offsets.swap(res_offsets);
+    rs.valid = true;
+  }
   for (int i = 0; i < count; i++) {
     const PairState& st = states[i];
     b200reg_result& r = out[i];
@@ -340,7 +452,9 @@ static int icp_solve(b200reg_ctx* c, LoopCapture& cap, int count, b200reg_cloud*
   if (rc || !cap.on()) return rc;
   std::vector<float> fine_tf(16 * (size_t)count);
   for (int i = 0; i < count; i++) memcpy(&fine_tf[16 * (size_t)i], out[i].Tf, sizeof(out[i].Tf));
-  return cap.finish(nullptr, fine_tf.data());
+  rc = cap.finish(nullptr, fine_tf.data());
+  if (rc) c->residuals.valid = false;
+  return rc;
 }
 
 // one chunk of pairs, raw records already on the device
@@ -358,6 +472,7 @@ static int icp_alignment_device(b200reg_ctx* c, LoopCapture& cap, int count, con
 int b200reg_icp_alignment(b200reg_ctx* c, int count, const float* const* src_xyz, const size_t* src_n,
                           const float* const* tgt_xyz, const size_t* tgt_n, size_t stride_bytes, int on_device,
                           const b200reg_gicp_params* params, b200reg_result* out) {
+  if (c) c->residuals.valid = false;  // its solve records them; a refused or failed call holds none
   if (!c || count <= 0 || !src_xyz || !src_n || !tgt_xyz || !tgt_n || !params || !out)
     return fail(B200REG_EINVAL, "bad argument");
   if (stride_bytes < 12 || stride_bytes % 4) return fail(B200REG_EINVAL, "stride_bytes must be a multiple of 4, >= 12");
@@ -365,6 +480,8 @@ int b200reg_icp_alignment(b200reg_ctx* c, int count, const float* const* src_xyz
     if (!src_xyz[i] || !tgt_xyz[i] || src_n[i] == 0 || tgt_n[i] == 0) return fail(B200REG_EINVAL, "empty cloud");
   CU(cudaSetDevice(c->device));
   LoopCapture cap(c, count);
+  ResidualSlab rslab(c);
+  if (const int rc = rslab.reserve(count, src_n)) return rc;
   if (on_device) return icp_alignment_device(c, cap, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, params, out);
   // Host buffers: all uploads are queued on the copy stream up front, chunk by chunk; the compute stream processes
   // chunk k as soon as its records have landed, so the PCIe time of chunk k+1 hides behind the kernels of chunk k.

@@ -476,7 +476,7 @@ extern "C" {
 
 int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
                                  const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out) {
-  if (c) c->quatro_matches.valid = false;  // a refused call holds no matches either
+  if (c) c->quatro_matches.valid = c->residuals.valid = false;  // a refused call holds no matches or residuals either
   if (!c || !kf || count <= 0 || !query_idx || !closest_idx || !cfg || !out) return fail(B200REG_EINVAL, "bad argument");
   return perform_loop_closure(c, kf->st, count, query_idx, closest_idx, cfg, out, quatro_out);
 }
@@ -488,6 +488,7 @@ static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, co
                                 const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out) {
   LoopCapture cap(c, count);
   c->quatro_matches.valid = false;  // its Quatro stage records them for its subset; renumbered below, dropped on failure
+  c->residuals.valid = false;       // and its fine stage the residuals
   std::vector<int32_t> qs, cs;
   std::vector<int> where;
   for (int i = 0; i < count; i++) {
@@ -502,8 +503,9 @@ static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, co
   if (qs.empty()) {
     lm_trace_remap(c, count, where);
     quatro_matches_remap(c, count, where);
+    residuals_remap(c, count, where);
     const int rc = cap.finish(nullptr, nullptr);
-    if (rc) c->quatro_matches.valid = false;
+    if (rc) c->quatro_matches.valid = c->residuals.valid = false;
     return rc;
   }
   const int m = (int)qs.size();
@@ -518,6 +520,12 @@ static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, co
   bag.cl = sc;
   bag.cl.insert(bag.cl.end(), dc.begin(), dc.end());
   if ((rc = cap.clouds(where, sc.data(), dc.data(), true, cfg->enable_quatro != 0))) return rc;
+  ResidualSlab rslab(c);
+  {
+    std::vector<size_t> sn(m);  // the fine stage's source clouds have the sizes of the assembled sources
+    for (int k = 0; k < m; k++) sn[k] = (size_t)sc[k]->dev.n;
+    if ((rc = rslab.reserve(m, sn.data()))) return rc;
+  }
   std::vector<b200reg_result> res(m);
   std::vector<b200reg_quatro_info> qi(m);
   std::vector<float> fine_tf(16 * (size_t)m);  // the fine stage's transform of align()'s output cloud
@@ -533,8 +541,9 @@ static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, co
   }
   if (!rc) lm_trace_remap(c, count, where);
   if (!rc) quatro_matches_remap(c, count, cfg->enable_quatro ? where : std::vector<int>());
+  if (!rc) residuals_remap(c, count, where);
   if (!rc) rc = cap.finish(cfg->enable_quatro ? qi.data() : nullptr, fine_tf.data());
-  if (rc) c->quatro_matches.valid = false;
+  if (rc) c->quatro_matches.valid = c->residuals.valid = false;
   return rc;
 }
 

@@ -89,6 +89,7 @@ int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* sr
     }
   }
   lm_trace_remap(c, count, vidx);
+  residuals_remap(c, count, vidx);
   return B200REG_OK;
 }
 
@@ -860,19 +861,23 @@ int b200reg_loop_closure(b200reg_ctx* c, int count, const float* const* src_xyz,
                          const size_t* tgt_n, size_t stride_bytes, int on_device, const b200reg_quatro_params* qp,
                          const b200reg_gicp_params* gp, b200reg_result* out, b200reg_quatro_info* quatro_out) {
   if (c) c->quatro_matches.valid = false;  // its Quatro stage records them, and a later failure drops them again
+  if (c) c->residuals.valid = false;       // so does its fine stage with the residuals
   if (!c || count <= 0 || !src_xyz || !src_n || !tgt_xyz || !tgt_n || !qp || !gp || !out) return fail(B200REG_EINVAL, "bad argument");
   CU(cudaSetDevice(c->device));
   LoopCapture cap(c, count);
+  ResidualSlab rslab(c);
+  int rc = rslab.reserve(count, src_n);  // the fine stage's source clouds have the sizes of the sources
+  if (rc) return rc;
   CloudBag bag(c);
   std::vector<b200reg_cloud*> sc(count), tc(count);
-  int rc = create_pair_clouds(c, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, on_device, cap.on(), bag, sc.data(), tc.data());
+  rc = create_pair_clouds(c, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, on_device, cap.on(), bag, sc.data(), tc.data());
   if (!rc) rc = cap.clouds({}, sc.data(), tc.data(), false, true);
   std::vector<b200reg_quatro_info> own(quatro_out ? 0 : count);  // the capture reads the coarse stage's infos
   b200reg_quatro_info* qi = quatro_out ? quatro_out : own.data();
   std::vector<float> fine_tf(cap.on() ? 16 * (size_t)count : 0);
   if (!rc) rc = coarse_to_fine_on_clouds(c, count, sc.data(), tc.data(), qp, gp, out, qi, cap.on() ? fine_tf.data() : nullptr);
   if (!rc) rc = cap.finish(qi, fine_tf.data());
-  if (rc) c->quatro_matches.valid = false;
+  if (rc) c->quatro_matches.valid = c->residuals.valid = false;
   return rc;
 }
 

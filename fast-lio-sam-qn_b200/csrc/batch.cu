@@ -2,9 +2,9 @@
 // own host thread with its own CUDA streams and memory pool, take alternate jobs.  While one context waits for a PCIe
 // upload or polls its LM loop, the kernels of the others keep the SMs busy -- the batch-level concurrency SURVEY.md §8(d)
 // names as the lever for the HBM fraction.  Host code only; everything it calls is the public C ABI, except the jobs over
-// the keyframe store, which go through the job interface of api_keyframes.cu (api.cuh), and the loop clouds, LM trace and
-// Quatro matches of a capturing job, which it moves out of the worker's context and reads with the context getters'
-// copy-out (api.cuh).
+// the keyframe store, which go through the job interface of api_keyframes.cu (api.cuh), and the loop clouds, LM trace,
+// Quatro matches and residuals of a capturing job, which it moves out of the worker's context and reads with the context
+// getters' copy-out (api.cuh).
 //
 // Reference context: the reference registers ONE pair per 2 Hz timer tick, serially, on one thread
 // (fast_lio_sam_qn/src/fast_lio_sam_qn.cpp:203-219, LoopClosure is not re-entrant, :81).
@@ -24,21 +24,23 @@
 
 namespace {
 
-// A job's loop clouds, LM trace and Quatro matches, moved out of its worker's context when the job ends: they outlive the
-// wait, until b200reg_batch_release or b200reg_batch_destroy
+// A job's loop clouds, LM trace, Quatro matches and residuals, moved out of its worker's context when the job ends: they
+// outlive the wait, until b200reg_batch_release or b200reg_batch_destroy
 struct Captured {
   b200reg_ctx::LoopClouds clouds;
   b200reg_ctx::LmTrace trace;
   b200reg_ctx::QuatroMatches matches;
+  b200reg_ctx::Residuals residuals;
 };
 
 struct Capture {  // the capture settings of a job
   int cloud_mask = 0;
   bool lm_trace = false;
   bool quatro_matches = false;
-  bool on() const { return cloud_mask || lm_trace || quatro_matches; }
+  bool residuals = false;
+  bool on() const { return cloud_mask || lm_trace || quatro_matches || residuals; }
   bool operator!=(const Capture& o) const {
-    return cloud_mask != o.cloud_mask || lm_trace != o.lm_trace || quatro_matches != o.quatro_matches;
+    return cloud_mask != o.cloud_mask || lm_trace != o.lm_trace || quatro_matches != o.quatro_matches || residuals != o.residuals;
   }
 };
 
@@ -54,8 +56,8 @@ struct Job {
   std::shared_ptr<KfJob> kfjob;  // kind 2: its arguments and the store's state at submit
   b200reg_result* out = nullptr;
   b200reg_quatro_info* qout = nullptr;
-  // the driver's capture settings at submit (b200reg_batch_set_loop_clouds / _set_lm_trace / _set_quatro_matches), and what
-  // the job captured
+  // the driver's capture settings at submit (b200reg_batch_set_loop_clouds / _set_lm_trace / _set_quatro_matches /
+  // _set_residuals), and what the job captured
   Capture capture;
   std::shared_ptr<Captured> captured;
   // completion
@@ -109,6 +111,7 @@ static void run_worker(b200reg_batch* b, Worker* w) {
       c->loop_clouds.mask = j->capture.cloud_mask;
       c->lm_trace.enabled = j->capture.lm_trace;
       c->quatro_matches.enabled = j->capture.quatro_matches;
+      c->residuals.enabled = j->capture.residuals;
     }
     int rc;
     if (j->kind == 0)
@@ -126,10 +129,12 @@ static void run_worker(b200reg_batch* b, Worker* w) {
         std::swap(j->captured->clouds, c->loop_clouds);
         std::swap(j->captured->trace, c->lm_trace);
         std::swap(j->captured->matches, c->quatro_matches);
+        std::swap(j->captured->residuals, c->residuals);
       }
       c->loop_clouds = b200reg_ctx::LoopClouds();
       c->lm_trace = b200reg_ctx::LmTrace();
       c->quatro_matches = b200reg_ctx::QuatroMatches();
+      c->residuals = b200reg_ctx::Residuals();
     }
     {
       std::lock_guard<std::mutex> lk(b->mu);
@@ -304,19 +309,26 @@ int b200reg_batch_set_quatro_matches(b200reg_batch* b, int enable) {
   return B200REG_OK;
 }
 
+int b200reg_batch_set_residuals(b200reg_batch* b, int enable) {
+  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
+  b->capture.residuals = enable != 0;
+  return B200REG_OK;
+}
+
 }  // extern "C"
 
 // The outputs the getters read for `ticket` (the pointer keeps them alive while they are copied out, outside the lock), or
 // null; `none` is the getters' message when the output is missing, saying why.  kind: a B200REG_CLOUD_* bit, 0 for the LM
-// trace, MATCHES for the Quatro matches.  B200REG_EINVAL for a ticket never handed out.
-constexpr int MATCHES = -1;
+// trace, MATCHES for the Quatro matches, RESIDUALS for the residuals.  B200REG_EINVAL for a ticket never handed out.
+constexpr int MATCHES = -1, RESIDUALS = -2;
 static int find_captured(b200reg_batch* b, int64_t ticket, int kind, std::shared_ptr<Captured>* out, std::string* none) {
-  const std::string missing = std::string(kind > 0 ? "no such loop clouds: " : kind == 0 ? "no LM trace: " : "no Quatro matches: ") +
-                              "batch job " + std::to_string(ticket);
-  const std::string off = kind > 0   ? " did not capture this kind (b200reg_batch_set_loop_clouds at its submit)"
-                          : kind == 0 ? " was not traced (b200reg_batch_set_lm_trace at its submit)"
-                                      : " did not record them (b200reg_batch_set_quatro_matches at its submit, or a job without a "
-                                        "Quatro stage)";
+  const char* what = kind > 0 ? "no such loop clouds: " : kind == 0 ? "no LM trace: " : kind == MATCHES ? "no Quatro matches: " : "no residuals: ";
+  const std::string missing = what + std::string("batch job ") + std::to_string(ticket);
+  const std::string off = kind > 0         ? " did not capture this kind (b200reg_batch_set_loop_clouds at its submit)"
+                          : kind == 0       ? " was not traced (b200reg_batch_set_lm_trace at its submit)"
+                          : kind == MATCHES ? " did not record them (b200reg_batch_set_quatro_matches at its submit, or a job "
+                                              "without a Quatro stage)"
+                                            : " did not record them (b200reg_batch_set_residuals at its submit)";
   std::lock_guard<std::mutex> lk(b->mu);
   if (ticket < 0 || ticket >= b->next_ticket) return fail(B200REG_EINVAL, "ticket " + std::to_string(ticket) + " was never handed out");
   if (b->jobs.count(ticket)) {
@@ -331,7 +343,7 @@ static int find_captured(b200reg_batch* b, int64_t ticket, int kind, std::shared
   }
   const auto s = b->capture_from.upper_bound(ticket);  // the settings the job copied at its submit
   const Capture cap = s == b->capture_from.begin() ? Capture() : std::prev(s)->second;
-  const bool wanted = kind > 0 ? (cap.cloud_mask & kind) != 0 : kind == 0 ? cap.lm_trace : cap.quatro_matches;
+  const bool wanted = kind > 0 ? (cap.cloud_mask & kind) != 0 : kind == 0 ? cap.lm_trace : kind == MATCHES ? cap.quatro_matches : cap.residuals;
   *none = missing + (wanted ? " was released (b200reg_batch_release)" : off);
   return B200REG_OK;
 }
@@ -362,6 +374,14 @@ int b200reg_batch_quatro_matches(b200reg_batch* b, int64_t ticket, int64_t* offs
   if (const int rc = find_captured(b, ticket, MATCHES, &cap, &none)) return rc;
   return quatro_matches_copy(cap ? &cap->matches : nullptr, offsets_out, capacity, corr_out, inlier_out, src_xyz_out, dst_xyz_out,
                              none);
+}
+
+int b200reg_batch_residuals(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out) {
+  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
+  std::shared_ptr<Captured> cap;
+  std::string none;
+  if (const int rc = find_captured(b, ticket, RESIDUALS, &cap, &none)) return rc;
+  return residuals_copy(cap ? &cap->residuals : nullptr, offsets_out, capacity, nn_out, d2_out, none);
 }
 
 int b200reg_batch_release(b200reg_batch* b, int64_t ticket) {

@@ -496,7 +496,8 @@ __global__ void __launch_bounds__(STEP_THREADS, 16) k_gicp_search(const PairDev*
     }
     knn_walk<SEARCH_STACK, STEP_THREADS>(P.tgt, qx, qy, qz, res, &s_stack[0][threadIdx.x]);
     P.sqd[i] = res.d[0];
-    if (phase == PH_LINEARIZE) P.corr[i] = ((double)res.d[0] < max_corr_dist2) ? res.p[0] : -1;
+    // PH_FITNESS keeps the ungated nearest position: nothing reads corr after that pass but the residual capture
+    P.corr[i] = (phase == PH_FITNESS || (double)res.d[0] < max_corr_dist2) ? res.p[0] : -1;
   }
 }
 
@@ -865,9 +866,25 @@ __global__ void __launch_bounds__(256) k_transform_out(CloudDev c, const float* 
   out3[o + 2] = q.z;
 }
 
+// residual capture (b200reg_residuals): the fitness pass's per-point values of every pair of a call, scattered from sorted
+// source position to ORIGINAL source index; the nearest target position becomes the target point's original index
+__global__ void __launch_bounds__(256) k_residual_rows(const ResidualRow* rows, ResidualOut out) {
+  const ResidualRow& R = rows[blockIdx.y];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= R.n) return;
+  const long long o = R.off + __float_as_int(R.spts[i].w);
+  const int p = R.corr[i];
+  out.nn[o] = p >= 0 ? __float_as_int(R.tpts[p].w) : -1;
+  out.d2[o] = R.sqd[i];
+}
+
 // ---------------------------------------------------------------------------------------
 // host launchers
 // ---------------------------------------------------------------------------------------
+void launch_residual_rows(const ResidualRow* d_rows, int count, int max_n, ResidualOut out, cudaStream_t s) {
+  k_residual_rows<<<dim3((max_n + 255) / 256, count), 256, 0, s>>>(d_rows, out);
+}
+
 int launch_covariances(const CloudDev* d_clouds, int count, int max_n, int k, int method, unsigned long long* slab, cudaStream_t s) {
   dim3 grid((max_n + STEP_THREADS - 1) / STEP_THREADS, count);
   if (k < 1 || method < 0 || method > 4) return -1;

@@ -186,10 +186,26 @@ struct LmCall {
 
 struct PairDev {
   CloudDev src, tgt;
-  int* corr;       // [src.n] sorted target position or -1 (per sorted source position)
+  int* corr;       // [src.n] sorted target position or -1 (per sorted source position); ungated after the fitness pass
   float* sqd;      // [src.n]
   double* mahal;   // [6 * src.n]
   double* partial; // [ceil(src.n / 32) * NRED] one row per warp of the accumulate kernel
+};
+
+// One pair of the residual capture (b200reg_residuals): what its fitness pass left per sorted source position -- sqd, and
+// in corr the ungated nearest target position -- and its first row in the call's slab
+struct ResidualRow {
+  const float4* spts;  // sorted source points, w = original index
+  const float4* tpts;  // sorted target points, w = original index
+  const int* corr;     // [n]
+  const float* sqd;    // [n]
+  int n;
+  long long off;
+};
+// the slab: two arrays over every row of the call
+struct ResidualOut {
+  int* nn;    // [rows] original target index
+  float* d2;  // [rows]
 };
 
 struct LmGraph {  // host side: the instantiated graph of one context's LM solve (gicp.cu: lm_graph_build)

@@ -102,5 +102,7 @@ int launch_assemble_voxelize(const AssembleJob* d_jobs, const SortDev* d_sorts, 
 // CaptureRow of a call (max_n = the longest row)
 void launch_gather_intensity(const BuildDev* d_builds, int count, int max_n, float* const* d_inten, cudaStream_t s);
 void launch_capture_rows(const CaptureRow* d_rows, int nrows, int max_n, cudaStream_t s);
+// gicp.cu: residual capture, every point of every ResidualRow of a call into `out` (max_n = the largest source cloud)
+void launch_residual_rows(const ResidualRow* d_rows, int count, int max_n, ResidualOut out, cudaStream_t s);
 
 }  // namespace b200

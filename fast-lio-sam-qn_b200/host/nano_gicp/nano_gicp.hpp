@@ -20,6 +20,8 @@
 //   * setDebugPrint(true) prints the reference's LM table to std::cout, row for row, but all of it when the solve has
 //     finished on the device (the rows come from the solve's trace, b200reg_lm_trace), not while it runs; lastLmTrace()
 //     returns the records themselves.
+//   * getFitnessScore(max_range) sums the per-point squared distances the device's fitness pass found in the last align()
+//     (b200reg_residuals); lastResiduals() returns those rows.
 #pragma once
 #include <array>
 #include <cmath>
@@ -51,6 +53,12 @@ class NanoGICP {
   using Cov = Eigen::Matrix4d;  // 4th row/col zero (nano_gicp_impl.hpp:354)
   using CovVector = std::vector<Eigen::Matrix4d, Eigen::aligned_allocator<Eigen::Matrix4d>>;  // nano_gicp.hpp:91-106
   using Matrix6d = Eigen::Matrix<double, 6, 6>;
+  // per source point of the last align(), in the source cloud's order: the nearest target point at the final pose and its
+  // fp32 squared distance, the values getFitnessScore() averages (b200reg_residuals)
+  struct Residuals {
+    std::vector<int32_t> nn;
+    std::vector<float> d2;
+  };
 
   NanoGICP() {
     source_kdtree_.reset(new nanoflann::KdTreeFLANN<PointSource>);  // nano_gicp_impl.hpp:62-63
@@ -153,12 +161,17 @@ class NanoGICP {
     b200reg_cloud* t[1] = {tgt_.get()};
     b200reg_ctx* ctx = b200reg_host::context();
     lm_trace_.clear();
+    residuals_.nn.clear();
+    residuals_.d2.clear();
     if (lm_debug_print_) b200reg_ctx_set_lm_trace(ctx, 1);
+    b200reg_ctx_set_residuals(ctx, 1);  // getFitnessScore(max_range) reads the fitness pass's rows
     const int rc = b200reg_gicp_align(ctx, 1, s, t, g, &prm_, &res_);
     if (lm_debug_print_) {
       if (rc == 0) fetch_lm_trace(ctx);
       b200reg_ctx_set_lm_trace(ctx, 0);
     }
+    if (rc == 0) fetch_residuals(ctx);
+    b200reg_ctx_set_residuals(ctx, 0);
     if (rc != 0) {
       std::fprintf(stderr, "b200reg: gicp_align failed (%d): %s\n", rc, b200reg_last_error());
       return;
@@ -188,17 +201,14 @@ class NanoGICP {
     b200reg_host::from_rowmajor(rm, m);
     return m;
   }
-  // mean squared 1-NN distance of the transformed source; the default (no range cap) is what loop_closure.cpp:127 uses
-  double getFitnessScore(double max_range = std::numeric_limits<double>::max()) {
+  // mean squared 1-NN distance of the transformed source; the default (no range cap) is what loop_closure.cpp:127 uses.
+  // With a cap, pcl::Registration::getFitnessScore's rule over the last align()'s rows: a point counts iff its SQUARED
+  // distance is <= max_range, summed in point order in double; DBL_MAX when none counts (a NaN max_range keeps none)
+  double getFitnessScore(double max_range = std::numeric_limits<double>::max()) const {
     if (max_range == std::numeric_limits<double>::max()) return res_.fitness;
-    std::vector<float> xyz(3 * input_->size());
-    b200reg_transform_cloud(b200reg_host::context(), src_.get(), res_.Tf, xyz.data());
-    std::vector<int32_t> idx(input_->size());
-    std::vector<float> d2(input_->size());
-    b200reg_knn(b200reg_host::context(), tgt_.get(), xyz.data(), input_->size(), 12, 1, idx.data(), d2.data());
     double s = 0;
     size_t nr = 0;
-    for (float v : d2)
+    for (float v : residuals_.d2)
       if (v <= max_range) {
         s += v;
         nr++;
@@ -209,6 +219,8 @@ class NanoGICP {
   const b200reg_result& lastResult() const { return res_; }
   // every LM trial of the last align(), in execution order; empty unless setDebugPrint(true)
   const std::vector<b200reg_lm_trial>& lastLmTrace() const { return lm_trace_; }
+  // the fitness pass's rows of the last align() (empty before the first and after a failed one)
+  const Residuals& lastResiduals() const { return residuals_; }
 
   // nano_gicp.hpp:121-122: search the clouds set by setInputSource / setInputTarget (radiusSearch takes a SQUARED radius)
   std::shared_ptr<nanoflann::KdTreeFLANN<PointSource>> source_kdtree_;
@@ -230,6 +242,18 @@ class NanoGICP {
     if (rc != 0) {
       std::fprintf(stderr, "b200reg: lm_trace failed (%d): %s\n", rc, b200reg_last_error());
       lm_trace_.clear();
+    }
+  }
+  void fetch_residuals(b200reg_ctx* ctx) {
+    int64_t off[2] = {0, 0};
+    b200reg_residuals(ctx, off, 0, nullptr, nullptr);  // B200REG_ESTATE unless the source is empty: off[1] is the count either way
+    residuals_.nn.resize(off[1]);
+    residuals_.d2.resize(off[1]);
+    const int rc = b200reg_residuals(ctx, off, residuals_.d2.size(), residuals_.nn.data(), residuals_.d2.data());
+    if (rc != 0) {
+      std::fprintf(stderr, "b200reg: residuals failed (%d): %s\n", rc, b200reg_last_error());
+      residuals_.nn.clear();
+      residuals_.d2.clear();
     }
   }
   // what LsqRegistration prints with lm_debug_print_ (lsq_registration_impl.hpp:95-99, 183-189), one row per trial
@@ -303,6 +327,7 @@ class NanoGICP {
   bool src_cov_ok_ = false, tgt_cov_ok_ = false, converged_ = false;
   bool lm_debug_print_ = false;  // lsq_registration.hpp:92
   std::vector<b200reg_lm_trial> lm_trace_;
+  Residuals residuals_;
   std::array<float, 16> final_;
   Matrix6d final_hessian_;
   int ransac_iterations_ = 0;

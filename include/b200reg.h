@@ -347,6 +347,33 @@ int b200reg_ctx_set_quatro_matches(b200reg_ctx* ctx, int enable);
 int b200reg_quatro_matches(b200reg_ctx* ctx, int64_t* offsets_out, size_t capacity, int32_t* corr_out, int32_t* inlier_out,
                            float* src_xyz_out, float* dst_xyz_out);
 
+/* Residuals: what the fitness pass of the fine stage (getFitnessScore, b200reg_result::fitness) found per source point
+ * at the final pose, per pair: the nearest target point and its squared distance.
+ *   Which calls record.  Recording is off by default.  While it is on, every call that runs the fine stage records:
+ *     b200reg_gicp_align, b200reg_icp_alignment, b200reg_loop_closure, b200reg_perform_loop_closure, and the batch jobs of
+ *     all three kinds (b200reg_batch_set_residuals).  Each such call replaces the stored rows.  Such a call with recording
+ *     off discards them.  b200reg_quatro_align, b200reg_quatro_align_ex and the taps leave them untouched.
+ *   Rows.  Pairs follow the caller's pair or query order; pair i has one row per point of its source cloud, in the cloud's
+ *     ORIGINAL point order.  Row r is nn_out[r], the original index of the nearest target point after the final fp32
+ *     transformation (x*c0 + (y*c1 + (z*c2 + c3)), ties to the lower index; -1 only if no target point is a candidate), and
+ *     d2_out[r], its fp32 squared distance: bit for bit the value the fitness pass sums, so the mean of a pair's d2 is its
+ *     fitness up to that pass's fixed summation order.  A pair whose fine stage did not run has an empty row: a query with
+ *     no candidate, and a pair whose Quatro solve is invalid.
+ *   Indices.  For the raw-buffer calls the rows and nn are rows of the caller's buffers.  For b200reg_perform_loop_closure
+ *     the rows are rows of its SOURCE loop cloud (the same rows as COARSE in Quatro mode) and nn indexes its TARGET loop
+ *     cloud.  For b200reg_gicp_align they are rows of the cloud handles.
+ *   Cost.  With recording off nothing is allocated or launched.  With it on, a call allocates 8 bytes per source point of
+ *     every pair that can run the fine stage, before its first stage, for its own duration, and adds one kernel launch per
+ *     fine stage.  Results, LM traces, loop clouds and Quatro matches stay byte-identical.  If the rows cannot be allocated
+ *     the call returns B200REG_ECUDA with the bytes needed.  */
+int b200reg_ctx_set_residuals(b200reg_ctx* ctx, int enable);
+/* The residuals of the context's most recent recording call, as CSR over that call's pairs: pair i's rows are
+ * offsets_out[i] .. offsets_out[i + 1]), offsets_out has count + 1 entries.  Either output pointer may be NULL.  If the
+ * rows exceed `capacity` the call fills offsets_out, writes nothing else and returns B200REG_ESTATE.  offsets_out == NULL:
+ * returns that call's pair count (>= 0) and writes nothing.  Before any recording call, after a call that did not record,
+ * and after a call that failed: B200REG_ESTATE.                                                                          */
+int b200reg_residuals(b200reg_ctx* ctx, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out);
+
 /* ---- "next" rows (SURVEY.md §8f): device-resident keyframes, candidate search, cloud assembly ---------- */
 typedef struct b200reg_keyframes b200reg_keyframes;
 
@@ -520,6 +547,15 @@ int b200reg_batch_lm_trace(b200reg_batch* b, int64_t ticket, int64_t* offsets_ou
 int b200reg_batch_set_quatro_matches(b200reg_batch* b, int enable);
 int b200reg_batch_quatro_matches(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity, int32_t* corr_out,
                                  int32_t* inlier_out, float* src_xyz_out, float* dst_xyz_out);
+/* Residuals of driver jobs (b200reg_ctx_set_residuals / b200reg_residuals per job).  The setting is off by default and is
+ * copied at submit like the ones above.  A job of any of the three kinds that ran with it on returns, byte for byte, what
+ * b200reg_residuals returns on a context after the synchronous call with the same inputs.  The record moves into the
+ * job's outputs without a copy and stays readable from b200reg_batch_wait until b200reg_batch_release or
+ * b200reg_batch_destroy.  The getter follows the rules of b200reg_residuals and the ticket rules above; a job submitted
+ * with recording off holds no residuals (B200REG_ESTATE).                                                              */
+int b200reg_batch_set_residuals(b200reg_batch* b, int enable);
+int b200reg_batch_residuals(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity, int32_t* nn_out,
+                            float* d2_out);
 int b200reg_batch_release(b200reg_batch* b, int64_t ticket);
 int64_t b200reg_batch_launch_count(const b200reg_batch* b);
 int b200reg_batch_depth(const b200reg_batch* b);
