@@ -179,61 +179,42 @@ def _check(rc):
         raise B200RegError("b200reg error %d: %s" % (rc, lib().b200reg_last_error().decode()))
 
 
-def _lm_trace(get):
-    """The CSR trace behind get(offsets, capacity, trials) (b200reg_lm_trace's rules) -> one LM_TRIAL_DTYPE array per pair."""
-    n = get(None, C.c_size_t(0), None)
+def _csr(get, columns):
+    """The CSR record behind get(offsets, capacity, *outputs) (the rules every record getter shares: b200reg_lm_trace,
+    b200reg_loop_clouds, b200reg_quatro_matches, b200reg_residuals), one output per (dtype, row shape) in `columns` ->
+    per pair, a tuple of its rows of each column."""
+    none = [None] * len(columns)
+    n = get(None, C.c_size_t(0), *none)
     _check(min(n, 0))
     offsets = np.empty(n + 1, np.int64)
-    rc = get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None)  # offsets only
+    rc = get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), *none)  # offsets only
     if rc != ESTATE:
         _check(rc)
-    trials = np.empty(int(offsets[-1]), LM_TRIAL_DTYPE)
-    _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(trials)), trials.ctypes.data_as(C.c_void_p)))
-    return [trials[offsets[i]:offsets[i + 1]] for i in range(n)]
+    m = int(offsets[-1])
+    cols = [np.empty((m,) + tuple(shape), dtype) for dtype, shape in columns]
+    _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(m), *(a.ctypes.data_as(C.c_void_p) for a in cols)))
+    return [tuple(a[lo:hi] for a in cols) for lo, hi in zip(offsets[:-1], offsets[1:])]
+
+
+def _lm_trace(get):
+    """-> one LM_TRIAL_DTYPE array per pair."""
+    return [t for (t,) in _csr(get, [(LM_TRIAL_DTYPE, ())])]
 
 
 def _loop_clouds(get):
-    """The CSR clouds behind get(offsets, capacity, xyzi) (b200reg_loop_clouds' rules) -> one (n, 4) float32 array per pair."""
-    n = get(None, C.c_size_t(0), None)
-    _check(min(n, 0))
-    offsets = np.empty(n + 1, np.int64)
-    rc = get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None)  # offsets only
-    if rc != ESTATE:
-        _check(rc)
-    pts = np.empty((int(offsets[-1]), 4), np.float32)
-    _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(len(pts)), pts.ctypes.data_as(C.c_void_p)))
-    return [pts[offsets[i]:offsets[i + 1]] for i in range(n)]
+    """-> one (n, 4) float32 array (x, y, z, intensity) per pair."""
+    return [p for (p,) in _csr(get, [(np.float32, (4,))])]
 
 
 def _quatro_matches(get):
-    """The CSR matches behind get(offsets, capacity, corr, inlier, src_xyz, dst_xyz) (b200reg_quatro_matches' rules) -> one
-    dict per pair: corr (m, 2) int32 (src, dst), inlier (m,) int32, src_xyz and dst_xyz (m, 3) float32."""
-    n = get(None, C.c_size_t(0), None, None, None, None)
-    _check(min(n, 0))
-    offsets = np.empty(n + 1, np.int64)
-    rc = get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None, None, None, None)  # offsets only
-    if rc != ESTATE:
-        _check(rc)
-    m = int(offsets[-1])
-    corr, inlier = np.empty((m, 2), np.int32), np.empty(m, np.int32)
-    sx, dx = np.empty((m, 3), np.float32), np.empty((m, 3), np.float32)
-    _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(m), *(a.ctypes.data_as(C.c_void_p) for a in (corr, inlier, sx, dx))))
-    return [dict(corr=corr[a:b], inlier=inlier[a:b], src_xyz=sx[a:b], dst_xyz=dx[a:b]) for a, b in zip(offsets[:-1], offsets[1:])]
+    """-> one dict per pair: corr (m, 2) int32 (src, dst), inlier (m,) int32, src_xyz and dst_xyz (m, 3) float32."""
+    rows = _csr(get, [(np.int32, (2,)), (np.int32, ()), (np.float32, (3,)), (np.float32, (3,))])
+    return [dict(zip(("corr", "inlier", "src_xyz", "dst_xyz"), r)) for r in rows]
 
 
 def _residuals(get):
-    """The CSR rows behind get(offsets, capacity, nn, d2) (b200reg_residuals' rules) -> one (nn int32[n], d2 float32[n])
-    pair per pair."""
-    n = get(None, C.c_size_t(0), None, None)
-    _check(min(n, 0))
-    offsets = np.empty(n + 1, np.int64)
-    rc = get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(0), None, None)  # offsets only
-    if rc != ESTATE:
-        _check(rc)
-    m = int(offsets[-1])
-    nn, d2 = np.empty(m, np.int32), np.empty(m, np.float32)
-    _check(get(offsets.ctypes.data_as(C.c_void_p), C.c_size_t(m), nn.ctypes.data_as(C.c_void_p), d2.ctypes.data_as(C.c_void_p)))
-    return [(nn[a:b], d2[a:b]) for a, b in zip(offsets[:-1], offsets[1:])]
+    """-> one (nn int32[n], d2 float32[n]) pair per pair."""
+    return _csr(get, [(np.int32, ()), (np.float32, ())])
 
 
 def fitness_score(d2, max_range=float("inf")):

@@ -80,6 +80,99 @@ int sorted_to_original(b200reg_ctx* c, const CloudDev& d, std::vector<int>& orig
   if (pts_out) pts_out->swap(pts);
   return B200REG_OK;
 }
+
+// ---- recorded outputs -------------------------------------------------------------------------------------------------
+void CsrRecord::remap(int count, const std::vector<int>& where) {
+  const size_t stages = where.empty() ? (size_t)count : where.size();
+  std::vector<int64_t> o(count + 1, 0);
+  size_t k = 0;  // the next stage pair
+  for (int i = 0; i < count; i++) {
+    int64_t n = 0;
+    if (k < stages && (where.empty() ? (int)k : where[k]) == i) {
+      if (k + 1 < offsets.size()) n = offsets[k + 1] - offsets[k];
+      k++;
+    }
+    o[i + 1] = o[i] + n;
+  }
+  if (offsets.empty()) rows.clear();  // no stage wrote the record this call
+  offsets.swap(o);
+}
+
+Recording::Recording(b200reg_ctx* c, unsigned touches) : c_(c) {
+  if (!c || c->recording) return;
+  c->recording = true;
+  touches_ = touches;
+  for (int r = 0; r < Records::N; r++)
+    if (touches >> r & 1) c->records.rec[r].offsets.clear();  // `rows` keeps its memory for the next recording call
+  c->records.held &= ~touches;
+}
+
+Recording::~Recording() {
+  if (touches_) c_->recording = false;
+}
+
+int Recording::commit(int rc, int count, const std::vector<int>& where) {
+  if (rc || !touches_) return rc;
+  for (int r = 0; r < Records::N; r++)
+    if ((touches_ >> r & 1) && c_->capture.wants(r)) {
+      c_->records.rec[r].remap(count, where);
+      c_->records.held |= 1u << r;
+    }
+  return rc;
+}
+
+namespace {
+// each record's columns (bytes per row, in the order of the getter's outputs) and how its capacity message counts rows
+struct RecordLayout {
+  size_t width[4];
+  const char* holds;
+  const char* rows;
+};
+const RecordLayout kRecordLayout[Records::N] = {
+    {{sizeof(b200reg_lm_trial)}, "LM trace holds ", " records"},
+    {{4, 4}, "residuals hold ", " rows"},               // nn, d2
+    {{8, 4, 12, 12}, "Quatro matches number ", ""},     // corr, inlier, src xyz, dst xyz
+    {{16}, "loop clouds hold ", " points"},             // (x, y, z, intensity), one record per kind
+    {{16}, "loop clouds hold ", " points"},
+    {{16}, "loop clouds hold ", " points"},
+    {{16}, "loop clouds hold ", " points"},
+};
+}  // namespace
+
+int record_copy(const Records* rs, int r, const std::string& none, int64_t* offsets_out, size_t capacity,
+                std::initializer_list<void*> cols) {
+  if (r < 0) return fail(B200REG_EINVAL, "kind: one of B200REG_CLOUD_SOURCE, _TARGET, _COARSE, _FINAL");
+  if (!rs || !(rs->held >> r & 1)) return fail(B200REG_ESTATE, none);
+  const CsrRecord& rec = rs->rec[r];
+  if (!offsets_out) return (int)rec.offsets.size() - 1;
+  memcpy(offsets_out, rec.offsets.data(), sizeof(int64_t) * rec.offsets.size());
+  const RecordLayout& l = kRecordLayout[r];
+  const size_t total = (size_t)rec.offsets.back();
+  if (total > capacity)
+    return fail(B200REG_ESTATE, l.holds + std::to_string(total) + l.rows + ", capacity " + std::to_string(capacity));
+  const char* block = rec.rows.data();
+  int j = 0;
+  for (void* out : cols) {
+    const size_t bytes = l.width[j++] * total;
+    if (out && bytes) memcpy(out, block, bytes);
+    block += bytes;
+  }
+  return B200REG_OK;
+}
+
+int cloud_record(int kind) {
+  for (int s = 0; s < 4; s++)
+    if (kind == 1 << s) return Records::CLOUD + s;
+  return -1;
+}
+
+static int no_ctx() { return fail(B200REG_EINVAL, "ctx is NULL"); }
+template <class T>
+static int set_capture(b200reg_ctx* c, T Capture::*setting, T value) {
+  if (!c) return no_ctx();
+  c->capture.*setting = value;
+  return B200REG_OK;
+}
 }  // namespace b200
 
 extern "C" {
@@ -175,6 +268,49 @@ int b200reg_ctx_synchronize(b200reg_ctx* c) {
 }
 
 int64_t b200reg_ctx_launch_count(const b200reg_ctx* c) { return c ? c->launches : 0; }
+
+// the settings and getters of the recorded outputs (Capture, Records)
+int b200reg_ctx_set_lm_trace(b200reg_ctx* c, int enable) { return set_capture(c, &Capture::lm_trace, enable != 0); }
+
+int b200reg_lm_trace(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out) {
+  return c ? record_copy(&c->records, Records::TRACE, "no LM trace: the context's last LM solve was not traced, or failed (b200reg_ctx_set_lm_trace)",
+                         offsets_out, capacity, {trials_out})
+           : no_ctx();
+}
+
+int b200reg_ctx_set_loop_clouds(b200reg_ctx* c, int mask) {
+  if (c && (mask & ~(B200REG_CLOUD_SOURCE | B200REG_CLOUD_TARGET | B200REG_CLOUD_COARSE | B200REG_CLOUD_FINAL)))
+    return fail(B200REG_EINVAL, "mask: an OR of B200REG_CLOUD_SOURCE, _TARGET, _COARSE, _FINAL");
+  return set_capture(c, &Capture::cloud_mask, mask);
+}
+
+int b200reg_loop_clouds(b200reg_ctx* c, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out) {
+  return c ? record_copy(&c->records, cloud_record(kind),
+                         "no such loop clouds: the context's last loop-closure call did not capture this kind, or failed "
+                         "(b200reg_ctx_set_loop_clouds)",
+                         offsets_out, capacity, {xyzi_out})
+           : no_ctx();
+}
+
+int b200reg_ctx_set_quatro_matches(b200reg_ctx* c, int enable) { return set_capture(c, &Capture::quatro_matches, enable != 0); }
+
+int b200reg_quatro_matches(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, int32_t* corr_out, int32_t* inlier_out,
+                           float* src_xyz_out, float* dst_xyz_out) {
+  return c ? record_copy(&c->records, Records::MATCHES,
+                         "no Quatro matches: the context's last call with a Quatro stage did not record them, or failed "
+                         "(b200reg_ctx_set_quatro_matches)",
+                         offsets_out, capacity, {corr_out, inlier_out, src_xyz_out, dst_xyz_out})
+           : no_ctx();
+}
+
+int b200reg_ctx_set_residuals(b200reg_ctx* c, int enable) { return set_capture(c, &Capture::residuals, enable != 0); }
+
+int b200reg_residuals(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out) {
+  return c ? record_copy(&c->records, Records::RESIDUALS,
+                         "no residuals: the context's last registration did not record them, or failed (b200reg_ctx_set_residuals)",
+                         offsets_out, capacity, {nn_out, d2_out})
+           : no_ctx();
+}
 
 int b200reg_ctx_set_profiling(b200reg_ctx* c, int enable) {
   if (!c) return fail(B200REG_EINVAL, "ctx is NULL");

@@ -8,6 +8,7 @@
 
 #include <cstddef>
 #include <cstdint>
+#include <initializer_list>
 #include <memory>
 #include <string>
 #include <vector>
@@ -33,6 +34,50 @@ int fail(int code, const std::string& msg);  // sets b200reg_last_error() and re
 
 enum { CLS_BUILD = 0, CLS_COV = 1, CLS_STEP = 2, CLS_MISC = 3, CLS_FPFH = 4, CLS_MATCH = 5, CLS_SEARCH = 6, CLS_ACCUM = 7, CLS_CTRL = 8, NCLS = 9 };
 
+namespace b200 {
+
+// One recorded output of a call, CSR over its pairs, on the host: `offsets` (pairs + 1; empty until a stage of the call
+// writes the record) and `rows`, the record's columns one block after another, each column a fixed number of bytes per
+// row (record_copy's table).  The device slab a stage fills has the same layout, so one copy brings it to the host.
+// `rows` keeps its memory from call to call: a stage resizes it in place.
+struct CsrRecord {
+  std::vector<int64_t> offsets;
+  std::vector<char> rows;
+  // Stage pair k becomes caller pair where[k] (empty `where`: pair k); every other caller pair, and every pair the
+  // record does not hold, gets an empty row.  `where` ascends, as every stage's subset of its caller's pairs does, so the
+  // rows keep their order and only the offsets change.
+  void remap(int count, const std::vector<int>& where);
+};
+
+// The records a call can leave for its caller (include/b200reg.h: b200reg_lm_trace, b200reg_residuals,
+// b200reg_quatro_matches, b200reg_loop_clouds), and which of them the most recent recording call that touched them stored
+struct Records {
+  enum { TRACE, RESIDUALS, MATCHES, CLOUD, N = CLOUD + 4 };  // CLOUD + s: the loop clouds of kind 1 << s (B200REG_CLOUD_*)
+  CsrRecord rec[N];
+  unsigned held = 0;  // bit r: rec[r] is stored
+};
+constexpr unsigned REC_TRACE = 1u << Records::TRACE, REC_RESIDUALS = 1u << Records::RESIDUALS, REC_MATCHES = 1u << Records::MATCHES,
+                   REC_CLOUDS = 15u << Records::CLOUD, REC_ALL = REC_TRACE | REC_RESIDUALS | REC_MATCHES | REC_CLOUDS;
+
+// The recording settings (b200reg_ctx_set_loop_clouds / _set_lm_trace / _set_quatro_matches / _set_residuals): a
+// context's, or the driver's that a batch job copies at its submit
+struct Capture {
+  int cloud_mask = 0;
+  bool lm_trace = false;
+  bool quatro_matches = false;
+  bool residuals = false;
+  bool on() const { return cloud_mask || lm_trace || quatro_matches || residuals; }
+  bool wants(int r) const {  // record r (Records) is recorded
+    return r == Records::TRACE ? lm_trace : r == Records::RESIDUALS ? residuals : r == Records::MATCHES ? quatro_matches
+                                                                                                       : (cloud_mask >> (r - Records::CLOUD) & 1) != 0;
+  }
+  bool operator!=(const Capture& o) const {
+    return cloud_mask != o.cloud_mask || lm_trace != o.lm_trace || quatro_matches != o.quatro_matches || residuals != o.residuals;
+  }
+};
+
+}  // namespace b200
+
 struct b200reg_ctx {
   int device = 0;
   cudaStream_t own_stream = nullptr;
@@ -54,43 +99,13 @@ struct b200reg_ctx {
     PairState* h_states = nullptr;  // pinned read-back
     LmGraph graph;
   } lm;
-  // LM trace of the most recent call that ran the LM solve (b200reg_ctx_set_lm_trace / b200reg_lm_trace), CSR over the pairs
-  // of that call, on the host
-  struct LmTrace {
-    bool enabled = false;
-    bool valid = false;  // false before a traced solve and after an untraced one
-    std::vector<int64_t> offsets;  // pairs + 1
-    std::vector<b200reg_lm_trial> trials;
-  } lm_trace;
-  // loop clouds (b200reg_ctx_set_loop_clouds / b200reg_loop_clouds): the kinds the capturing calls record, and the clouds of
-  // the most recent such call, CSR over its pairs per kind (slot = log2 of the kind's bit), on the host
-  struct LoopClouds {
-    int mask = 0;
-    int stored = 0;  // kinds held; 0 before a capturing call and after an uncaptured one
-    std::vector<int64_t> offsets[4];  // pairs + 1 each
-    std::vector<float4> pts[4];       // (x, y, z, intensity)
-  } loop_clouds;
-  // Quatro matches (b200reg_ctx_set_quatro_matches / b200reg_quatro_matches) of the most recent call that reached the Quatro
-  // stage with recording on, CSR over its pairs, on the host.  `words` holds four blocks over all `total` matches, as the
-  // capture slab does: corr (2 per match), inlier (1), src xyz (3 float bits), dst xyz (3 float bits)
-  struct QuatroMatches {
-    bool enabled = false;
-    bool valid = false;  // false before a recording call, after one that did not record and after one that failed
-    std::vector<int64_t> offsets;  // pairs + 1
-    std::vector<int32_t> words;    // 9 per match
-  } quatro_matches;
-  // residuals (b200reg_ctx_set_residuals / b200reg_residuals) of the most recent call that ran the fine stage with recording
-  // on, CSR over its pairs, on the host: per source point in original order, the fitness pass's nearest target point
-  // (original index) and fp32 squared distance
-  struct Residuals {
-    bool enabled = false;
-    bool valid = false;  // false before a recording call, after one that did not record and after one that failed
-    std::vector<int64_t> offsets;  // pairs + 1
-    std::vector<int32_t> nn;
-    std::vector<float> d2;
-    int32_t* slab = nullptr;  // device rows reserved by the call in flight (ResidualSlab): nn block, then d2 block
-    size_t slab_points = 0;
-  } residuals;
+  // the recorded outputs: what to record, what is stored, and whether a recording call is running (Recording)
+  Capture capture;
+  Records records;
+  bool recording = false;
+  // device rows reserved for the residuals by the call in flight (ResidualSlab): nn block, then d2 block
+  int32_t* residual_slab = nullptr;
+  size_t residual_slab_points = 0;
   // the path's one collective (b200reg_comm_*): NCCL communicator of this rank
   ncclComm_t comm = nullptr;
   int rank = -1, world = 1;
@@ -240,37 +255,34 @@ int kf_job_create(b200reg_keyframes* kf, int device, int count, const int32_t* q
                   const b200reg_loop_config* cfg, std::shared_ptr<KfJob>* out);
 int kf_job_run(b200reg_ctx* c, KfJob* j, b200reg_result* out, b200reg_quatro_info* quatro_out);
 
-// The stored LM trace belongs to the pairs of the last b200reg_gicp_align.  A caller that ran that solve on a subset of its
-// `count` pairs (solve pair k = its pair where[k]; `where` empty when no solve ran) renumbers it to its own pairs; the
-// others get no records.  Does nothing but keep the trace invalid when tracing is off.  (api_gicp.cu)
-void lm_trace_remap(b200reg_ctx* c, int count, const std::vector<int>& where);
+// The one lifecycle rule of the records (include/b200reg.h), for an entry point that records.  Constructed on entry,
+// before the argument checks, it discards every record in `touches`.  The call's stages then write their records into
+// c->records as they run, numbered as they saw their pairs.  commit() stores them, renumbered to the caller's pairs, only
+// when the call succeeds, and only those the settings ask for.  A scope opened while another is open (b200reg_gicp_align or
+// b200reg_quatro_align as a stage of a larger call) does nothing: the outermost call discards and stores for all of them.
+class Recording {
+ public:
+  Recording(b200reg_ctx* c, unsigned touches);
+  ~Recording();
+  Recording(const Recording&) = delete;
+  Recording& operator=(const Recording&) = delete;
+  // rc == B200REG_OK: stores the touched records, stage pair k as the caller's pair where[k] (CsrRecord::remap).  Returns rc.
+  int commit(int rc, int count, const std::vector<int>& where = {});
 
-// The copy-out rules of b200reg_lm_trace / b200reg_loop_clouds over one stored trace or set of clouds: a context's, or a
-// batch-driver job's (b200reg_batch_lm_trace / b200reg_batch_loop_clouds).  A kind that is not one B200REG_CLOUD_* bit is
-// B200REG_EINVAL; a null `tr` / `lc`, an invalid trace or a kind not held is B200REG_ESTATE with the message `none`;
-// then the CSR offsets and the capacity rule of include/b200reg.h.  (api_gicp.cu, api_loop_clouds.cu)
-int lm_trace_copy(const b200reg_ctx::LmTrace* tr, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out,
-                  const std::string& none);
-int loop_clouds_copy(const b200reg_ctx::LoopClouds* lc, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out,
-                     const std::string& none);
+ private:
+  b200reg_ctx* c_;
+  unsigned touches_ = 0;  // 0: a nested scope
+};
 
-// The stored Quatro matches belong to the pairs of the last b200reg_quatro_align.  A caller that ran it on a subset of its
-// `count` pairs (Quatro pair k = its pair where[k]; `where` empty when no Quatro stage ran) renumbers them to its own pairs;
-// the others get empty rows.  Does nothing but keep them invalid when recording is off.  (api_quatro.cu)
-void quatro_matches_remap(b200reg_ctx* c, int count, const std::vector<int>& where);
-// The copy-out rules of b200reg_quatro_matches over a context's or a batch-driver job's record (b200reg_batch_quatro_matches):
-// a null or invalid record is B200REG_ESTATE with the message `none`; then the CSR offsets and the capacity rule.
-int quatro_matches_copy(const b200reg_ctx::QuatroMatches* qm, int64_t* offsets_out, size_t capacity, int32_t* corr_out,
-                        int32_t* inlier_out, float* src_xyz_out, float* dst_xyz_out, const std::string& none);
+// The copy-out rules of every record getter, over a context's records or a batch-driver job's (null: none held): r < 0
+// (a loop-cloud kind that is not one B200REG_CLOUD_* bit, cloud_record) is B200REG_EINVAL; a record not held is
+// B200REG_ESTATE with the message `none`; offsets_out NULL returns the pair count; then the offsets, the capacity rule of
+// include/b200reg.h, and column j of the record into cols[j] unless that is NULL.  (api.cu)
+int record_copy(const Records* rs, int r, const std::string& none, int64_t* offsets_out, size_t capacity,
+                std::initializer_list<void*> cols);
+// Records::CLOUD + log2 of a B200REG_CLOUD_* bit; -1 for anything else
+int cloud_record(int kind);
 
-// The stored residuals belong to the pairs of the last b200reg_gicp_align.  A caller that ran that solve on a subset of its
-// `count` pairs (solve pair k = its pair where[k]) renumbers them to its own pairs; the others get empty rows.  Does
-// nothing but keep them invalid when recording is off.  (api_gicp.cu)
-void residuals_remap(b200reg_ctx* c, int count, const std::vector<int>& where);
-// The copy-out rules of b200reg_residuals over a context's or a batch-driver job's record (b200reg_batch_residuals): a null
-// or invalid record is B200REG_ESTATE with the message `none`; then the CSR offsets and the capacity rule.
-int residuals_copy(const b200reg_ctx::Residuals* r, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out,
-                   const std::string& none);
 // The device rows of the residual capture of one b200reg_icp_alignment, b200reg_loop_closure or
 // b200reg_perform_loop_closure call, reserved as soon as its source clouds exist, so that a failed allocation costs no
 // registration: one row per source point of every pair that can run the fine stage.  The call's b200reg_gicp_align writes
@@ -280,8 +292,8 @@ class ResidualSlab {
   explicit ResidualSlab(b200reg_ctx* c) : c_(c), scratch_(c) {}
   int reserve(int count, const size_t* src_n);
   ~ResidualSlab() {
-    c_->residuals.slab = nullptr;
-    c_->residuals.slab_points = 0;
+    c_->residual_slab = nullptr;
+    c_->residual_slab_points = 0;
   }
 
  private:
@@ -295,28 +307,24 @@ int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* sr
                              const b200reg_quatro_params* qp, const b200reg_gicp_params* gp, b200reg_result* out,
                              b200reg_quatro_info* quatro_out, float* fine_tf16);
 
-// The loop clouds of one call of b200reg_icp_alignment, b200reg_loop_closure or b200reg_perform_loop_closure, over the
-// CALLER's pairs (api_loop_clouds.cu).  The constructor discards the stored clouds.  The call then hands over what its
-// stages ran on, numbered as the stages saw their pairs: stage pair k is the caller's pair where[k], and this is the one
-// place that renumbers them (an empty `where`: stage pair k is the caller's pair k).
-//   clouds()  the source and target clouds, as soon as they exist: sizes the device slab for every row that can be present,
-//             so that a failed allocation costs no registration;
+// The loop clouds of one call of b200reg_icp_alignment, b200reg_loop_closure or b200reg_perform_loop_closure, numbered as
+// its stages saw their pairs (api_loop_clouds.cu); the call's Recording renumbers them to its own pairs.
+//   clouds()  the `count` source and target clouds of the stages, as soon as they exist: sizes the device slab for every
+//             row that can be present, so that a failed allocation costs no registration;
 //   finish()  the coarse stage's infos (nullptr: the call has no Quatro stage; the fine stage ran where they are valid) and
-//             the fine stage's fp32 transforms (16 per stage pair): writes every row in one launch and stores the result.
+//             the fine stage's fp32 transforms (16 per stage pair): writes every row in one launch and into c->records.
 // With capture off every step returns at once: no allocation, no launch.
 class LoopCapture {
  public:
-  LoopCapture(b200reg_ctx* c, int count);
+  explicit LoopCapture(b200reg_ctx* c) : c_(c), mask_(c->capture.cloud_mask), scratch_(c) {}
   bool on() const { return mask_ != 0; }
-  int clouds(const std::vector<int>& where, b200reg_cloud* const* src, b200reg_cloud* const* dst, bool src_tgt_rows,
-             bool coarse_rows);
+  int clouds(int count, b200reg_cloud* const* src, b200reg_cloud* const* dst, bool src_tgt_rows, bool coarse_rows);
   int finish(const b200reg_quatro_info* qi, const float* fine_tf16);
 
  private:
   b200reg_ctx* c_;
-  int count_, mask_;
+  int mask_;
   Scratch scratch_;
-  std::vector<int> where_;
   std::vector<const b200reg_cloud*> src_, dst_;  // per stage pair
   bool src_tgt_rows_ = false;
   float4* slab_[4] = {nullptr, nullptr, nullptr, nullptr};

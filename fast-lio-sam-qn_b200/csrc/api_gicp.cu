@@ -75,89 +75,18 @@ void lm_arena_free(b200reg_ctx* c) {
   a = b200reg_ctx::LmArena();
 }
 
-void lm_trace_remap(b200reg_ctx* c, int count, const std::vector<int>& where) {
-  auto& tr = c->lm_trace;
-  if (!tr.enabled) {
-    tr.valid = false;
-    return;
-  }
-  std::vector<int> solved(count, -1);  // caller pair -> solve pair
-  for (size_t k = 0; k < where.size(); k++) solved[where[k]] = (int)k;
-  std::vector<int64_t> offsets(count + 1, 0);
-  std::vector<b200reg_lm_trial> trials;
-  for (int i = 0; i < count; i++) {
-    const int k = solved[i];
-    if (k >= 0) trials.insert(trials.end(), tr.trials.begin() + tr.offsets[k], tr.trials.begin() + tr.offsets[k + 1]);
-    offsets[i + 1] = (int64_t)trials.size();
-  }
-  tr.offsets.swap(offsets);
-  tr.trials.swap(trials);
-  tr.valid = true;
-}
-
-int lm_trace_copy(const b200reg_ctx::LmTrace* tr, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out,
-                  const std::string& none) {
-  if (!tr || !tr->valid) return fail(B200REG_ESTATE, none);
-  const int pairs = (int)tr->offsets.size() - 1;
-  if (!offsets_out) return pairs;
-  memcpy(offsets_out, tr->offsets.data(), sizeof(int64_t) * tr->offsets.size());
-  if (tr->trials.size() > capacity)
-    return fail(B200REG_ESTATE, "LM trace holds " + std::to_string(tr->trials.size()) + " records, capacity " + std::to_string(capacity));
-  if (trials_out && !tr->trials.empty()) memcpy(trials_out, tr->trials.data(), sizeof(b200reg_lm_trial) * tr->trials.size());
-  return B200REG_OK;
-}
-
-void residuals_remap(b200reg_ctx* c, int count, const std::vector<int>& where) {
-  auto& r = c->residuals;
-  if (!r.enabled) {
-    r.valid = false;
-    return;
-  }
-  std::vector<int> solved(count, -1);  // caller pair -> solve pair
-  for (size_t k = 0; k < where.size(); k++) solved[where[k]] = (int)k;
-  std::vector<int64_t> offsets(count + 1, 0);
-  std::vector<int32_t> nn;
-  std::vector<float> d2;
-  for (int i = 0; i < count; i++) {
-    const int k = solved[i];
-    if (k >= 0) {
-      nn.insert(nn.end(), r.nn.begin() + r.offsets[k], r.nn.begin() + r.offsets[k + 1]);
-      d2.insert(d2.end(), r.d2.begin() + r.offsets[k], r.d2.begin() + r.offsets[k + 1]);
-    }
-    offsets[i + 1] = (int64_t)nn.size();
-  }
-  r.offsets.swap(offsets);
-  r.nn.swap(nn);
-  r.d2.swap(d2);
-  r.valid = true;
-}
-
-int residuals_copy(const b200reg_ctx::Residuals* r, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out,
-                   const std::string& none) {
-  if (!r || !r->valid) return fail(B200REG_ESTATE, none);
-  const int pairs = (int)r->offsets.size() - 1;
-  if (!offsets_out) return pairs;
-  memcpy(offsets_out, r->offsets.data(), sizeof(int64_t) * r->offsets.size());
-  if (r->nn.size() > capacity)
-    return fail(B200REG_ESTATE, "residuals hold " + std::to_string(r->nn.size()) + " rows, capacity " + std::to_string(capacity));
-  if (nn_out && !r->nn.empty()) memcpy(nn_out, r->nn.data(), sizeof(int32_t) * r->nn.size());
-  if (d2_out && !r->d2.empty()) memcpy(d2_out, r->d2.data(), sizeof(float) * r->d2.size());
-  return B200REG_OK;
-}
-
 int ResidualSlab::reserve(int count, const size_t* src_n) {
-  auto& r = c_->residuals;
-  r.slab = nullptr;
-  r.slab_points = 0;
-  if (!r.enabled) return B200REG_OK;
+  c_->residual_slab = nullptr;
+  c_->residual_slab_points = 0;
+  if (!c_->capture.residuals) return B200REG_OK;
   size_t points = 0;
   for (int i = 0; i < count; i++) points += src_n[i];
   void* p = nullptr;
   const cudaError_t e = scratch_.alloc(&p, 8 * points);
   if (e != cudaSuccess)
     return fail(B200REG_ECUDA, "residuals: cannot allocate " + std::to_string(8 * points) + " bytes: " + cudaGetErrorString(e));
-  r.slab = (int32_t*)p;
-  r.slab_points = points;
+  c_->residual_slab = (int32_t*)p;
+  c_->residual_slab_points = points;
   return B200REG_OK;
 }
 }  // namespace b200
@@ -241,33 +170,9 @@ static int tap_begin(b200reg_ctx* c, const b200reg_cloud* src, const b200reg_clo
 
 extern "C" {
 
-int b200reg_ctx_set_lm_trace(b200reg_ctx* c, int enable) {
-  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
-  c->lm_trace.enabled = enable != 0;
-  return B200REG_OK;
-}
-
-int b200reg_lm_trace(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out) {
-  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
-  return lm_trace_copy(&c->lm_trace, offsets_out, capacity, trials_out,
-                       "no LM trace: the context's last LM solve was not traced (b200reg_ctx_set_lm_trace)");
-}
-
-int b200reg_ctx_set_residuals(b200reg_ctx* c, int enable) {
-  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
-  c->residuals.enabled = enable != 0;
-  return B200REG_OK;
-}
-
-int b200reg_residuals(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out) {
-  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
-  return residuals_copy(&c->residuals, offsets_out, capacity, nn_out, d2_out,
-                        "no residuals: the context's last registration did not record them, or failed (b200reg_ctx_set_residuals)");
-}
-
 int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* tgt,
                        const double* guess16, const b200reg_gicp_params* params, b200reg_result* out) {
-  if (c) c->residuals.valid = false;  // only a call that records and succeeds holds residuals
+  Recording rec(c, REC_TRACE | REC_RESIDUALS);
   if (!c || count <= 0 || !src || !tgt || !params || !out) return fail(B200REG_EINVAL, "bad argument");
   CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
@@ -290,15 +195,14 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
       return rc;
   }
   // residual rows: those the enclosing call reserved (ResidualSlab), else this call's own, before the solve
-  auto& rs = c->residuals;
   std::vector<int64_t> res_offsets;
   ResidualOut res_out{nullptr, nullptr};
-  if (rs.enabled) {
+  if (c->capture.residuals) {
     res_offsets.assign(count + 1, 0);
     for (int i = 0; i < count; i++) res_offsets[i + 1] = res_offsets[i] + src[i]->dev.n;
     const size_t total = (size_t)res_offsets[count];
-    int32_t* slab = rs.slab;
-    if (!slab || rs.slab_points < total) {
+    int32_t* slab = c->residual_slab;
+    if (!slab || c->residual_slab_points < total) {
       const cudaError_t e = scratch.alloc((void**)&slab, 8 * total);
       if (e != cudaSuccess)
         return fail(B200REG_ECUDA, "residuals: cannot allocate " + std::to_string(8 * total) + " bytes: " + cudaGetErrorString(e));
@@ -322,9 +226,7 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
   hc.max_steps = std::max(params->max_iterations, 0) * (1 + std::max(params->lm_max_iterations, 1)) + 2;
   hc.cond_handle = A.graph.cond_handle;
   hc.prm = prm;
-  auto& tr = c->lm_trace;
-  tr.valid = false;
-  if (tr.enabled) {
+  if (c->capture.lm_trace) {
     // every outer iteration makes at most lm_max_iterations trials (none when that is <= 0): the buffer holds any solve's records
     hc.trace_stride = (long long)std::max(params->max_iterations, 0) * std::max(params->lm_max_iterations, 1);
     const size_t bytes = sizeof(b200reg_lm_trial) * (size_t)hc.trace_stride * count;
@@ -364,25 +266,25 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
   CU(cudaStreamSynchronize(s));
   if (!no_graph) c->launches += 1 + 3 * (int64_t)hsched.steps;  // init + (search, accumulate, control) per executed step, counted by the device
   if (A.h_call->overrun) return fail(B200REG_ESTATE, "LM state machine did not terminate");
-  if (tr.enabled) {  // pair i's records are the first n_err of its region: one strided copy of the longest, then compacted
+  if (c->capture.lm_trace) {  // pair i's records are the first n_err of its region: one strided copy of the longest, then compacted
+    CsrRecord& tr = c->records.rec[Records::TRACE];
     int widest = 0;
     tr.offsets.assign(count + 1, 0);
     for (int i = 0; i < count; i++) {
       tr.offsets[i + 1] = tr.offsets[i] + states[i].n_err;
       widest = std::max(widest, states[i].n_err);
     }
-    std::vector<b200reg_lm_trial> rows((size_t)count * widest);
     const size_t rec = sizeof(b200reg_lm_trial);
+    std::vector<char> rows(rec * count * widest);
     if (widest > 0) {
       CU(cudaMemcpy2DAsync(rows.data(), rec * widest, hc.trace, rec * hc.trace_stride, rec * widest, count, cudaMemcpyDeviceToHost, s));
       CU(cudaStreamSynchronize(s));
     }
-    tr.trials.resize(tr.offsets[count]);
+    tr.rows.resize(rec * tr.offsets[count]);
     for (int i = 0; i < count; i++)
-      std::copy(rows.begin() + (size_t)i * widest, rows.begin() + (size_t)i * widest + states[i].n_err, tr.trials.begin() + tr.offsets[i]);
-    tr.valid = true;
+      if (states[i].n_err > 0) memcpy(&tr.rows[rec * tr.offsets[i]], &rows[rec * i * widest], rec * states[i].n_err);
   }
-  if (rs.enabled) {  // the fitness pass's per-point values of every pair, in one launch and one copy per array
+  if (c->capture.residuals) {  // the fitness pass's per-point values of every pair, in one launch and one copy
     const size_t total = (size_t)res_offsets[count];
     std::vector<ResidualRow> rows;
     int max_n = 0;
@@ -391,8 +293,8 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
       rows.push_back(ResidualRow{pairs[i].src.pts, pairs[i].tgt.pts, pairs[i].corr, pairs[i].sqd, pairs[i].src.n, res_offsets[i]});
       max_n = std::max(max_n, pairs[i].src.n);
     }
-    rs.nn.resize(total);
-    rs.d2.resize(total);
+    CsrRecord& rs = c->records.rec[Records::RESIDUALS];
+    rs.rows.resize(8 * total);  // nn block, then d2 block, as in the slab
     if (!rows.empty()) {
       ResidualRow* d_rows = nullptr;
       CU(scratch.upload(&d_rows, rows.data(), sizeof(ResidualRow) * rows.size()));
@@ -403,12 +305,10 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
         c->prof_bytes[CLS_MISC] += 48.0 * total;  // 16 source + 8 corr / sqd + 16 target in, 8 out
       }
       CU(cudaGetLastError());
-      CU(cudaMemcpyAsync(rs.nn.data(), res_out.nn, total * 4, cudaMemcpyDeviceToHost, s));
-      CU(cudaMemcpyAsync(rs.d2.data(), res_out.d2, total * 4, cudaMemcpyDeviceToHost, s));
+      CU(cudaMemcpyAsync(rs.rows.data(), res_out.nn, total * 8, cudaMemcpyDeviceToHost, s));
       CU(cudaStreamSynchronize(s));
     }
     rs.offsets.swap(res_offsets);
-    rs.valid = true;
   }
   for (int i = 0; i < count; i++) {
     const PairState& st = states[i];
@@ -441,20 +341,18 @@ int b200reg_gicp_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b20
       c->prof_bytes[CLS_STEP] += (136.0 * st.n_lin + 132.0 * st.n_err + 16.0) * N;
     }
   }
-  return B200REG_OK;
+  return rec.commit(B200REG_OK, count);
 }
 
 // the solve of icpAlignment over built clouds, with its loop clouds: FINAL is align()'s output cloud of every pair
 static int icp_solve(b200reg_ctx* c, LoopCapture& cap, int count, b200reg_cloud* const* sc, b200reg_cloud* const* tc,
                      const b200reg_gicp_params* params, b200reg_result* out) {
-  int rc = cap.clouds({}, sc, tc, false, false);
+  int rc = cap.clouds(count, sc, tc, false, false);
   if (!rc) rc = b200reg_gicp_align(c, count, sc, tc, nullptr, params, out);
   if (rc || !cap.on()) return rc;
   std::vector<float> fine_tf(16 * (size_t)count);
   for (int i = 0; i < count; i++) memcpy(&fine_tf[16 * (size_t)i], out[i].Tf, sizeof(out[i].Tf));
-  rc = cap.finish(nullptr, fine_tf.data());
-  if (rc) c->residuals.valid = false;
-  return rc;
+  return cap.finish(nullptr, fine_tf.data());
 }
 
 // one chunk of pairs, raw records already on the device
@@ -472,17 +370,18 @@ static int icp_alignment_device(b200reg_ctx* c, LoopCapture& cap, int count, con
 int b200reg_icp_alignment(b200reg_ctx* c, int count, const float* const* src_xyz, const size_t* src_n,
                           const float* const* tgt_xyz, const size_t* tgt_n, size_t stride_bytes, int on_device,
                           const b200reg_gicp_params* params, b200reg_result* out) {
-  if (c) c->residuals.valid = false;  // its solve records them; a refused or failed call holds none
+  Recording rec(c, REC_TRACE | REC_RESIDUALS | REC_CLOUDS);
   if (!c || count <= 0 || !src_xyz || !src_n || !tgt_xyz || !tgt_n || !params || !out)
     return fail(B200REG_EINVAL, "bad argument");
   if (stride_bytes < 12 || stride_bytes % 4) return fail(B200REG_EINVAL, "stride_bytes must be a multiple of 4, >= 12");
   for (int i = 0; i < count; i++)
     if (!src_xyz[i] || !tgt_xyz[i] || src_n[i] == 0 || tgt_n[i] == 0) return fail(B200REG_EINVAL, "empty cloud");
   CU(cudaSetDevice(c->device));
-  LoopCapture cap(c, count);
+  LoopCapture cap(c);
   ResidualSlab rslab(c);
   if (const int rc = rslab.reserve(count, src_n)) return rc;
-  if (on_device) return icp_alignment_device(c, cap, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, params, out);
+  if (on_device)
+    return rec.commit(icp_alignment_device(c, cap, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, params, out), count);
   // Host buffers: all uploads are queued on the copy stream up front, chunk by chunk; the compute stream processes
   // chunk k as soon as its records have landed, so the PCIe time of chunk k+1 hides behind the kernels of chunk k.
   cudaStream_t s = c->stream;
@@ -541,7 +440,7 @@ int b200reg_icp_alignment(b200reg_ctx* c, int count, const float* const* src_xyz
     if (!rc) rc = b200reg_clouds_covariances_ex(c, 2 * m, &bag.cl[bag.cl.size() - 2 * m], params->k_correspondences, params->regularization);
   }
   if (!rc) rc = icp_solve(c, cap, count, sc.data(), tc.data(), params, out);
-  return rc;  // clouds, events and the copy stream are released / drained by the scope guards
+  return rec.commit(rc, count);  // clouds, events and the copy stream are released / drained by the scope guards
 }
 
 int b200reg_linearize(b200reg_ctx* c, const b200reg_cloud* src, const b200reg_cloud* tgt, const double* T16,

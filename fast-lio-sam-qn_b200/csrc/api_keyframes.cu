@@ -74,8 +74,9 @@ static int assemble_clouds(b200reg_ctx* c, const KfState& kf, int count, const i
                            b200reg_cloud** dst_out);
 static int fetch_closest(b200reg_ctx* c, const KfState& kf, int count, const int32_t* query_idx, double radius, double tdiff,
                          int32_t* closest_out);
-static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
-                                const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out);
+static int perform_loop_closure(b200reg_ctx* c, Recording& rec, const KfState& kf, int count, const int32_t* query_idx,
+                                const int32_t* closest_idx, const b200reg_loop_config* cfg, b200reg_result* out,
+                                b200reg_quatro_info* quatro_out);
 
 // the configuration ranges sub-map assembly refuses (nullptr: none), for the call itself and for a job's submit
 static const char* assembly_config_error(const b200reg_loop_config* cfg) {
@@ -476,19 +477,19 @@ extern "C" {
 
 int b200reg_perform_loop_closure(b200reg_ctx* c, b200reg_keyframes* kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
                                  const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out) {
-  if (c) c->quatro_matches.valid = c->residuals.valid = false;  // a refused call holds no matches or residuals either
+  Recording rec(c, REC_ALL);
   if (!c || !kf || count <= 0 || !query_idx || !closest_idx || !cfg || !out) return fail(B200REG_EINVAL, "bad argument");
-  return perform_loop_closure(c, kf->st, count, query_idx, closest_idx, cfg, out, quatro_out);
+  return perform_loop_closure(c, rec, kf->st, count, query_idx, closest_idx, cfg, out, quatro_out);
 }
 
 }  // extern "C"
 
-// b200reg_perform_loop_closure on a view of the store: the live one, or a batch-driver job's copy
-static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, const int32_t* query_idx, const int32_t* closest_idx,
-                                const b200reg_loop_config* cfg, b200reg_result* out, b200reg_quatro_info* quatro_out) {
-  LoopCapture cap(c, count);
-  c->quatro_matches.valid = false;  // its Quatro stage records them for its subset; renumbered below, dropped on failure
-  c->residuals.valid = false;       // and its fine stage the residuals
+// b200reg_perform_loop_closure on a view of the store: the live one, or a batch-driver job's copy.  Its stages run on the
+// queries with a candidate, where[k] for stage pair k, and `rec` stores their records renumbered to all queries.
+static int perform_loop_closure(b200reg_ctx* c, Recording& rec, const KfState& kf, int count, const int32_t* query_idx,
+                                const int32_t* closest_idx, const b200reg_loop_config* cfg, b200reg_result* out,
+                                b200reg_quatro_info* quatro_out) {
+  LoopCapture cap(c);
   std::vector<int32_t> qs, cs;
   std::vector<int> where;
   for (int i = 0; i < count; i++) {
@@ -500,14 +501,7 @@ static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, co
       where.push_back(i);
     }
   }
-  if (qs.empty()) {
-    lm_trace_remap(c, count, where);
-    quatro_matches_remap(c, count, where);
-    residuals_remap(c, count, where);
-    const int rc = cap.finish(nullptr, nullptr);
-    if (rc) c->quatro_matches.valid = c->residuals.valid = false;
-    return rc;
-  }
+  if (qs.empty()) return rec.commit(B200REG_OK, count, where);  // no stage runs: every row is empty
   const int m = (int)qs.size();
   // at the time query q was the latest keyframe the vector held q + 1 keyframes (fast_lio_sam_qn.cpp:205-219); a batch
   // replays several ticks, so every pair carries the size its own tick saw (the sub-map bounds of loop_closure.cpp:72,79,100)
@@ -519,7 +513,7 @@ static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, co
   CloudBag bag(c);
   bag.cl = sc;
   bag.cl.insert(bag.cl.end(), dc.begin(), dc.end());
-  if ((rc = cap.clouds(where, sc.data(), dc.data(), true, cfg->enable_quatro != 0))) return rc;
+  if ((rc = cap.clouds(m, sc.data(), dc.data(), true, cfg->enable_quatro != 0))) return rc;
   ResidualSlab rslab(c);
   {
     std::vector<size_t> sn(m);  // the fine stage's source clouds have the sizes of the assembled sources
@@ -539,12 +533,8 @@ static int perform_loop_closure(b200reg_ctx* c, const KfState& kf, int count, co
     out[where[k]] = res[k];
     if (quatro_out && cfg->enable_quatro) quatro_out[where[k]] = qi[k];
   }
-  if (!rc) lm_trace_remap(c, count, where);
-  if (!rc) quatro_matches_remap(c, count, cfg->enable_quatro ? where : std::vector<int>());
-  if (!rc) residuals_remap(c, count, where);
   if (!rc) rc = cap.finish(cfg->enable_quatro ? qi.data() : nullptr, fine_tf.data());
-  if (rc) c->quatro_matches.valid = c->residuals.valid = false;
-  return rc;
+  return rec.commit(rc, count, where);
 }
 
 // ---- b200reg_perform_loop_closure as a job of the batch driver (batch.cu) ------------------------------------------
@@ -585,6 +575,7 @@ int kf_job_create(b200reg_keyframes* kf, int device, int count, const int32_t* q
 }
 
 int kf_job_run(b200reg_ctx* c, KfJob* j, b200reg_result* out, b200reg_quatro_info* quatro_out) {
+  Recording rec(c, REC_ALL);
   CU(cudaSetDevice(c->device));
   if (j->ingest) CU(cudaStreamWaitEvent(c->stream, j->ingest->ev, 0));  // the adds' uploads land before any read
   const int count = (int)j->query.size();
@@ -594,7 +585,7 @@ int kf_job_run(b200reg_ctx* c, KfJob* j, b200reg_result* out, b200reg_quatro_inf
     rc = fetch_closest(c, j->st, count, j->query.data(), j->cfg.loop_detection_radius, j->cfg.loop_detection_timediff_threshold,
                        j->closest.data());
   }
-  if (!rc) rc = perform_loop_closure(c, j->st, count, j->query.data(), j->closest.data(), &j->cfg, out, quatro_out);
+  if (!rc) rc = perform_loop_closure(c, rec, j->st, count, j->query.data(), j->closest.data(), &j->cfg, out, quatro_out);
   // a failed call may return with its kernels still queued: none may read a keyframe once the job counts as finished
   const cudaError_t e = cudaStreamSynchronize(c->stream);
   if (!rc && e != cudaSuccess) rc = fail(B200REG_ECUDA, std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e));

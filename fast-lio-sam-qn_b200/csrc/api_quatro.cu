@@ -88,8 +88,9 @@ int coarse_to_fine_on_clouds(b200reg_ctx* c, int count, b200reg_cloud* const* sr
       out[i] = r;
     }
   }
-  lm_trace_remap(c, count, vidx);
-  residuals_remap(c, count, vidx);
+  // the fine stage ran on the pairs vidx: its records, renumbered to these pairs
+  c->records.rec[Records::TRACE].remap(count, vidx);
+  c->records.rec[Records::RESIDUALS].remap(count, vidx);
   return B200REG_OK;
 }
 
@@ -413,8 +414,8 @@ static int record_begin(QuatroCall& qc, int count) {
   return B200REG_OK;
 }
 
-// A recording call, once every pair is solved: every match row into the slab in one launch, one copy to the host, and
-// the context's record replaced
+// A recording call, once every pair is solved: every match row into the slab in one launch and one copy into the
+// context's record
 static int record_finish(QuatroCall& qc, int count) {
   b200reg_ctx* c = qc.c;
   const int64_t total = qc.rec_offsets[count];
@@ -444,8 +445,8 @@ static int record_finish(QuatroCall& qc, int count) {
     rows.push_back(r);
     max_n = std::max(max_n, n);
   }
-  auto& qm = c->quatro_matches;
-  qm.words.resize((size_t)total * 9);
+  CsrRecord& qm = c->records.rec[Records::MATCHES];
+  qm.rows.resize((size_t)total * 36);
   if (!rows.empty()) {
     MatchCaptureRow* d_rows = nullptr;
     CU(qc.scratch.upload(&d_rows, rows.data(), sizeof(MatchCaptureRow) * rows.size()));
@@ -456,11 +457,10 @@ static int record_finish(QuatroCall& qc, int count) {
       c->prof_bytes[CLS_MISC] += 76.0 * total;  // 8 corr + 32 points + ~4 clique in, 36 out
     }
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(qm.words.data(), qc.rec_slab, qm.words.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(qm.rows.data(), qc.rec_slab, qm.rows.size(), cudaMemcpyDeviceToHost, c->stream));
   }
   CU(cudaStreamSynchronize(c->stream));
   qm.offsets = qc.rec_offsets;
-  qm.valid = true;
   return B200REG_OK;
 }
 
@@ -470,7 +470,6 @@ static int record_finish(QuatroCall& qc, int count) {
 // most max_corres + 3 <= BIGC: k_teaser_solve solves the sets of at most MAXC in that pass, and solve_opt_big the rest.
 static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst, const b200reg_quatro_params* prm,
                       b200reg_quatro_info* out, int32_t* corr_fixed, int64_t* offsets_out, size_t capacity, int32_t* corr_csr) {
-  if (c) c->quatro_matches.valid = false;  // only a call that records and succeeds holds matches
   if (!c || count <= 0 || !src || !dst || !prm || !out) return fail(B200REG_EINVAL, "bad argument");
   if (prm->estimate_scale) return fail(B200REG_EINVAL, "estimate_scale is not supported (the deployment sets it false)");
   const bool advanced = !prm->use_optimized_matching;  // Matcher::advancedMatching (matcher.cc:118-356)
@@ -489,7 +488,7 @@ static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* sr
     }
     if ((rc = b200reg_clouds_fpfh(c, (int)all.size(), all.data(), prm->fpfh_normal_radius, prm->fpfh_radius))) return rc;
   }
-  QuatroCall qc{c, scratch, quatro_params_dev(prm, advanced), out, {}, {}, c->quatro_matches.enabled, {}, {}};
+  QuatroCall qc{c, scratch, quatro_params_dev(prm, advanced), out, {}, {}, c->capture.quatro_matches, {}, {}};
   if ((rc = match_and_solve_first(qc, count, src, dst, corr_stride, corr_fixed))) return rc;
   std::vector<int> big, wide;
   for (int i = 0; i < count; i++) {
@@ -534,53 +533,6 @@ static int quatro_align_impl(b200reg_ctx* c, int count, b200reg_cloud* const* sr
   return qc.record ? record_finish(qc, count) : B200REG_OK;
 }
 
-void quatro_matches_remap(b200reg_ctx* c, int count, const std::vector<int>& where) {
-  auto& qm = c->quatro_matches;
-  if (!qm.enabled) {
-    qm.valid = false;
-    return;
-  }
-  const size_t total = where.empty() ? 0 : (size_t)qm.offsets.back();
-  std::vector<int> solved(count, -1);  // caller pair -> Quatro pair
-  for (size_t k = 0; k < where.size(); k++) solved[where[k]] = (int)k;
-  std::vector<int64_t> offsets(count + 1, 0);
-  for (int i = 0; i < count; i++) offsets[i + 1] = offsets[i] + (solved[i] >= 0 ? qm.offsets[solved[i] + 1] - qm.offsets[solved[i]] : 0);
-  // each of the four blocks keeps its words per match; rows move from Quatro order to caller order within it
-  static const int kWords[4] = {2, 1, 3, 3};
-  std::vector<int32_t> words(9 * (size_t)offsets[count]);
-  size_t from = 0, to = 0;
-  for (int b = 0; b < 4; b++) {
-    const int w = kWords[b];
-    for (int i = 0; i < count; i++) {
-      const int k = solved[i];
-      if (k < 0) continue;
-      std::copy(qm.words.begin() + from + w * qm.offsets[k], qm.words.begin() + from + w * qm.offsets[k + 1],
-                words.begin() + to + w * offsets[i]);
-    }
-    from += w * total;
-    to += w * (size_t)offsets[count];
-  }
-  qm.offsets.swap(offsets);
-  qm.words.swap(words);
-  qm.valid = true;
-}
-
-int quatro_matches_copy(const b200reg_ctx::QuatroMatches* qm, int64_t* offsets_out, size_t capacity, int32_t* corr_out,
-                        int32_t* inlier_out, float* src_xyz_out, float* dst_xyz_out, const std::string& none) {
-  if (!qm || !qm->valid) return fail(B200REG_ESTATE, none);
-  const int pairs = (int)qm->offsets.size() - 1;
-  if (!offsets_out) return pairs;
-  memcpy(offsets_out, qm->offsets.data(), sizeof(int64_t) * qm->offsets.size());
-  const size_t total = (size_t)qm->offsets.back();
-  if (total > capacity)
-    return fail(B200REG_ESTATE, "Quatro matches number " + std::to_string(total) + ", capacity " + std::to_string(capacity));
-  const int32_t* w = qm->words.data();
-  if (corr_out && total) memcpy(corr_out, w, total * 8);
-  if (inlier_out && total) memcpy(inlier_out, w + 2 * total, total * 4);
-  if (src_xyz_out && total) memcpy(src_xyz_out, w + 3 * total, total * 12);
-  if (dst_xyz_out && total) memcpy(dst_xyz_out, w + 6 * total, total * 12);
-  return B200REG_OK;
-}
 }  // namespace b200
 
 extern "C" {
@@ -684,14 +636,16 @@ int b200reg_get_fpfh(b200reg_ctx* c, const b200reg_cloud* cl, float* normals_out
 
 int b200reg_quatro_align(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst,
                          const b200reg_quatro_params* prm, b200reg_quatro_info* out, int32_t* corr_out) {
-  return quatro_align_impl(c, count, src, dst, prm, out, corr_out, nullptr, 0, nullptr);
+  Recording rec(c, REC_MATCHES);
+  return rec.commit(quatro_align_impl(c, count, src, dst, prm, out, corr_out, nullptr, 0, nullptr), count);
 }
 
 int b200reg_quatro_align_ex(b200reg_ctx* c, int count, b200reg_cloud* const* src, b200reg_cloud* const* dst,
                             const b200reg_quatro_params* prm, b200reg_quatro_info* out, int64_t* offsets_out, size_t capacity,
                             int32_t* corr_out) {
+  Recording rec(c, REC_MATCHES);
   if (!offsets_out) return fail(B200REG_EINVAL, "bad argument");
-  return quatro_align_impl(c, count, src, dst, prm, out, nullptr, offsets_out, capacity, corr_out);
+  return rec.commit(quatro_align_impl(c, count, src, dst, prm, out, nullptr, offsets_out, capacity, corr_out), count);
 }
 
 int b200reg_quatro_solve_tap(b200reg_ctx* c, int n, const float* src_xyz, const float* dst_xyz, int wide,
@@ -860,39 +814,23 @@ int b200reg_match_tap(b200reg_ctx* c, int count, const float* const* fi, const i
 int b200reg_loop_closure(b200reg_ctx* c, int count, const float* const* src_xyz, const size_t* src_n, const float* const* tgt_xyz,
                          const size_t* tgt_n, size_t stride_bytes, int on_device, const b200reg_quatro_params* qp,
                          const b200reg_gicp_params* gp, b200reg_result* out, b200reg_quatro_info* quatro_out) {
-  if (c) c->quatro_matches.valid = false;  // its Quatro stage records them, and a later failure drops them again
-  if (c) c->residuals.valid = false;       // so does its fine stage with the residuals
+  Recording rec(c, REC_ALL);
   if (!c || count <= 0 || !src_xyz || !src_n || !tgt_xyz || !tgt_n || !qp || !gp || !out) return fail(B200REG_EINVAL, "bad argument");
   CU(cudaSetDevice(c->device));
-  LoopCapture cap(c, count);
+  LoopCapture cap(c);
   ResidualSlab rslab(c);
   int rc = rslab.reserve(count, src_n);  // the fine stage's source clouds have the sizes of the sources
   if (rc) return rc;
   CloudBag bag(c);
   std::vector<b200reg_cloud*> sc(count), tc(count);
   rc = create_pair_clouds(c, count, src_xyz, src_n, tgt_xyz, tgt_n, stride_bytes, on_device, cap.on(), bag, sc.data(), tc.data());
-  if (!rc) rc = cap.clouds({}, sc.data(), tc.data(), false, true);
+  if (!rc) rc = cap.clouds(count, sc.data(), tc.data(), false, true);
   std::vector<b200reg_quatro_info> own(quatro_out ? 0 : count);  // the capture reads the coarse stage's infos
   b200reg_quatro_info* qi = quatro_out ? quatro_out : own.data();
   std::vector<float> fine_tf(cap.on() ? 16 * (size_t)count : 0);
   if (!rc) rc = coarse_to_fine_on_clouds(c, count, sc.data(), tc.data(), qp, gp, out, qi, cap.on() ? fine_tf.data() : nullptr);
   if (!rc) rc = cap.finish(qi, fine_tf.data());
-  if (rc) c->quatro_matches.valid = c->residuals.valid = false;
-  return rc;
-}
-
-int b200reg_ctx_set_quatro_matches(b200reg_ctx* c, int enable) {
-  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
-  c->quatro_matches.enabled = enable != 0;
-  return B200REG_OK;
-}
-
-int b200reg_quatro_matches(b200reg_ctx* c, int64_t* offsets_out, size_t capacity, int32_t* corr_out, int32_t* inlier_out,
-                           float* src_xyz_out, float* dst_xyz_out) {
-  if (!c) return fail(B200REG_EINVAL, "ctx is NULL");
-  return quatro_matches_copy(&c->quatro_matches, offsets_out, capacity, corr_out, inlier_out, src_xyz_out, dst_xyz_out,
-                             "no Quatro matches: the context's last call with a Quatro stage did not record them, or failed "
-                             "(b200reg_ctx_set_quatro_matches)");
+  return rec.commit(rc, count);
 }
 
 }  // extern "C"

@@ -2,9 +2,9 @@
 // own host thread with its own CUDA streams and memory pool, take alternate jobs.  While one context waits for a PCIe
 // upload or polls its LM loop, the kernels of the others keep the SMs busy -- the batch-level concurrency SURVEY.md §8(d)
 // names as the lever for the HBM fraction.  Host code only; everything it calls is the public C ABI, except the jobs over
-// the keyframe store, which go through the job interface of api_keyframes.cu (api.cuh), and the loop clouds, LM trace,
-// Quatro matches and residuals of a capturing job, which it moves out of the worker's context and reads with the context
-// getters' copy-out (api.cuh).
+// the keyframe store, which go through the job interface of api_keyframes.cu (api.cuh), and the records of a capturing
+// job (loop clouds, LM trace, Quatro matches, residuals), which it moves out of the worker's context and reads with the
+// context getters' copy-out (api.cuh).
 //
 // Reference context: the reference registers ONE pair per 2 Hz timer tick, serially, on one thread
 // (fast_lio_sam_qn/src/fast_lio_sam_qn.cpp:203-219, LoopClosure is not re-entrant, :81).
@@ -24,26 +24,6 @@
 
 namespace {
 
-// A job's loop clouds, LM trace, Quatro matches and residuals, moved out of its worker's context when the job ends: they
-// outlive the wait, until b200reg_batch_release or b200reg_batch_destroy
-struct Captured {
-  b200reg_ctx::LoopClouds clouds;
-  b200reg_ctx::LmTrace trace;
-  b200reg_ctx::QuatroMatches matches;
-  b200reg_ctx::Residuals residuals;
-};
-
-struct Capture {  // the capture settings of a job
-  int cloud_mask = 0;
-  bool lm_trace = false;
-  bool quatro_matches = false;
-  bool residuals = false;
-  bool on() const { return cloud_mask || lm_trace || quatro_matches || residuals; }
-  bool operator!=(const Capture& o) const {
-    return cloud_mask != o.cloud_mask || lm_trace != o.lm_trace || quatro_matches != o.quatro_matches || residuals != o.residuals;
-  }
-};
-
 struct Job {
   int kind = 0;  // 0 icpAlignment, 1 coarseToFineAlignment, 2 performLoopClosure over a keyframe store
   int count = 0;
@@ -57,9 +37,10 @@ struct Job {
   b200reg_result* out = nullptr;
   b200reg_quatro_info* qout = nullptr;
   // the driver's capture settings at submit (b200reg_batch_set_loop_clouds / _set_lm_trace / _set_quatro_matches /
-  // _set_residuals), and what the job captured
+  // _set_residuals), and the records the job left, moved out of its worker's context when it ended: they outlive the wait,
+  // until b200reg_batch_release or b200reg_batch_destroy
   Capture capture;
-  std::shared_ptr<Captured> captured;
+  std::shared_ptr<Records> captured;
   // completion
   int status = 0;
   std::string error;
@@ -90,7 +71,7 @@ struct b200reg_batch {
   // that never captures keeps none); the outputs of the waited-for jobs that captured (null: the job failed), until released
   Capture capture;
   std::map<int64_t, Capture> capture_from;
-  std::map<int64_t, std::shared_ptr<Captured>> kept;
+  std::map<int64_t, std::shared_ptr<Records>> kept;
 };
 
 static thread_local std::string g_batch_err;
@@ -106,13 +87,7 @@ static void run_worker(b200reg_batch* b, Worker* w) {
       w->q.pop_front();
     }
     b200reg_ctx* c = w->ctx;
-    const bool capture = j->capture.on();
-    if (capture) {  // for this job only
-      c->loop_clouds.mask = j->capture.cloud_mask;
-      c->lm_trace.enabled = j->capture.lm_trace;
-      c->quatro_matches.enabled = j->capture.quatro_matches;
-      c->residuals.enabled = j->capture.residuals;
-    }
+    c->capture = j->capture;  // for this job only
     int rc;
     if (j->kind == 0)
       rc = b200reg_icp_alignment(c, j->count, j->src.data(), j->src_n.data(), j->tgt.data(), j->tgt_n.data(), j->stride, j->on_device,
@@ -123,18 +98,10 @@ static void run_worker(b200reg_batch* b, Worker* w) {
     else
       rc = kf_job_run(c, j->kfjob.get(), j->out, j->qout);
     j->kfjob.reset();  // the store no longer counts the job as in flight: a wait that returns sees it finished
-    if (capture) {  // the job takes the stored outputs without a copy; nothing carries over to the worker's next job
-      if (!rc) {
-        j->captured = std::make_shared<Captured>();
-        std::swap(j->captured->clouds, c->loop_clouds);
-        std::swap(j->captured->trace, c->lm_trace);
-        std::swap(j->captured->matches, c->quatro_matches);
-        std::swap(j->captured->residuals, c->residuals);
-      }
-      c->loop_clouds = b200reg_ctx::LoopClouds();
-      c->lm_trace = b200reg_ctx::LmTrace();
-      c->quatro_matches = b200reg_ctx::QuatroMatches();
-      c->residuals = b200reg_ctx::Residuals();
+    if (j->capture.on()) {  // the job takes the stored records without a copy; nothing carries over to the worker's next job
+      auto rec = std::make_shared<Records>();
+      std::swap(*rec, c->records);
+      if (!rc) j->captured = std::move(rec);
     }
     {
       std::lock_guard<std::mutex> lk(b->mu);
@@ -317,76 +284,73 @@ int b200reg_batch_set_residuals(b200reg_batch* b, int enable) {
 
 }  // extern "C"
 
-// The outputs the getters read for `ticket` (the pointer keeps them alive while they are copied out, outside the lock), or
-// null; `none` is the getters' message when the output is missing, saying why.  kind: a B200REG_CLOUD_* bit, 0 for the LM
-// trace, MATCHES for the Quatro matches, RESIDUALS for the residuals.  B200REG_EINVAL for a ticket never handed out.
-constexpr int MATCHES = -1, RESIDUALS = -2;
-static int find_captured(b200reg_batch* b, int64_t ticket, int kind, std::shared_ptr<Captured>* out, std::string* none) {
-  const char* what = kind > 0 ? "no such loop clouds: " : kind == 0 ? "no LM trace: " : kind == MATCHES ? "no Quatro matches: " : "no residuals: ";
-  const std::string missing = what + std::string("batch job ") + std::to_string(ticket);
-  const std::string off = kind > 0         ? " did not capture this kind (b200reg_batch_set_loop_clouds at its submit)"
-                          : kind == 0       ? " was not traced (b200reg_batch_set_lm_trace at its submit)"
-                          : kind == MATCHES ? " did not record them (b200reg_batch_set_quatro_matches at its submit, or a job "
-                                              "without a Quatro stage)"
-                                            : " did not record them (b200reg_batch_set_residuals at its submit)";
-  std::lock_guard<std::mutex> lk(b->mu);
-  if (ticket < 0 || ticket >= b->next_ticket) return fail(B200REG_EINVAL, "ticket " + std::to_string(ticket) + " was never handed out");
-  if (b->jobs.count(ticket)) {
-    *none = missing + " has not been waited for yet (b200reg_batch_wait)";
-    return B200REG_OK;
+// What the getters say of a job without record r: the start of the message, and the end for a job that did not record it
+// because of its settings at submit
+struct RecordText {
+  const char* missing;
+  const char* off;
+};
+static const RecordText kRecordText[Records::N] = {
+    {"no LM trace: ", " was not traced (b200reg_batch_set_lm_trace at its submit)"},
+    {"no residuals: ", " did not record them (b200reg_batch_set_residuals at its submit)"},
+    {"no Quatro matches: ", " did not record them (b200reg_batch_set_quatro_matches at its submit, or a job without a Quatro stage)"},
+    {"no such loop clouds: ", " did not capture this kind (b200reg_batch_set_loop_clouds at its submit)"},
+    {"no such loop clouds: ", " did not capture this kind (b200reg_batch_set_loop_clouds at its submit)"},
+    {"no such loop clouds: ", " did not capture this kind (b200reg_batch_set_loop_clouds at its submit)"},
+    {"no such loop clouds: ", " did not capture this kind (b200reg_batch_set_loop_clouds at its submit)"},
+};
+
+// The getters of a job's record r: the ticket rules, then record_copy over the records the job left (the pointer keeps them
+// alive while they are copied out, outside the lock), with the message that says why record r is missing.  r < 0 (a bad
+// loop-cloud kind) is refused by record_copy, after the ticket.
+static int batch_record(b200reg_batch* b, int64_t ticket, int r, int64_t* offsets_out, size_t capacity,
+                        std::initializer_list<void*> cols) {
+  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
+  std::shared_ptr<Records> rec;
+  std::string none;
+  {
+    std::lock_guard<std::mutex> lk(b->mu);
+    if (ticket < 0 || ticket >= b->next_ticket) return fail(B200REG_EINVAL, "ticket " + std::to_string(ticket) + " was never handed out");
+    if (r >= 0) {
+      const std::string missing = kRecordText[r].missing + std::string("batch job ") + std::to_string(ticket);
+      const auto k = b->kept.find(ticket);
+      if (b->jobs.count(ticket)) {
+        none = missing + " has not been waited for yet (b200reg_batch_wait)";
+      } else if (k != b->kept.end()) {
+        rec = k->second;
+        none = missing + (rec ? kRecordText[r].off : " failed");
+      } else {
+        const auto s = b->capture_from.upper_bound(ticket);  // the settings the job copied at its submit
+        const Capture cap = s == b->capture_from.begin() ? Capture() : std::prev(s)->second;
+        none = missing + (cap.wants(r) ? " was released (b200reg_batch_release)" : kRecordText[r].off);
+      }
+    }
   }
-  const auto k = b->kept.find(ticket);
-  if (k != b->kept.end()) {
-    *out = k->second;
-    *none = missing + (k->second ? off : " failed");
-    return B200REG_OK;
-  }
-  const auto s = b->capture_from.upper_bound(ticket);  // the settings the job copied at its submit
-  const Capture cap = s == b->capture_from.begin() ? Capture() : std::prev(s)->second;
-  const bool wanted = kind > 0 ? (cap.cloud_mask & kind) != 0 : kind == 0 ? cap.lm_trace : kind == MATCHES ? cap.quatro_matches : cap.residuals;
-  *none = missing + (wanted ? " was released (b200reg_batch_release)" : off);
-  return B200REG_OK;
+  return record_copy(rec.get(), r, none, offsets_out, capacity, cols);
 }
 
 extern "C" {
 
 int b200reg_batch_loop_clouds(b200reg_batch* b, int64_t ticket, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out) {
-  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
-  std::shared_ptr<Captured> cap;
-  std::string none;
-  if (const int rc = find_captured(b, ticket, kind, &cap, &none)) return rc;
-  return loop_clouds_copy(cap ? &cap->clouds : nullptr, kind, offsets_out, capacity, xyzi_out, none);
+  return batch_record(b, ticket, cloud_record(kind), offsets_out, capacity, {xyzi_out});
 }
 
 int b200reg_batch_lm_trace(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out) {
-  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
-  std::shared_ptr<Captured> cap;
-  std::string none;
-  if (const int rc = find_captured(b, ticket, 0, &cap, &none)) return rc;
-  return lm_trace_copy(cap ? &cap->trace : nullptr, offsets_out, capacity, trials_out, none);
+  return batch_record(b, ticket, Records::TRACE, offsets_out, capacity, {trials_out});
 }
 
 int b200reg_batch_quatro_matches(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity, int32_t* corr_out,
                                  int32_t* inlier_out, float* src_xyz_out, float* dst_xyz_out) {
-  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
-  std::shared_ptr<Captured> cap;
-  std::string none;
-  if (const int rc = find_captured(b, ticket, MATCHES, &cap, &none)) return rc;
-  return quatro_matches_copy(cap ? &cap->matches : nullptr, offsets_out, capacity, corr_out, inlier_out, src_xyz_out, dst_xyz_out,
-                             none);
+  return batch_record(b, ticket, Records::MATCHES, offsets_out, capacity, {corr_out, inlier_out, src_xyz_out, dst_xyz_out});
 }
 
 int b200reg_batch_residuals(b200reg_batch* b, int64_t ticket, int64_t* offsets_out, size_t capacity, int32_t* nn_out, float* d2_out) {
-  if (!b) return fail(B200REG_EINVAL, "batch is NULL");
-  std::shared_ptr<Captured> cap;
-  std::string none;
-  if (const int rc = find_captured(b, ticket, RESIDUALS, &cap, &none)) return rc;
-  return residuals_copy(cap ? &cap->residuals : nullptr, offsets_out, capacity, nn_out, d2_out, none);
+  return batch_record(b, ticket, Records::RESIDUALS, offsets_out, capacity, {nn_out, d2_out});
 }
 
 int b200reg_batch_release(b200reg_batch* b, int64_t ticket) {
   if (!b) return fail(B200REG_EINVAL, "batch is NULL");
-  std::shared_ptr<Captured> drop;  // freed after the lock is released
+  std::shared_ptr<Records> drop;  // freed after the lock is released
   std::lock_guard<std::mutex> lk(b->mu);
   if (ticket < 0 || ticket >= b->next_ticket) return fail(B200REG_EINVAL, "ticket " + std::to_string(ticket) + " was never handed out");
   if (b->jobs.count(ticket)) return fail(B200REG_ESTATE, "batch job " + std::to_string(ticket) + " has not been waited for yet (b200reg_batch_wait)");

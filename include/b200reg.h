@@ -199,14 +199,15 @@ int b200reg_ctx_get_profile(b200reg_ctx* ctx, int family, const char** name, dou
  * b200reg_perform_loop_closure) records each trial of each pair.  The device buffer holds count x max_iterations x
  * max(lm_max_iterations, 1) records (no pair can have more, nothing is truncated) and lives for the call only; if it cannot
  * be allocated the call returns B200REG_ECUDA with the bytes in the message.  Tracing changes no result and no launch.
- * With tracing disabled nothing is recorded or allocated, and such a call discards the stored trace.                    */
+ * Each such call discards the stored trace on entry and stores its own only if it succeeds with tracing on; a refused or
+ * failed call, or one with tracing off, leaves none.  With tracing off nothing is recorded or allocated.               */
 int b200reg_ctx_set_lm_trace(b200reg_ctx* ctx, int enable);
 /* The trace of the context's most recent call that ran the LM solve, as CSR over that call's pairs (the CALLER's pair
  * indices; a pair whose fine stage did not run -- invalid Quatro, no loop candidate -- has no records): the trials of pair
  * i are trials_out[offsets_out[i] .. offsets_out[i + 1]), in execution order; offsets_out has count + 1 entries.  If the
  * records exceed `capacity` the call fills offsets_out, writes nothing else and returns B200REG_ESTATE.  offsets_out ==
- * NULL: returns that call's pair count (>= 0) and writes nothing.  Before any traced solve, or after an untraced one:
- * B200REG_ESTATE.                                                                                                       */
+ * NULL: returns that call's pair count (>= 0) and writes nothing.  Before any traced solve, and after a call that ran
+ * untraced, was refused or failed: B200REG_ESTATE.                                                                      */
 int b200reg_lm_trace(b200reg_ctx* ctx, int64_t* offsets_out, size_t capacity, b200reg_lm_trial* trials_out);
 
 /* Loop clouds: the four clouds loopTimerFunc publishes after each loop attempt (fast_lio_sam_qn.cpp:245-248), as the batched
@@ -229,18 +230,19 @@ int b200reg_lm_trace(b200reg_ctx* ctx, int64_t* offsets_out, size_t capacity, b2
 #define B200REG_CLOUD_COARSE 4
 #define B200REG_CLOUD_FINAL 8
 /* Capture the kinds in `mask` (an OR of B200REG_CLOUD_*; 0, the default, turns capture off) in the following calls of the
- * three entry points above; no other entry point touches the stored clouds.  A call with capture on replaces the stored
- * clouds, one with capture off discards them.  Capture changes no result, trace or solve.  Its device slab (16 bytes per
- * point per kind: 512 pairs x 100k points x 4 kinds is about 3.3 GB) lives for the call only and is sized before Quatro
- * for every row that can be present; if it cannot be allocated the call returns B200REG_ECUDA with the bytes in the
- * message.  With capture off nothing is allocated or launched.                                                         */
+ * three entry points above; no other entry point touches the stored clouds.  Each such call discards the stored clouds
+ * on entry and stores its own only if it succeeds with capture on; a refused or failed call, or one with capture off,
+ * leaves none.  Capture changes no result, trace or solve.  Its device slab (16 bytes per point per kind: 512 pairs x
+ * 100k points x 4 kinds is about 3.3 GB) lives for the call only and is sized before Quatro for every row that can be
+ * present; if it cannot be allocated the call returns B200REG_ECUDA with the bytes in the message.  With capture off
+ * nothing is allocated or launched.                                                                                   */
 int b200reg_ctx_set_loop_clouds(b200reg_ctx* ctx, int mask);
 /* The clouds of one kind from the context's most recent capturing call, as CSR over that call's pairs (the CALLER's pair
  * order): pair i's points are xyzi_out[4 * offsets_out[i] .. 4 * offsets_out[i + 1]), in the order above; offsets_out has
  * count + 1 entries; pairs without such a cloud (no loop candidate, invalid Quatro ...) have empty rows.  If the points
  * exceed `capacity` the call fills offsets_out, writes nothing else and returns B200REG_ESTATE.  offsets_out == NULL:
- * returns that call's pair count (>= 0) and writes nothing.  A kind that call did not capture, or no capturing call since
- * the last uncaptured one: B200REG_ESTATE.  A kind that is not one B200REG_CLOUD_* bit: B200REG_EINVAL.              */
+ * returns that call's pair count (>= 0) and writes nothing.  A kind that call did not capture, and after a call that
+ * ran uncaptured, was refused or failed: B200REG_ESTATE.  A kind that is not one B200REG_CLOUD_* bit: B200REG_EINVAL. */
 int b200reg_loop_clouds(b200reg_ctx* ctx, int kind, int64_t* offsets_out, size_t capacity, float* xyzi_out);
 
 /* ---- clouds: replaces KdTreeFLANN::setInputCloud / buildIndex

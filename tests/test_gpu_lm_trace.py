@@ -311,6 +311,23 @@ def test_abi_contract(synth):
         assert rc == ESTATE and off.tolist() == [0, len(rows[0]), total] and np.array_equal(buf, sentinel)
         rc = lib.b200reg_lm_trace(c.h, off.ctypes.data_as(C.c_void_p), C.c_size_t(total), buf.ctypes.data_as(C.c_void_p))
         assert rc == 0 and buf.tobytes() == b"".join(r.tobytes() for r in rows)
+        # a refused call and a call that fails in a stage both discard the trace
+        with pytest.raises(native.B200RegError):  # an empty source cloud
+            c.icp_alignment_ptrs([src.ctypes.data], [0], [dst.ctypes.data], [len(dst)], 16, False)
+        assert lib.b200reg_lm_trace(c.h, None, C.c_size_t(0), None) == ESTATE
+        kf = c.keyframes()
+        try:
+            kf.add(src, np.eye(4), 0.0)
+            kf.add(dst, np.eye(4), 1.0)
+            c.icp_alignment([src], [dst])
+            assert lib.b200reg_lm_trace(c.h, None, C.c_size_t(0), None) == 1
+            cfg = b200reg.default_loop_config()
+            cfg.quatro.estimate_scale = 1  # refused by the Quatro stage, after sub-map assembly
+            with pytest.raises(native.B200RegError):
+                kf.perform_loop_closure([1], [0], cfg)
+            assert lib.b200reg_lm_trace(c.h, None, C.c_size_t(0), None) == ESTATE
+        finally:
+            kf.destroy()
     finally:
         c.close()
 

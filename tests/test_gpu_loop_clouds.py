@@ -293,6 +293,26 @@ def test_abi_contract(synth, native):
         assert rc == ESTATE and off.tolist() == [0, len(rows[0]), total] and np.array_equal(buf, sentinel)
         rc = lib.b200reg_loop_clouds(c.h, FINAL, off.ctypes.data_as(C.c_void_p), C.c_size_t(total), buf.ctypes.data_as(C.c_void_p))
         assert rc == 0 and buf.tobytes() == b"".join(r.tobytes() for r in rows)
+        # a refused call and a call that fails in a stage both discard the clouds
+        src, dst = pairs[0][0], pairs[0][1]
+        kf = c.keyframes()
+        c.set_loop_clouds(FINAL)
+        try:
+            with pytest.raises(native.B200RegError):  # an empty source cloud
+                c.icp_alignment_ptrs([src.ctypes.data], [0], [dst.ctypes.data], [len(dst)], 16, False)
+            assert lib.b200reg_loop_clouds(c.h, FINAL, None, C.c_size_t(0), None) == ESTATE
+            kf.add(src, np.eye(4), 0.0)
+            kf.add(dst, np.eye(4), 1.0)
+            c.icp_alignment([src], [dst])
+            assert lib.b200reg_loop_clouds(c.h, FINAL, None, C.c_size_t(0), None) == 1
+            bad = _cfg()
+            bad.quatro.estimate_scale = 1  # refused by the Quatro stage, after sub-map assembly
+            with pytest.raises(native.B200RegError):
+                kf.perform_loop_closure([1], [0], bad)
+            assert lib.b200reg_loop_clouds(c.h, FINAL, None, C.c_size_t(0), None) == ESTATE
+        finally:
+            c.set_loop_clouds(0)
+            kf.destroy()
     finally:
         c.close()
 
